@@ -1,8 +1,9 @@
-"""bench.py — MultiMAE-B pre-training step throughput on B200 (BASELINE.json metric).
+"""bench.py — MultiMAE-B pre-training step throughput on H100 (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                      # this framework (CUDA path)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 ... bench.py --gpus 8 --steps K --warmup W
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1      # CPU arm: the oracle port on the host cores
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR   # also write the last timed step's outputs as .npy
 
 Workload (config.workload): BASELINE.json configs[1] — MultiMAE-B, rgb+depth+semseg in/out + norm_rgb decoder, 224x224,
 98 visible tokens, bs=128 per GPU, bf16 tensor-core operands / fp32 accumulate; data-parallel for N>1 (weak scaling).
@@ -41,16 +42,22 @@ WORKLOADS = {
 }
 
 
+# NVIDIA's H100 SXM data sheet (700 W): dense BF16 tensor-core peak and HBM3 bandwidth
+H100_BF16_TFLOPS = 989.0
+H100_HBM_GBS = 3350.0
+
+
 def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), d.get("hbm_gbs", 6650.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return (d.get("bf16_tflops_sustained", d.get("bf16_tflops", H100_BF16_TFLOPS)), d.get("hbm_gbs", H100_HBM_GBS),
+                "measured")
+    return H100_BF16_TFLOPS, H100_HBM_GBS, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -145,23 +152,11 @@ def _note(msg):
     print("[bench %6.1fs] %s" % (time.perf_counter() - _T0, msg), file=sys.stderr, flush=True)
 
 
-def ncu_evidence():
-    """Figures that only a profiler can give (DRAM bytes of the dominant GEMM, tensor-pipe % of the attention kernels) are
-    READ from the committed summary of the `ncu --set full` capture - profiles/ncu_hot_kernels.json, written by
-    scripts/ncu_raw_table.py --json together with the commit it was taken at - never typed into this file."""
-    path = os.path.join(ROOT, "profiles", "ncu_hot_kernels.json")
-    try:
-        with open(path) as fh:
-            return json.load(fh)
-    except Exception:  # noqa: BLE001
-        return None
-
-
 def encoder_tc_from_table(agg, rows_enc, D_enc, peak_tf):
     """BASELINE metric, second half ("encoder TC util%").  `agg`: {(M, N, K, operand-major flags, split): [launches, ms]}
     of one profiled step.  The GEMMs of the encoder blocks (QKV, proj, fc1, fc2; forward, dgrad, wgrad) are the launches
     whose three extents are the encoder row count B*(visible+1) and two of {D, 3D, 4D}; their FLOPs over their CUDA-event
-    time, against the measured and the nominal dense bf16 peak."""
+    time, against the measured (or data-sheet) and the data-sheet dense bf16 peak."""
     widths = {D_enc, 3 * D_enc, 4 * D_enc}
     fl_enc = ms_enc = 0.0
     n_enc = 0
@@ -178,12 +173,8 @@ def encoder_tc_from_table(agg, rows_enc, D_enc, peak_tf):
         return None
     tf_enc = fl_enc / (ms_enc * 1e-3) / 1e12
     out = {"encoder_gemm_tflops": round(tf_enc, 1), "launches_per_step": n_enc, "ms_per_step": round(ms_enc, 3),
-           "frac_of_measured_peak": round(tf_enc / peak_tf, 4), "frac_of_nominal_2250": round(tf_enc / 2250.0, 4)}
-    ev = ncu_evidence()
-    if ev is not None:
-        out["tensor_pipe_pct_ncu"] = {k: v.get("tensor_pct") for k, v in ev.get("kernels", {}).items()
-                                      if "attn" in k or "gemm" in k}
-        out["ncu_capture"] = {"file": "profiles/ncu_hot_kernels.json", "commit": ev.get("commit"), "when": ev.get("when")}
+           "frac_of_measured_peak": round(tf_enc / peak_tf, 4),
+           "frac_of_datasheet_peak": round(tf_enc / H100_BF16_TFLOPS, 4)}
     return out
 
 
@@ -231,7 +222,7 @@ def run_ours(args, rank, world, local_rank):
         torch.cuda.synchronize()
         if args.sm_budget:
             lib.mmae_set_sm_budget(args.sm_budget)
-    # ------------------------------------------------------------------ roofline of the dominant kernel (tcgen05 GEMM): one
+    # ------------------------------------------------------------------ roofline of the dominant kernel (wgmma GEMM): one
     # eager step with CUDA events around every GEMM launch, taken BEFORE the step is captured (a captured graph cannot be
     # profiled per launch, and eager collectives must not be mixed in behind captured ones)
     for _ in range(2):
@@ -240,7 +231,7 @@ def run_ours(args, rank, world, local_rank):
     peak_tf, peak_gbs, peak_src = peaks()
     # The profiled step runs the four task decoders one after the other on ONE stream: an event pair around a launch measures
     # that launch only when nothing else shares the SMs - with the decoders on their own streams (the timed legs below) every
-    # K=256 GEMM is charged for its neighbours' kernels (25088x256x256: 54 TF/s "measured" that way, ~3x its stand-alone rate)
+    # K=256 GEMM is charged for its neighbours' kernels
     streams_on = model.decoder_streams
     model.decoder_streams = False
     stepper._step(resident[0])
@@ -316,7 +307,7 @@ def run_ours(args, rank, world, local_rank):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(args.steps):
-        loss, _ = train_step(resident[i % 2])
+        loss, grad_norm = train_step(resident[i % 2])
     e1.record()
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
@@ -325,6 +316,8 @@ def run_ours(args, rank, world, local_rank):
         launches = launches_per_step * args.steps          # a replayed graph re-issues the captured launches
     clocks = sampler.stop() if rank == 0 else None
     final_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, grad_norm, opt)
 
     if rank == 0:
         _note("leg 1 (HBM-resident inputs): %.3f ms/step" % (ms_total / args.steps))
@@ -376,7 +369,7 @@ def run_ours(args, rank, world, local_rank):
         return max_over_ranks(e0.elapsed_time(e1))
 
     # (The replayed step issues no host -> device copy of its own: a small H2D on the compute stream would queue behind the
-    # in-flight 106 MB input copy on the H2D engine and stall the step by the ~2 ms that copy takes - measured.)
+    # in-flight 106 MB input copy on the H2D engine and stall the step until that copy is done.)
     ms_e2e, e2e_mode = e2e_leg(True), ("cuda-graph" if stepper.graph is not None else "eager")
 
     if rank == 0:
@@ -433,7 +426,7 @@ def run_ours(args, rank, world, local_rank):
         "config": {"workload": wl["name"] + (" + truncated depth standardisation" if args.standardize_depth else ""),
                    "global_batch": args.batch * world, "per_gpu_batch": args.batch,
                    "parallelism": "dp%d" % world,
-                   "l2": "two alternating input batches (212 MB) and a >9 GB per-step activation working set exceed the 126 MB L2",
+                   "l2": "two alternating input batches (212 MB) and a >9 GB per-step activation working set exceed the 50 MB L2",
                    "loss_scaling": "none (bf16)",
                    "sm_budget": args.sm_budget or None,
                    "e2e_pipeline": "H2D of step i+1 prefetched on a copy stream during step i; every step's loss read on "
@@ -442,10 +435,9 @@ def run_ours(args, rank, world, local_rank):
                 "d2h_bytes_per_step": 4, "h2d_link_gbs_measured": round(h2d_gbs, 1), "launch_mode": e2e_mode},
         "gpu_launches": int(launches),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel (tcgen05, all operand-major variants)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel (wgmma, all operand-major variants)",
                      "achieved": round(gemm_tf, 1), "peak": peak_tf, "unit": "TFLOP/s",
-                     "frac": round(gemm_tf / peak_tf, 4), "traffic": None,
-                     "traffic_note": None, "peak_source": peak_src + " (sustained bf16)",
+                     "frac": round(gemm_tf / peak_tf, 4), "peak_source": peak_src + " (dense bf16)",
                      "launches_per_step": int(n_g.value), "kernel_ms_per_step": round(ms_g.value, 3),
                      "kernel_share_of_step": round(ms_g.value / ms_step, 3),
                      "how": "CUDA events around every GEMM launch of one eager step with the task decoders serialised on one "
@@ -454,14 +446,6 @@ def run_ours(args, rank, world, local_rank):
     }
     if encoder_tc is not None:
         out["encoder_tc"] = encoder_tc
-    ev = ncu_evidence() if args.workload == "cfg2" else None
-    gemm_ev = (ev or {}).get("dominant_gemm")
-    if gemm_ev:          # dram__bytes_read + dram__bytes_write of one launch of the dominant GEMM, from the committed capture
-        out["roofline"]["traffic"] = gemm_ev.get("dram_bytes")
-        out["roofline"]["traffic_note"] = "%s: %s (ncu --set full, commit %s, profiles/ncu_hot_kernels.json)" % (
-            gemm_ev.get("what"), gemm_ev.get("note"), ev.get("commit"))
-    else:
-        out["roofline"]["traffic_note"] = "no committed ncu capture for this workload's GEMM shapes"
     if world == 1 and args.eager_baseline:
         # free this process's ~10 GB of activations / graph memory pools first: the eager oracle needs room of its own
         _note("GPU legs done (%.1f samples/s); timing torch eager (oracle port) on this GPU" % value)
@@ -474,6 +458,26 @@ def run_ours(args, rank, world, local_rank):
     _emit(out)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_PARAM_SAMPLE = 1 << 20
+
+
+def dump_outputs(directory, loss, grad_norm, opt):
+    """What the caller of the timed step holds after its last step, as float32 .npy files: the summed loss and the
+    gradient norm the step returned, and the updated fp32 parameters - a fixed, seeded sample of 2^20 entries of the flat
+    parameter buffer (4 MB) together with their indices (float64, 8 MB)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    flat = opt.flat_params.detach()
+    g = torch.Generator().manual_seed(0)
+    n = flat.numel()
+    idx = torch.randperm(n, generator=g)[:DUMP_PARAM_SAMPLE].sort().values if n > DUMP_PARAM_SAMPLE else torch.arange(n)
+    arrays = {"loss": loss.detach().float().reshape(1), "grad_norm": grad_norm.detach().float().reshape(1),
+              "params_sample": flat[idx.to(flat.device)].float()}
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), t.cpu().numpy())
+    np.save(os.path.join(directory, "params_sample_index.npy"), idx.numpy().astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -569,12 +573,12 @@ def _gpu_eager_steps(workload, dtype, steps=5, warmup=2):
     return B / (statistics.median(times) * 1e-3)
 
 
-def gpu_eager_baseline(workload="cfg2"):
+def gpu_eager_baseline(workload="cfg2", steps=5, warmup=2):
     out = {"unit": "samples/s", "what": "oracle port of the reference PyTorch path, eager on this GPU, fwd+4 losses+bwd at the "
            "workload's batch (no optimizer step), median of 5 steps after 2 warm-ups, CUDA events"}
     for name, dt in (("fp16_autocast", torch.float16), ("bf16_autocast", torch.bfloat16)):
         try:
-            out[name] = round(_gpu_eager_steps(workload, dt), 1)
+            out[name] = round(_gpu_eager_steps(workload, dt, steps=steps, warmup=warmup), 1)
         except Exception as e:  # noqa: BLE001
             out[name] = None
             out[name + "_error"] = str(e).splitlines()[0][:160] if str(e) else type(e).__name__
@@ -585,7 +589,8 @@ def gpu_eager_baseline(workload="cfg2"):
 def gpu_eager_baseline_bounded(limit_s=150, workload="cfg2"):
     """In a child process (its ~40 GB of eager activations are gone when it exits) with a hard time limit."""
     try:
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "gpu-eager", "--workload", workload],
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "gpu-eager", "--workload", workload,
+                            "--steps", "5", "--warmup", "2"],
                            capture_output=True, text=True, timeout=limit_s)
         for line in reversed(r.stdout.splitlines()):
             if line.startswith("{"):
@@ -599,7 +604,8 @@ def gpu_eager_baseline_bounded(limit_s=150, workload="cfg2"):
 def cpu_baseline_bounded(limit_s=150, workload="cfg2"):
     """The CPU sample in a child process with a hard time limit: a slow or oversubscribed host must not cost the GPU line."""
     try:
-        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "cpu-baseline", "--workload", workload],
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--impl", "cpu-baseline", "--workload", workload,
+                            "--steps", "2"],
                            capture_output=True, text=True, timeout=limit_s)
         for line in reversed(r.stdout.splitlines()):
             if line.startswith("{"):
@@ -618,21 +624,21 @@ def run_reference(args, rank, world):
     # GPU arm's; the thread count is probed at a small batch, the step count is bounded
     batch = wl["batch"] if args.workload == "cfg2" else 2
     threads = _best_thread_count(8 if args.workload == "cfg2" else 2, args.workload)
-    steps = min(args.steps, 3)
-    times = _cpu_steps(batch, steps, 1, threads=threads, workload=args.workload)
+    steps = args.steps
+    times = _cpu_steps(batch, steps, args.warmup, threads=threads, workload=args.workload)
     ms_step = statistics.mean(times) * 1e3
     value = batch / (ms_step * 1e-3)
     base = {"value": round(value, 2), "unit": "samples/s", "cores": torch.get_num_threads(), "kind": "port",
-            "sample": "%d steps (after 1 warm-up) of fwd+4 losses+bwd+grad-norm at bs=%d on the host cores, fp32, no optimizer "
-                      "update (the oracle port of the reference path; bounded step count)" % (steps, batch)}
+            "sample": "%d steps (after %d warm-up) of fwd+4 losses+bwd+grad-norm at bs=%d on the host cores, fp32, no "
+                      "optimizer update (the oracle port of the reference path)" % (steps, args.warmup, batch)}
     _emit({
         "impl": "reference", "metric": wl["metric"], "value": round(value, 2), "unit": "samples/s", "n_gpus": world,
-        "steps": steps, "warmup": 1, "ms_per_step": round(ms_step, 1), "higher_is_better": True,
+        "steps": steps, "warmup": args.warmup, "ms_per_step": round(ms_step, 1), "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": wl["name"], "global_batch": batch, "per_gpu_batch": batch,
-                   "note": "CPU arm: oracle port of the reference path (the reference is pure PyTorch and /root/reference "
-                           "does not travel to the GPU box); fp32 on the host cores, no optimizer update; with N > 1 it is "
-                           "still ONE host process - compare it with the N = 1 line only"},
+                   "note": "CPU arm: oracle port of the reference path (the reference is pure PyTorch); fp32 on the "
+                           "host cores, no optimizer update; with N > 1 it is still ONE host process - compare it with the "
+                           "N = 1 line only"},
         "cpu_baseline": base,
         "e2e": {"value": round(value, 2), "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     })
@@ -652,11 +658,14 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "cpu-baseline", "gpu-eager"])
     ap.add_argument("--graph", type=int, default=1, help="1: replay the step as one CUDA graph (data parallel: the bucketed NCCL "
                          "all-reduces are captured in it); 0: eager launches")
-    ap.add_argument("--sm-budget", type=int, default=0, help="N>1: SMs the persistent kernels may claim (0 = all; the rest is "
-                         "left to NCCL's all-reduce CTAs)")
+    ap.add_argument("--sm-budget", type=int, default=0, help="N>1: SMs the SM-count-sized grids may claim (0 = all; the rest "
+                         "is left to NCCL's all-reduce CTAs)")
     ap.add_argument("--eager-baseline", type=int, default=1, help="0: skip the torch-eager-on-this-GPU sample of the oracle port")
     ap.add_argument("--e2e-probe", action="store_true", help="extra timed loops that isolate the H2D / loss-read costs")
     ap.add_argument("--gemm-shapes", default=None, help="write a per-shape GEMM time table of one profiled step here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss, gradient norm and a seeded sample of the updated "
+                         "parameters with its indices to DIR/<name>.npy (float32 / float64, 12 MB in all)")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = WORKLOADS[args.workload]["batch"]
@@ -665,10 +674,10 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if args.impl == "cpu-baseline":
-        _emit(cpu_baseline(sample_steps=2, batch=4 if args.workload == "cfg2" else 2, workload=args.workload))
+        _emit(cpu_baseline(sample_steps=args.steps, batch=4 if args.workload == "cfg2" else 2, workload=args.workload))
         return
     if args.impl == "gpu-eager":
-        _emit(gpu_eager_baseline(args.workload))
+        _emit(gpu_eager_baseline(args.workload, steps=args.steps, warmup=args.warmup))
         return
     if args.impl == "reference":
         run_reference(args, rank, world)

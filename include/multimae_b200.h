@@ -1,10 +1,10 @@
 /*
- * multimae_b200 — C ABI of the B200-native (sm_100a) MultiMAE pre-training hot path.
+ * multimae_b200 — C ABI of the H100-native (sm_90a) MultiMAE pre-training hot path.
  *
  * The reference (EPFL-VILAB/MultiMAE) is pure Python on top of PyTorch: it has no FFI layer of its own.
  * The "plugin boundary" of the hot path is the Python module API consumed by run_pretraining_multimae.py
  * (SURVEY.md §8b).  This header is what the Python host side (multimae_b200/*.py, loaded with ctypes)
- * binds; every entry point names the reference code it replaces (path:line in /root/reference).
+ * binds; every entry point names the reference code it replaces (path:line in the EPFL-VILAB/MultiMAE tree).
  *
  * Conventions
  *   - every pointer is a DEVICE pointer unless the name ends in _host; no PyTorch types cross this ABI;
@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 4
+#define MMAE_ABI_VERSION 5
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -39,7 +39,7 @@ int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launches);
 int64_t mmae_profile_gemm_dump(char* buf_host, int64_t capacity);
 
 /* ------------------------------------------------------------------------------------------------
- * GEMM on the tcgen05 tensor cores (bf16 x bf16 -> fp32 accumulate in TMEM), TMA-fed.
+ * GEMM on the Hopper tensor cores (wgmma, bf16 x bf16 -> fp32 accumulate in registers), TMA-fed.
  * Replaces every nn.Linear / nn.Conv2d(k=s=P) matmul of the path:
  *   multimae/multimae_utils.py:149,153,172,180,203-204,212 ; multimae/input_adapters.py:110,232 ;
  *   multimae/output_adapters.py:258,274 and their autograd backward (dgrad / wgrad).
@@ -58,7 +58,7 @@ int64_t mmae_profile_gemm_dump(char* buf_host, int64_t capacity);
  * dgelu_z, preact_bf16 and out_bf16 are not allowed with split_k > 1.
  * split_k <= 0: automatic - split count and tile width are chosen together so that one wave of ~SM-count work items
  * covers the problem (fp32-only linear epilogues; anything else runs unsplit).  The accumulation then uses TMA
- * reduce-add tiles (cp.reduce.async.bulk.tensor) instead of per-lane atomics.
+ * reduce-add tiles (cp.reduce.async.bulk.tensor) unless mmae_gemm_set_tma_store(0).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct mmae_gemm_epilogue {
   float alpha;
@@ -74,19 +74,19 @@ typedef struct mmae_gemm_epilogue {
   int64_t ld_residual, ld_dgelu_z, ld_preact, ld_out_f32, ld_out_bf16;
 } mmae_gemm_epilogue;
 
-/* Kernel variant selection for measurements: -1 = heuristic (default), 0 = one-tile-per-CTA 128x128,
- * 1 = persistent 128x128 with double-buffered TMEM, 2 = persistent 128x256, 3 = persistent 128x192,
- * 4 / 5 / 6 = CTA-pair kernels (cluster of 2, tcgen05 cta_group::2) with 256x256 / 256x192 / 256x128 tiles.
- * Env MMAE_GEMM_VARIANT sets the initial value; MMAE_GEMM_PAIR=0 keeps the heuristic off the pair kernels. */
+/* Kernel variant for measurements: -1 = heuristic (default), 0 / 1 / 3 / 2 = one CTA per 128 x 64 / 128 / 192 / 256
+ * tile, 6 / 5 / 4 = two-CTA cluster per 256 x 128 / 192 / 256 tile (the B tile loaded once and multicast to both CTAs).
+ * Env MMAE_GEMM_VARIANT sets the initial value. */
 int mmae_gemm_set_variant(int variant);
-/* 1 (default): bf16-only epilogues of the persistent kernels leave through shared memory + TMA tile stores;
- * 0: per-lane global stores (kept for A/B measurements and for epilogues with extra operands).  Env MMAE_GEMM_TMA_STORE. */
+/* 1 (default): plain bf16 / fp32 outputs (optionally with bias / GELU) leave through shared memory + TMA tile stores, fp32
+ * accumulation (split-K, accumulate) through TMA reduce-add tiles; 0: per-thread global stores / red.global adds.
+ * Env MMAE_GEMM_TMA_STORE sets the initial value. */
 int mmae_gemm_set_tma_store(int enable);
 /* 1: kernels are launched with programmatic stream serialization and start with griddepcontrol (launch_dependents +
  * wait), so the next kernel's blocks are scheduled while the previous one drains; 0 (default): plain stream order - a
  * programmatically launched dependent keeps stale L1 lines for non-coherent loads (see runtime.cu).  Env MMAE_PDL. */
 int mmae_set_pdl(int enable);
-/* SM budget of the persistent kernels (GEMM, warp-specialised attention, one-wave element-wise grids): 0 = every SM
+/* SM budget of the SM-count-sized grids (GEMM split-K / tile choice, one-wave element-wise grids): 0 = every SM
  * (default), n = at most n.  Data-parallel runs leave NCCL's all-reduce CTAs their SMs.  Env MMAE_SM_BUDGET. */
 int mmae_set_sm_budget(int sms);
 /* 1: mmae_block_backward runs its four weight-gradient GEMMs on a library-owned side stream, forked behind the kernel
@@ -113,8 +113,8 @@ int mmae_colsum_bf16(const void* src_bf16, int64_t ld_src, float* colsum, int M,
 int mmae_gelu_bf16(const void* z, void* io, int64_t n, int backward, void* stream);
 /* dz[m,n] *= gelu'(z[m,n]) in place and colsum[n] += sum_m dz[m,n] (fc1 bias gradient) in one pass */
 int mmae_dgelu_colsum_bf16(const void* z, void* dz, int64_t ld, float* colsum, int M, int N, void* stream);
-/* 1: the module-level entry points fuse GELU / GELU' into the GEMM epilogue; 0 (default): streaming kernel after the
- * GEMM (measured faster: the epilogue is instruction-issue bound).  Env MMAE_FUSE_GELU sets the initial value. */
+/* 1: the module-level entry points fuse GELU / GELU' into the GEMM epilogue; 0: streaming kernel after the GEMM.
+ * Default and its measurement: modules.cu.  Env MMAE_FUSE_GELU sets the initial value. */
 int mmae_set_fuse_gelu(int enable);
 /* out[i] = x[i] + float(y_bf16[i]); n must be a multiple of 8 */
 int mmae_add_bf16_f32(const float* x, const void* y_bf16, float* out, int64_t n, void* stream);
@@ -152,17 +152,12 @@ int mmae_layernorm_backward_ex(const void* dy, int dy_is_bf16, int64_t lddy, con
  * buffers: head h = columns [h*head_dim, (h+1)*head_dim) from the given base pointer, batch b = rows
  * [b*N, (b+1)*N).  head_dim in {32, 64}.  lse[B,H,Nq] = log-sum-exp of the scaled scores (saved for backward).
  * backward: delta_ws is a [B,H,Nq] fp32 scratch; dq/dk/dv are written (not accumulated).
+ * Kernels: wgmma forward (<= 256 keys) / backward and warp-level mma.sync forward / backward (bf16 in, fp32 accumulate).
  * ---------------------------------------------------------------------------------------------- */
-/* bit mask: 1 = fused single-tile tcgen05 kernels (Nq, Nk <= 128, head_dim 64), 2 = general tcgen05 forward (head_dim
- * 32/64; used for <= 128 keys, with 8 also for <= 256 keys), 4 = general tcgen05 backward; 0 = warp-MMA (mma.sync +
- * ldmatrix + cp.async) kernels everywhere; 32 / 64 = warp-specialised persistent tcgen05 forward / backward (TMA warp, MMA
- * warp, 8 compute warps; attention_ws.cu) for every shape they support (forward: <= 256 keys; backward: <= 256 queries).
- * 128 = the warp-specialised forward only where the alternative is the mma.sync kernel (129..256 keys).
- * Default 3 | 64 | 128 (env MMAE_ATTN_TC); a negative value restores the start-up default. */
+/* bit mask of kernel families: 1 = wgmma forward for <= 128 keys, 2 | 8 | 32 | 128 = wgmma forward for 129..256 keys,
+ * 4 | 64 = wgmma backward; otherwise the mma.sync kernels run (16: no Hopper kernel, ignored); 0 = mma.sync everywhere.
+ * Default 0, the fastest measured on H100 (attention.cu); env MMAE_ATTN_TC; a negative value restores the start-up default. */
 int mmae_attention_set_tc(int enable);
-/* diagnostics for the warp-specialised kernels (attention_ws.cu): a device buffer of 64 x 16 int64 that CTA 0 of the next
- * launches fills with clock64 stamps of its pipeline phases (slot 16 * item + phase); NULL switches it off. */
-int mmae_attention_ws_set_trace(long long* device_buffer);
 int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                            void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
                            float scale, void* stream);
@@ -356,7 +351,7 @@ int mmae_dectail_backward(const float* dpred, int B, int nh, int nw, int Dd, int
 
 /* ------------------------------------------------------------------------------------------------
  * fp32 tier for `fp32_output_adapters` (multimae/multimae.py:367-377: the listed output adapters run outside autocast;
- * the shipped pre-training config lists ['semseg']).  Every activation stays fp32; Linear layers run as ONE bf16 tcgen05
+ * the shipped pre-training config lists ['semseg']).  Every activation stays fp32; Linear layers run as ONE bf16 wgmma
  * GEMM over 3-way split, K-concatenated operands (x_hi W_hi + x_hi W_lo + x_lo W_hi, fp32 accumulation: ~2^-16 relative),
  * attention and GELU as fp32 CUDA-core kernels.  Same argument meaning as the bf16-tier entry points of the same name;
  * the parameter / gradient structs are shared.  head_dim 32 only (the decoders').
@@ -450,8 +445,8 @@ int mmae_patchify_bf16(const float* image, void* tokens_bf16, int64_t ld_tok, in
  * ---------------------------------------------------------------------------------------------- */
 int mmae_standardize_depth(const float* depth, float* out, int B, int n, int lo, int hi, float eps, float* stats,
                            void* stream);
-/* 1 (default): the kernel validated in round 1; 2: experimental second version (histogram copies, cluster split of
- * large maps over distributed shared memory) - also MMAE_DEPTH_STD_VARIANT=2 */
+/* 1: the single-CTA radix-select kernel; 2 (default): histogram copies per CTA and a cluster split of large maps over
+ * distributed shared memory.  Env MMAE_DEPTH_STD_VARIANT sets the initial value. */
 int mmae_standardize_depth_set_variant(int variant);
 
 #ifdef __cplusplus

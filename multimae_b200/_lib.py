@@ -144,7 +144,6 @@ SIGNATURES = {
                                            c_int, c_int, c_void_p]),
     "mmae_set_sm_budget": (c_int, [c_int]),
     "mmae_attention_set_tc": (c_int, [c_int]),
-    "mmae_attention_ws_set_trace": (c_int, [c_void_p]),
     "mmae_attention_forward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
                                        c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mmae_attention_backward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
@@ -240,7 +239,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 def lib():

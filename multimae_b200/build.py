@@ -1,8 +1,8 @@
-"""Build libmultimae_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libmultimae_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m multimae_b200.build [--force] [--verbose]
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU.  The .so and the object files are build products (git-ignored).
 """
 import argparse
 import hashlib
@@ -17,8 +17,9 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libmultimae_b200.so")
 
+ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", ARCH,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -65,7 +66,7 @@ def _compile_one(args):
 
 
 def build(force=False, verbose=False):
-    """Compile every csrc/*.cu for sm_100a and link libmultimae_b200.so. Returns the library path."""
+    """Compile every csrc/*.cu for sm_90a and link libmultimae_b200.so. Returns the library path."""
     os.makedirs(OBJ, exist_ok=True)
     nvcc = _nvcc()
     srcs = _sources()
@@ -78,7 +79,7 @@ def build(force=False, verbose=False):
             if r[2]:
                 sys.stderr.write(r[2])
     if changed or not os.path.exists(LIB):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static",
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", ARCH, "-lcudart_static",
                                                       "-Xlinker", "--no-undefined", "-lpthread", "-ldl", "-lrt"]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:

@@ -17,37 +17,12 @@
 
 namespace mmae {
 void count_launch();
-bool attn_tc_supported(int Nq, int Nk, int head_dim);
-bool attn_tc_fwd_gen_supported(int H, int Nq, int Nk, int head_dim);
-bool attn_tc_bwd_gen_supported(int H, int Nq, int Nk, int head_dim);
-bool attn_ws_fwd_supported(int H, int Nq, int Nk, int head_dim);
-bool attn_ws_bwd_supported(int H, int Nq, int Nk, int head_dim);
-int attn_ws_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
+bool attn_wg_fwd_supported(int Nk, int head_dim);
+int attn_wg_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
                     float* lse, int B, int H, int Nq, int Nk, int head_dim, float scale, cudaStream_t st);
-int attn_ws_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
-                     int64_t ldo, const void* d_o, int64_t lddo, const float* lse, void* dq, int64_t lddq, void* dk,
-                     int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale,
-                     cudaStream_t st);
-bool attn_ws_fwd_supported(int H, int Nq, int Nk, int head_dim);
-bool attn_ws_bwd_supported(int H, int Nq, int Nk, int head_dim);
-int attn_ws_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
-                    float* lse, int B, int H, int Nq, int Nk, int head_dim, float scale, cudaStream_t st);
-int attn_ws_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
-                     int64_t ldo, const void* d_o, int64_t lddo, const float* lse, void* dq, int64_t lddq, void* dk,
-                     int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale,
-                     cudaStream_t st);
-int attn_tc_backward_gen(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* d_o,
-                         int64_t lddo, const float* lse, const float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
-                         void* dv, int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale, cudaStream_t st);
-int attn_tc_forward_gen(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
-                        int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim, float scale, cudaStream_t st);
-int attn_tc_forward_persistent(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
-                               int64_t ldo, float* lse, int B, int H, int Nq, int Nk, float scale, cudaStream_t st);
-int attn_tc_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
-                    float* lse, int B, int H, int Nq, int Nk, float scale, cudaStream_t st);
-int attn_tc_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* d_o,
+int attn_wg_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* d_o,
                      int64_t lddo, const float* lse, const float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
-                     void* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale, cudaStream_t st);
+                     void* dv, int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale, cudaStream_t st);
 namespace {
 
 constexpr int ATT_ROWS = 64;    // stationary rows per CTA (4 warps x 16)
@@ -543,23 +518,25 @@ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 using namespace mmae;
 
-// bit 0: fused single-tile tcgen05 kernels (encoder shape) ; bit 1: general tcgen05 forward (query tiles, <= 256 keys,
-// head_dim 32/64) ; bit 2: general tcgen05 backward (measured slower than the warp-MMA backward at N = 196: off) ;
-// bit 5 (32) / bit 6 (64): warp-specialised persistent tcgen05 forward / backward (attention_ws.cu).
-// bit 7 (128): the warp-specialised forward for > 128 keys only (where the alternative is the mma.sync kernel).
-// 0 = warp-MMA kernels everywhere.  Default 3 | 64 | 128: measured on B200 at bs 128 (scripts/gpu_check_attention_ws.py) the
-// warp-specialised backward takes 43.8 us (encoder 99 x 99 x 64; was 76.5 with the delta kernel), 77.7 us (decoder
-// 196 x 196 x 32; was 130.8 on mma.sync) and 44.3 us (196 x 99 x 32; was 77.7); the warp-specialised forward does not beat
-// the one-CTA-per-item tcgen05 kernels at <= 128 keys yet (32.8 vs 27.2 us encoder, 36.6 vs 25.5 us at 99 keys) and is used
-// where it ties with / beats the mma.sync kernel: 196 keys (50.2 vs 52.3 us) - with it no mma.sync kernel is left on the
-// MultiMAE-B 224^2 path.
+// Kernel families, as a bit mask (the values keep the meaning they had on earlier architectures where Hopper has a
+// counterpart): 1 = wgmma forward (attention_wgmma.cu) for <= 128 keys; 2 | 8 | 32 | 128 = wgmma forward for 129..256 keys;
+// 4 | 64 = wgmma backward (any length); the forward above 256 keys and the backward without those bits use the warp-level
+// mma.sync kernels of this file (bit 16 selected a persistent variant that has no Hopper kernel and is ignored).
+// 0 = mma.sync kernels everywhere.
+// Default 0 (env MMAE_ATTN_TC), from scripts/gpu_time_attention.py and bench.py on one H100 80GB HBM3 capped at 400 W,
+// MultiMAE-B bs 128, us per call (forward mma.sync / wgmma, backward mma.sync / wgmma):
+//   encoder 99 x 99, dh 64      55.3 / 77.4    165.3 / 337.9
+//   decoder 196 x 99, dh 32     46.1 / 48.1    118.9 / 198.5
+//   decoder 196 x 196, dh 32    72.7 / 122.3   193.2 / 331.5
+// and the step: 44.5 ms (0), 47.8 ms (64: wgmma backward), 48.5 ms (195: wgmma forward + backward).  The wgmma kernels
+// stage every tile with plain loads and no pipelining.  A negative value restores the start-up default.
 static int g_attn_tc = []() {
   const char* e = getenv("MMAE_ATTN_TC");
-  return e ? atoi(e) : (3 | 64 | 128);
+  return e ? atoi(e) : 0;
 }();
 static const int g_attn_tc_default = g_attn_tc;
 extern "C" int mmae_attention_set_tc(int enable) {
-  g_attn_tc = enable < 0 ? g_attn_tc_default : enable;   // negative: back to the start-up default (MMAE_ATTN_TC or 3 | 64)
+  g_attn_tc = enable < 0 ? g_attn_tc_default : enable;
   return MMAE_OK;
 }
 
@@ -573,19 +550,8 @@ extern "C" int mmae_attention_forward(const void* q, int64_t ldq, const void* k,
              MMAE_ERR_ARG, "mmae_attention_forward: 16-byte alignment / ld %% 8 required");
   dim3 grid(ceil_div(Nq, ATT_ROWS), H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // bit 5 (32): warp-specialised persistent tcgen05 forward (attention_ws.cu) for every shape it supports
-  if (((g_attn_tc & 32) || ((g_attn_tc & 128) && Nk > 128)) && attn_ws_fwd_supported(H, Nq, Nk, head_dim))
-    return attn_ws_forward(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, st);
-  if ((g_attn_tc & 1) && attn_tc_supported(Nq, Nk, head_dim)) {
-    if (g_attn_tc & 16)   // experimental persistent variant (attention_tc.cu), never on by default
-      return attn_tc_forward_persistent(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, scale, st);
-    return attn_tc_forward(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, scale, st);
-  }
-  // general tcgen05 forward: wins for up to 128 keys (26-29 us vs 33 us at 196 x 99 x 32, B*H = 1024); with a second key
-  // box the mma.sync kernel with ldmatrix + cp.async double buffering is ahead (50 vs 63 us at 196 x 196 x 32); bit 3 of
-  // the switch (8) forces the tcgen05 kernel for every supported shape
-  if ((g_attn_tc & 2) && attn_tc_fwd_gen_supported(H, Nq, Nk, head_dim) && (Nk <= 128 || (g_attn_tc & 8)))
-    return attn_tc_forward_gen(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, st);
+  if (attn_wg_fwd_supported(Nk, head_dim) && ((Nk <= 128 && (g_attn_tc & 1)) || (Nk > 128 && (g_attn_tc & (2 | 8 | 32 | 128)))))
+    return attn_wg_forward(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, st);
   const bf16 *qp = (const bf16*)q, *kp = (const bf16*)k, *vp = (const bf16*)v;
   if (head_dim == 64)
     launch_k(attn_fwd_kernel<64>, grid, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, (bf16*)o, ldo, lse, Nq, Nk, H, scale);
@@ -617,27 +583,15 @@ extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k
   const bf16 *qp = (const bf16*)q, *kp = (const bf16*)k, *vp = (const bf16*)v, *op = (const bf16*)o,
              *dop = (const bf16*)d_o;
   dim3 gq(ceil_div(Nq, ATT_ROWS), H, B), gk(ceil_div(Nk, ATT_ROWS), H, B);
-  // bit 6 (64): warp-specialised persistent tcgen05 backward (attention_ws.cu): one kernel, dV / dK / dQ accumulate in TMEM
-  // (delta = rowsum(dO o O) is computed inside the kernel from the staged tiles: no delta launch)
-  if ((g_attn_tc & 64) && attn_ws_bwd_supported(H, Nq, Nk, head_dim))
-    return attn_ws_backward(q, ldq, k, ldk, v, ldv, o, ldo, d_o, lddo, lse, dq, lddq, dk, lddk, dv, lddv, B, H, Nq, Nk,
-                            head_dim, scale, st);
-  if ((g_attn_tc & 1) && attn_tc_supported(Nq, Nk, head_dim)) {
-    launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
-    count_launch();
-    MMAE_LAUNCH_OK();
-    return attn_tc_backward(q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv, B, H, Nq, Nk,
-                            scale, st);
-  }
-  if ((g_attn_tc & 4) && attn_tc_bwd_gen_supported(H, Nq, Nk, head_dim)) {
+  if (g_attn_tc & (4 | 64)) {   // wgmma backward (attention_wgmma.cu) behind the delta kernel
     if (head_dim == 64)
       launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
     else
       launch_k(attn_delta_kernel<32>, delta_grid(B, Nq, H, 32), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
     count_launch();
     MMAE_LAUNCH_OK();
-    return attn_tc_backward_gen(q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv, B, H, Nq,
-                                Nk, head_dim, scale, st);
+    return attn_wg_backward(q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv, B, H, Nq, Nk,
+                            head_dim, scale, st);
   }
   if (head_dim == 64) {
     launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);

@@ -224,10 +224,9 @@ depth_standardize_kernel(const float* x, float* y, int n, int lo, int hi, float 
 using namespace mmae;
 
 namespace {
-// 2 (default): depth_standardize_v2.cu - 16 histogram copies per CTA and a cluster split for large maps; validated on B200
-// against the oracle fixtures (round 2: 190.6 us at 128 x 224^2 vs 194.7 us, 204.9 us at 32 x 448^2 vs 859.7 us for the kernel
-// of this file, torch.sort: 757 / 562 us).  1: the single-CTA kernel of this file (also the fallback for maps beyond 8 CTAs'
-// shared memory).
+// 2 (default): depth_standardize_v2.cu - 16 histogram copies per CTA and a cluster split for large maps, checked against the
+// oracle fixtures (tests/test_cuda_kernels.py).  1: the single-CTA kernel of this file (also the fallback for maps beyond 8
+// CTAs' shared memory).
 int depth_std_variant() {
   static int v = [] {
     const char* e = getenv("MMAE_DEPTH_STD_VARIANT");

@@ -1,12 +1,8 @@
 // Truncated depth standardisation, second version - the default since round 2 (mmae_standardize_depth_set_variant(1) /
-// MMAE_DEPTH_STD_VARIANT=1 select the kernel of depth_standardize.cu).  Validated on B200 against the oracle fixtures
-// (tests/test_cuda_kernels.py) and timed (profiles/r02_depth_standardize_timing.log): 193 us at 128 x 224^2, 205 us at
-// 32 x 448^2 (variant 1: 195 / 860 us; the reference's torch.sort expression: 747 / 557 us).  Both variants are latency-bound
-// shared-memory selects at 0.04 of the 8 B/pixel HBM figure; clusters larger than the map needs are slower
-// (MMAE_DEPTH_STD_MIN_CLUSTER: 214 / 270 / 545 us for 2 / 4 / 8 CTAs at 224^2).
+// MMAE_DEPTH_STD_VARIANT=1 select the kernel of depth_standardize.cu), checked against the oracle fixtures
+// (tests/test_cuda_kernels.py).  Both variants are latency-bound shared-memory selects well below the 8 B/pixel HBM figure.
 //
-// What the round-1 measurement showed (profiles/r01_depth_standardize_timing.log): variant 1 runs at 0.04 of the 8 B/pixel
-// HBM bound.  Its first radix-select pass funnels 32 warps into a handful of shared-memory histogram bins (depth maps use
+// Variant 1's first radix-select pass funnels 32 warps into a handful of shared-memory histogram bins (depth maps use
 // few exponent values; warp aggregation removes only the intra-warp conflicts), and maps that do not fit one CTA's
 // shared memory (448^2) fall back to seven passes over L2 on only B CTAs.  This version
 //   * keeps 16 histogram copies (pass 0: one selection, 2 warps per copy; later passes: 2 selections x 8 copies);

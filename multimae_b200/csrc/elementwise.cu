@@ -219,8 +219,7 @@ __global__ void __launch_bounds__(256) colsum_bf16_kernel(const bf16* __restrict
 }
 
 // a = gelu(z)  /  dz *= gelu'(z): bf16 streams, 8 elements per thread.  Used when the GELU is NOT fused into the GEMM
-// epilogue: a tcgen05 epilogue has ~4 instruction-issue slots per clock next to a tile's MMA time, which the ~14
-// instructions/element of erf-GELU overrun; a full-occupancy streaming kernel does not.
+// epilogue (mmae_set_fuse_gelu(0), the default: faster on H100, see modules.cu).
 template <bool BACKWARD>
 __global__ void __launch_bounds__(256) gelu_stream_kernel(const bf16* __restrict__ z, bf16* __restrict__ io, int64_t n) {
   pdl_prologue();

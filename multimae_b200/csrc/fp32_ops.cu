@@ -3,8 +3,8 @@
 // cfgs/pretrain/multimae-b_98_rgb+-depth-semseg_1600e.yaml:28).
 //
 //   * fp32-accurate Linear on the bf16 tensor cores: x = x_hi + x_lo, W = W_hi + W_lo (two bf16 pieces each, 16 mantissa
-//     bits) and  x W^T ~= x_hi W_hi^T + x_hi W_lo^T + x_lo W_hi^T  is ONE tcgen05 GEMM over a K-concatenated operand pair
-//     A' = [x_hi | x_hi | x_lo], B' = [W_hi | W_lo | W_hi] (fp32 accumulation in TMEM; the dropped x_lo W_lo^T term and the
+//     bits) and  x W^T ~= x_hi W_hi^T + x_hi W_lo^T + x_lo W_hi^T  is ONE wgmma GEMM over a K-concatenated operand pair
+//     A' = [x_hi | x_hi | x_lo], B' = [W_hi | W_lo | W_hi] (fp32 accumulation; the dropped x_lo W_lo^T term and the
 //     split residuals are ~2^-16 relative).  dgrad / wgrad use the same trick with row-stacked (MN-major) operands.
 //   * attention, GELU in plain fp32 CUDA-core kernels (decoder sizes: 196 x <= 196 keys, head_dim 32 - 5 GFLOP per call).
 #include <cstdlib>

@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
 // dgamma/dbeta: per-lane register partials over the block's rows -> smem reduce over warps -> one partial row per block.
 //
 // Persistent: the grid is one wave (blocks = SMs x resident blocks), warps stride over the rows, so there is no partial
-// last wave (12672 rows in 64-row blocks were 198 blocks on 148 SMs: a third of the time ran at 1/3 occupancy) and the
+// last wave (12672 rows in 64-row blocks are 198 blocks: on 132 SMs half of the time would run at half occupancy) and the
 // column-sum atomics drop to one set per resident block.  The next row's x / dy loads are issued before the current
 // row's reductions (the per-lane column accumulators cap residency at 8 warps per SM for D = 768, so a warp has to
 // carry its own memory-level parallelism).

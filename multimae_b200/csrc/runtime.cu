@@ -69,7 +69,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
-    if (cached <= 0) cached = 148;
+    if (cached <= 0) cached = 132;
   }
   return g_sm_budget > 0 && g_sm_budget < cached ? g_sm_budget : cached;
 }
@@ -114,18 +114,18 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_
   return MMAE_OK;
 }
 
-// Output-tile map for the GEMM epilogue's TMA stores / reductions: box = 32 rows x 64 bytes (32 bf16 or 16 fp32 columns),
-// SWIZZLE_64B.  `ld` in elements.
+// Output-tile map for the GEMM epilogue's TMA stores / reductions: box = 64 rows x 32 columns, dense (no swizzle).
+// `ld` in elements.
 int make_tmap_2d_store(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld) {
   encode_tiled_fn fn = get_encode_fn();
   if (!fn) return MMAE_ERR_CUDA;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
-  cuuint32_t box[2] = {(cuuint32_t)(64 / elem_bytes), 32};
+  cuuint32_t box[2] = {32, 64};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
                   const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_last_error("cuTensorMapEncodeTiled(store) failed: %d (rows=%llu cols=%llu ld=%llu base=%p)", (int)r,

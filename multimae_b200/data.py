@@ -9,7 +9,7 @@ opt-in through the overlay launcher:
                          critical path (the same pipeline bench.py's end-to-end leg times).
   * MMAE_SYNTHETIC_DATA=N  `build_multimae_pretraining_dataset` returns N synthetic samples (rgb / depth / semseg tensors of
                          the configured input size) served from a small pool of pre-generated tensors: a data source that
-                         keeps up with a B200 (the PIL pipeline delivers a few hundred samples/s per worker), for measuring
+                         keeps up with an H100 (the PIL pipeline delivers a few hundred samples/s per worker), for measuring
                          the unchanged script end to end.
 """
 import os

@@ -18,7 +18,7 @@ from . import _lib as L
 
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise L.MmaeError("multimae_b200.%s needs CUDA tensors: the path is sm_100a kernels only (no CPU fallback)" % what)
+        raise L.MmaeError("multimae_b200.%s needs CUDA tensors: the path is sm_90a kernels only (no CPU fallback)" % what)
 
 
 class Workspace:

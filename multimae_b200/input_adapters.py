@@ -1,7 +1,7 @@
 """Input adapters with the reference's constructor / attribute / state_dict contract (multimae/input_adapters.py).
 
 Inside `MultiMAE.forward` the adapters are not called one by one: the model embeds only the visible patches of all
-modalities with one K-concatenated tcgen05 GEMM (functional.EmbedFunction).  Calling an adapter directly embeds all of
+modalities with one K-concatenated wgmma GEMM (functional.EmbedFunction).  Calling an adapter directly embeds all of
 its patches through the same kernels (MultiViT / stand-alone use)."""
 from typing import Optional, Tuple, Union
 

@@ -1,8 +1,8 @@
-"""MultiMAE / MultiViT with the reference's module API (multimae/multimae.py), executing on sm_100a kernels.
+"""MultiMAE / MultiViT with the reference's module API (multimae/multimae.py), executing on sm_90a (H100) kernels.
 
 Same constructor signature, parameter names / shapes (state_dict schema of SURVEY.md §A.1), factories registered under
 the same names, and the same `forward` contract — `(preds, task_masks)` — so run_pretraining_multimae.py can drive it
-unchanged.  What differs is the execution plan (DESIGN.md): gather-first patch embedding, one mask-sampler kernel,
+unchanged.  What differs is the execution plan: gather-first patch embedding, one mask-sampler kernel,
 fused transformer blocks, fused decoder head/tail, gradients accumulated into one flat arena.
 """
 import itertools

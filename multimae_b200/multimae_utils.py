@@ -1,5 +1,5 @@
 """Transformer building blocks with the reference's module / parameter names (multimae/multimae_utils.py), executing on
-the sm_100a kernels.  `Block` is the unit of execution (one fused forward / backward sequence); `Attention`, `Mlp` and
+the sm_90a kernels.  `Block` is the unit of execution (one fused forward / backward sequence); `Attention`, `Mlp` and
 `CrossAttention` are parameter containers with the reference constructor signatures so that `state_dict()` keys match
 (SURVEY.md §A.1)."""
 import math

@@ -1,5 +1,5 @@
 """Drop-in overlay: make `import multimae...` / `from utils import NativeScalerWithGradNormCount` resolve to this package
-so the reference's UNCHANGED run_pretraining_multimae.py drives the sm_100a path.
+so the reference's UNCHANGED run_pretraining_multimae.py drives the sm_90a path.
 
     python -m multimae_b200.overlay /path/to/MultiMAE/run_pretraining_multimae.py -c cfg.yaml [script args...]
 

@@ -71,7 +71,7 @@ class TrainStep:
         B = next(iter(example_x.values())).shape[0]
         self.static_x = {k: v.clone() for k, v in example_x.items()}
         # Task shares: drawn on the device inside the graph (no per-step host -> device copy: a small H2D on the compute
-        # stream queues behind the in-flight input-batch copy on the one H2D engine and stalls the step by its ~2 ms).
+        # stream queues behind the in-flight input-batch copy on the one H2D engine and stalls the step until it is done).
         # Sampling uniformly over task subsets keeps the reference's host draw, fed through a static buffer.
         self._shares_host = None
         self.model.external_shares = None
@@ -88,9 +88,8 @@ class TrainStep:
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
-        # Programmatic dependent launch pays off for eager launches (measured -3.5 % step time) but not inside a graph,
-        # whose kernel-to-kernel edges are already tight (measured +0.7 %, and +10 % with a concurrent H2D copy): the
-        # captured nodes get plain edges.
+        # Captured nodes get plain edges: a graph's kernel-to-kernel edges are already tight, and programmatic dependent
+        # launch can leave stale L1 lines for non-coherent loads (runtime.cu).
         lib = L.lib()
         lib.mmae_set_pdl(0)
         try:

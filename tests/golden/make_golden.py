@@ -1,12 +1,12 @@
-"""Generate the golden fixtures under tests/golden/ from the LIVE reference (runs only where /root/reference exists).
+"""Generate the golden fixtures under tests/golden/ from the LIVE reference (a checkout of EPFL-VILAB/MultiMAE).
 
-    python tests/golden/make_golden.py
+    MULTIMAE_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 
 The reference (EPFL-VILAB/MultiMAE) has no tests or golden vectors of its own, so these fixtures are what pins the
 oracle (oracle/multimae_oracle.py) and, through it, the CUDA path.  The reference is imported unmodified; the only
 shim is a stub `torch._six` module (utils/native_scaler.py:11 imports a module removed in torch >= 2.0).
 
-Fixtures (all fp32, CPU, torch.save of plain dicts of tensors):
+Fixtures (all fp32, CPU, plain dicts of tensors; helpers.save_fixture splits one above ~1 MB over <name>.<i>.pt):
   sampler_*.pt : Dirichlet shares + uniform noises fed to / index triples returned by generate_random_masks
   tiny3.pt     : 3-modality MultiMAE (dim 32, depth 2) fwd + 4 losses + all parameter gradients
   interp.pt    : RGB-only model built with the default 224 pos-emb grid run on 32x32 inputs (bicubic/bilinear resize)
@@ -29,13 +29,15 @@ from functools import partial
 
 import torch
 
-REF = "/root/reference"
+REF = os.environ.get("MULTIMAE_REFERENCE", "")
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(HERE))
+from helpers import save_fixture  # noqa: E402
 
 
 def import_reference():
     if not os.path.isdir(REF):
-        raise SystemExit("reference tree %s not present: fixtures can only be regenerated in the authoring container" % REF)
+        raise SystemExit("reference tree %r not present: set MULTIMAE_REFERENCE to a checkout of EPFL-VILAB/MultiMAE" % REF)
     six = types.ModuleType("torch._six")
     six.inf = math.inf
     sys.modules.setdefault("torch._six", six)
@@ -67,7 +69,7 @@ def record_sampler(R, name, B, tokens_per_task, num_encoded, alphas, seed):
         chk.append(torch.where(order < per_task[:, i:i + 1], 0, 1))
     ids_shuffle = torch.argsort(torch.cat(chk, 1) + noise_all, dim=1)
     assert torch.equal(ids_shuffle[:, :num_encoded], ids_keep), "RNG replay diverged from the reference"
-    torch.save({"shares": shares, "noises": noises, "noise_all": noise_all, "num_encoded": num_encoded,
+    save_fixture({"shares": shares, "noises": noises, "noise_all": noise_all, "num_encoded": num_encoded,
                 "task_masks": [masks[k] for k in fake], "ids_keep": ids_keep, "ids_restore": ids_restore},
                os.path.join(HERE, name))
     print("wrote", name)
@@ -142,7 +144,7 @@ def record_model(R, name, in_domains, B, size, num_encoded, seed, formula=False,
         state, grads_out = None, {k: digest(v) for k, v in grads.items()}
     else:
         state, grads_out = {k: v.detach().clone() for k, v in model.state_dict().items()}, grads
-    torch.save({
+    save_fixture({
         "config": dict(in_domains=list(in_domains), B=B, size=size, num_encoded=num_encoded, formula=formula, feed=feed,
                        **kw),
         "state_dict": state,
@@ -178,7 +180,7 @@ def record_fixed_masks(R, name):
     with torch.no_grad():
         preds_all, masks_all = model(x2, mask_inputs=False)
     assert all(int(v.sum()) == 0 for v in masks_all.values())
-    torch.save({"config": dict(in_domains=["rgb", "depth", "semseg"], **kw),
+    save_fixture({"config": dict(in_domains=["rgb", "depth", "semseg"], **kw),
                 "state_dict": {k: v.detach().clone() for k, v in model.state_dict().items()},
                 "x_fixed": x1, "task_masks": tm, "preds_fixed": {k: v.clone() for k, v in preds_fixed.items()},
                 "x_all": x2, "preds_all": {k: v.clone() for k, v in preds_all.items()}}, os.path.join(HERE, name))
@@ -213,7 +215,7 @@ def record_losses(R, name):
                 loss.backward()
                 rec["grad_" + mname] = pr.grad.clone()
         out["cases"][key] = rec
-    torch.save(out, os.path.join(HERE, name))
+    save_fixture(out, os.path.join(HERE, name))
     print("wrote", name, {k: round(float(v["loss_masked"]), 6) for k, v in out["cases"].items()})
 
 
@@ -238,7 +240,7 @@ def record_depth_standardize(name):
     depth[3, :, :12] = 7.25                                               # one value covering half of the map
     ns = {"torch": torch, "rearrange": rearrange, "tasks_dict": {"depth": depth.clone()}}
     exec(code, ns)
-    torch.save({"depth": depth, "standardized": ns["tasks_dict"]["depth"].clone()},
+    save_fixture({"depth": depth, "standardized": ns["tasks_dict"]["depth"].clone()},
                os.path.join(HERE, name))
     print("wrote", name, "(executed %d reference source lines)" % len(code.splitlines()))
 

@@ -48,16 +48,19 @@ def test_workload_table_matches_survey():
     assert bench.WORKLOADS["cfg2"]["metric"] == bench.METRIC
 
 
-def test_encoder_tensor_core_figure_from_the_committed_table():
-    """bench.encoder_tc_from_table on the per-shape table of the committed round-1 run: the 144 encoder GEMM launches
-    (12 blocks x {QKV, proj, fc1, fc2} x {forward, dgrad, wgrad}) and nothing from the decoders / embedding."""
+def test_encoder_tensor_core_figure_from_a_gemm_table():
+    """bench.encoder_tc_from_table on a per-shape table of one MultiMAE-B step (bs 128, 99 encoder rows per sample): the
+    144 encoder GEMM launches (12 blocks x {QKV, proj, fc1, fc2} x {forward, dgrad, wgrad}) and nothing from the decoders /
+    embedding.  Every encoder launch is timed at exactly 500 TFLOP/s."""
     sys.path.insert(0, ROOT)
     import bench
-    agg = {}
-    for line in open(os.path.join(ROOT, "profiles", "r01_gemm_per_shape_7330.txt")).read().splitlines()[1:]:
-        M, N, K, maj, split, cnt, ms, _tf = line.split()
-        agg[(int(M), int(N), int(K), int(maj), int(split))] = [int(cnt), float(ms)]
-    r = bench.encoder_tc_from_table(agg, 128 * 99, 768, 1436.1)
+    R, D = 128 * 99, 768
+    fwd = [(R, 3 * D, D), (R, D, D), (R, 4 * D, D), (R, D, 4 * D)]
+    shapes = [(m, n, k, 0) for m, n, k in fwd] + [(R, k, n, 2) for _, n, k in fwd] + [(n, k, R, 3) for _, n, k in fwd]
+    agg = {(m, n, k, maj, 1): [12, 12 * 2.0 * m * n * k / 500e12 * 1e3] for m, n, k, maj in shapes}
+    agg[(25088, 256, 256, 0, 1)] = [17, 0.3]                 # decoder / embedding shapes are not counted
+    agg[(R, 256, D, 0, 1)] = [4, 0.2]
+    r = bench.encoder_tc_from_table(agg, R, D, 989.0)
     assert r["launches_per_step"] == 144
-    assert 900 < r["encoder_gemm_tflops"] < 1300 and abs(r["frac_of_measured_peak"] - r["encoder_gemm_tflops"] / 1436.1) < 1e-3
-    assert bench.encoder_tc_from_table({(25088, 256, 256, 0, 1): [17, 0.3]}, 128 * 99, 768, 1436.1) is None
+    assert abs(r["encoder_gemm_tflops"] - 500.0) < 0.1 and abs(r["frac_of_measured_peak"] - 500.0 / 989.0) < 1e-3
+    assert bench.encoder_tc_from_table({(25088, 256, 256, 0, 1): [17, 0.3]}, R, D, 989.0) is None

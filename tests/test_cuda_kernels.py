@@ -93,7 +93,7 @@ def test_gemm_fused_epilogues(dev, KN, variant):
                                    (25088, 256, 256)])
 def test_gemm_tma_store_epilogue(dev, KN, variant, shape):
     """bf16 outputs through shared memory + TMA tile stores: ragged M / N edges, a strided output view, bias and GELU;
-    bit-identical to the per-lane store path and untouched bytes outside the [M, N] view."""
+    bit-identical to the per-thread store path and untouched bytes outside the [M, N] view."""
     from multimae_b200 import _lib as L
     L.lib().mmae_gemm_set_variant(variant)
     M, N, K = shape
@@ -127,18 +127,20 @@ def test_gemm_tma_store_epilogue(dev, KN, variant, shape):
 
 
 def test_gemm_heuristic_picks_pair_kernels_correctly(dev, KN):
-    """The default heuristic sends the big encoder shapes to the CTA-pair kernels: same results as the single-CTA ones."""
+    """On the big encoder shapes the heuristic's choice, a single-CTA 128 x 192 tile and the two-CTA cluster (pair) kernels
+    give the same results."""
     from multimae_b200 import _lib as L
     for (M, N, K, b_mn) in [(12672, 3072, 768, False), (12672, 3072, 768, True), (12672, 768, 3072, False)]:
         A, B = _bf16(dev, M, K), _bf16(dev, N, K)
         bias = torch.randn(N, device=dev)
         outs = []
-        for variant in (-1, 3):
+        for variant in (-1, 3, 4, 6):
             L.lib().mmae_gemm_set_variant(variant)
             o = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
             KN.gemm(A, B.t().contiguous() if b_mn else B, b_mn=b_mn, bias=bias, out_bf16=o)
             outs.append(o)
-        assert rel_l2(outs[0], outs[1]) < 1e-4, (M, N, K, b_mn)
+        for o in outs[1:]:
+            assert rel_l2(outs[0], o) < 1e-4, (M, N, K, b_mn)
 
 
 def test_gemm_rejects_bad_arguments(dev, KN):
@@ -184,9 +186,8 @@ ATTN_CASES = [(3, 12, 99, 99, 64, True), (2, 8, 196, 99, 32, False), (2, 8, 196,
               (1, 2, 100, 33, 64, False), (1, 2, 256, 256, 64, True), (1, 4, 200, 129, 32, False), (5, 8, 196, 196, 32, True)]
 
 
-# 15: every one-CTA-per-item tcgen05 kernel wherever it is supported; 195: the default (warp-specialised backward, and
-# forward for > 128 keys); 99: warp-specialised forward AND backward wherever supported (attention_ws.cu); 19: the
-# persistent encoder forward
+# switch values (attention.cu): 0 = mma.sync kernels everywhere; 1 = wgmma forward for <= 128 keys only; 3, 7, 15, 19, 195,
+# 99 = wgmma forward wherever it applies (<= 256 keys), mma.sync above 256 keys and for the backward
 @pytest.mark.parametrize("tc", [0, 1, 3, 7, 15, 19, 195, 99])
 @pytest.mark.parametrize("case", ATTN_CASES)
 def test_attention_forward_backward(dev, KN, tc, case):

@@ -8,7 +8,7 @@ import os
 import pytest
 import torch
 
-from helpers import formula_fill_, rel_l2
+from helpers import formula_fill_, load_fixture, rel_l2
 from multimae_b200 import _lib as L
 from oracle import multimae_oracle as O
 
@@ -26,7 +26,7 @@ def dev():
 
 
 def _load(golden_dir, name):
-    return torch.load(os.path.join(golden_dir, name), map_location="cpu", weights_only=False)
+    return load_fixture(golden_dir, name)
 
 
 def _build_model(c):
@@ -269,7 +269,7 @@ FP32_TOL = 1e-3          # north_star "1e-3 rel fp32": the fp32 tier of fp32_out
 
 @pytest.mark.parametrize("task", ["semseg", "rgb"])
 def test_fp32_output_adapter_tier(golden_dir, dev, task):
-    """fp32_output_adapters (multimae/multimae.py:367-377): an adapter run in the fp32 tier - 3 x bf16 split tcgen05 GEMMs,
+    """fp32_output_adapters (multimae/multimae.py:367-377): an adapter run in the fp32 tier - 3 x bf16 split wgmma GEMMs,
     fp32 attention / GELU / LayerNorm - against the fp32 oracle's decode_task on the SAME encoder tokens: prediction, the
     gradient w.r.t. the encoder tokens and every parameter gradient of the adapter to 1e-3."""
     fx = _load(golden_dir, "cuda_small.pt")

@@ -5,10 +5,13 @@
  * the product path refuses to run without CUDA (no CPU fallback)."""
 import os
 import re
+import subprocess
+import sys
 
 import pytest
 import torch
 
+from helpers import load_fixture
 from oracle import multimae_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -47,11 +50,15 @@ def test_abi_exports_every_declared_symbol():
     for name in declared:
         assert getattr(handle, name) is not None
     assert handle.mmae_abi_version() == L.ABI_VERSION
-    assert handle.mmae_launch_count() == 0     # nothing launched on a CPU box
+    # loading the library launches nothing: checked in a fresh process (earlier GPU tests of this session launched kernels)
+    code = ("import sys; sys.path.insert(0, %r); from multimae_b200 import _lib as L; "
+            "print(L.lib().mmae_launch_count())" % ROOT)
+    res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=120)
+    assert res.returncode == 0 and res.stdout.strip() == "0", res.stdout + res.stderr
 
 
 def test_state_dict_schema_and_roundtrip(golden_dir):
-    fx = torch.load(os.path.join(golden_dir, "cuda_small.pt"), map_location="cpu", weights_only=False)
+    fx = load_fixture(golden_dir, "cuda_small.pt")
     c = fx["config"]
     model = _build(tuple(c["in_domains"]), c["dim"], c["depth"], c["heads"], c["dec_dim"], c["dec_depth"], c["dec_heads"],
                    c["image_size"])
