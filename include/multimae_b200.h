@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 5
+#define MMAE_ABI_VERSION 6
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -264,6 +264,21 @@ int mmae_block_backward_chain(const float* x_in, const float* dx_out, const void
                               void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
                               const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
                               void* stream);
+/* Stochastic depth (drop path, multimae/multimae_utils.py:105-132, 230-231): the _chain forms with three per-sample fp32
+ * factors, each float[B] or NULL (factor 1).  Forward computes
+ *   x_mid = x + scale_attn[b] * attn(norm1(x)),   x_out = x_mid + scale_mlp[b] * mlp(norm2(x_mid))
+ * for the rows of sample b (row r of the [B*N, D] activation belongs to sample r / N), with the block input
+ * x = x_in + scale_prev[b] * x_add_bf16 when chained (scale_prev: the PREVIOUS block's scale_mlp; needs x_add_bf16).
+ * Backward takes the same three vectors: the gradient entering a branch is scaled, the residual-path gradient is not;
+ * dx_out_bf16 / dx_in_bf16 carry bf16(scale_mlp * dx_out) / bf16(scale_prev * dx_in) and their column sums go to the
+ * fc2 bias gradients (scale_prev needs dx_in_bf16).  All three NULL: the _chain forms exactly. */
+int mmae_block_forward_dp(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16, int B,
+                          int N, int D, int H, int hidden, float eps, const float* scale_attn, const float* scale_mlp,
+                          const float* scale_prev, const mmae_block_params* prm, void* saved, void* ws, void* stream);
+int mmae_block_backward_dp(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in, void* dx_in_bf16,
+                           float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* scale_attn,
+                           const float* scale_mlp, const float* scale_prev, const mmae_block_params* prm,
+                           const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SpatialOutputAdapter, split at its decoder_transformer (multimae/output_adapters.py:236-282):
@@ -378,6 +393,14 @@ int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D,
 int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
                             const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
                             void* stream);
+/* stochastic depth in the fp32 tier: per-sample factors of the attention / MLP branch, float[B] or NULL (see
+ * mmae_block_forward_dp); both NULL: mmae_block_f32_forward / _backward */
+int mmae_block_f32_forward_dp(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
+                              const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm, void* saved,
+                              void* ws, void* stream);
+int mmae_block_f32_backward_dp(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
+                               const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm,
+                               const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
 int64_t mmae_dechead_f32_saved_bytes(const mmae_decoder_index* ix, int D_enc, int H, int hidden);
 int64_t mmae_dechead_f32_workspace_bytes(const mmae_decoder_index* ix, int D_enc, int H, int hidden);
 int mmae_dechead_f32_forward(const float* enc, int D_enc, const mmae_decoder_index* ix, int H, int hidden, float eps,

@@ -171,6 +171,12 @@ SIGNATURES = {
     "mmae_block_backward_chain": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                           c_int, c_int, ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p,
                                           c_void_p, c_void_p]),
+    "mmae_block_forward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams), c_void_p, c_void_p,
+                                      c_void_p]),
+    "mmae_block_backward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                       c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams),
+                                       ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
     "mmae_dechead_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -223,6 +229,11 @@ SIGNATURES = {
     "mmae_block_f32_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                         ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
                                         c_void_p]),
+    "mmae_block_f32_forward_dp": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
+                                          ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
+    "mmae_block_f32_backward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                           ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
+                                           c_void_p]),
     "mmae_dechead_f32_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_f32_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_f32_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -239,7 +250,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 def lib():

@@ -82,7 +82,8 @@ __global__ void __launch_bounds__(256) cast_colsum_kernel(const void* __restrict
                                                           bf16* __restrict__ dst, int64_t ld_dst,
                                                           float* __restrict__ colsum, float* __restrict__ partial,
                                                           unsigned int* __restrict__ counters, int M, int N,
-                                                          int rows_per_block) {
+                                                          int rows_per_block, const float* __restrict__ row_scale,
+                                                          int rows_per_sample) {
   pdl_prologue();
   __shared__ float4 red[8][32];
   __shared__ float red2[8 * 32 * 5];
@@ -99,6 +100,10 @@ __global__ void __launch_bounds__(256) cast_colsum_kernel(const void* __restrict
         v = make_float4(a.x, a.y, b.x, b.y);
       } else {
         v = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(src_) + int64_t(r) * ld_src + col));
+        if (row_scale != nullptr) {   // per-sample factor (stochastic depth) on the cast copy and on the column sums
+          const float sc = __ldg(row_scale + r / rows_per_sample);
+          v = make_float4(sc * v.x, sc * v.y, sc * v.z, sc * v.w);
+        }
         if (dst) {
           uint2 o;
           o.x = pack_bf16x2(v.x, v.y);
@@ -333,18 +338,31 @@ __global__ void __launch_bounds__(256) dgelu_colsum_kernel(const bf16* __restric
   }
 }
 
-// out[i] = x[i] + float(y_bf16[i])   (residual add of a bf16 branch output onto the fp32 stream)
-__global__ void __launch_bounds__(256) add_bf16_f32_kernel(const float* __restrict__ x, const bf16* __restrict__ y,
-                                                           float* __restrict__ out, int64_t n) {
+// out[i] = x[i] + s * y[i]   (residual add of a branch output onto the fp32 stream; y bf16 or fp32)
+// s = row_scale[i / per_sample] (stochastic depth: 0 or 1/keep per sample), 1 without row_scale - then x + 1 * y == x + y
+// exactly, with or without FMA contraction.  x == null: out = s * y (the fp32 tier's scaled copy of a branch gradient).
+template <bool Y_BF16>
+__global__ void __launch_bounds__(256) add_bf16_f32_kernel(const float* __restrict__ x, const void* __restrict__ y_,
+                                                           float* __restrict__ out, int64_t n,
+                                                           const float* __restrict__ row_scale, int64_t per_sample) {
   pdl_prologue();
   const int64_t stride = int64_t(gridDim.x) * blockDim.x * 8;
   for (int64_t i = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) * 8; i < n; i += stride) {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(x + i));
-    const float4 b = __ldg(reinterpret_cast<const float4*>(x + i + 4));
-    const uint4 yv = __ldg(reinterpret_cast<const uint4*>(y + i));
-    const float2 y0 = unpack_bf16x2(yv.x), y1 = unpack_bf16x2(yv.y), y2 = unpack_bf16x2(yv.z), y3 = unpack_bf16x2(yv.w);
-    *reinterpret_cast<float4*>(out + i) = make_float4(a.x + y0.x, a.y + y0.y, a.z + y1.x, a.w + y1.y);
-    *reinterpret_cast<float4*>(out + i + 4) = make_float4(b.x + y2.x, b.y + y2.y, b.z + y3.x, b.w + y3.y);
+    const float4 a = x != nullptr ? __ldg(reinterpret_cast<const float4*>(x + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 b = x != nullptr ? __ldg(reinterpret_cast<const float4*>(x + i + 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float4 y0, y1;
+    if constexpr (Y_BF16) {
+      const uint4 yv = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const bf16*>(y_) + i));
+      const float2 p0 = unpack_bf16x2(yv.x), p1 = unpack_bf16x2(yv.y), p2 = unpack_bf16x2(yv.z), p3 = unpack_bf16x2(yv.w);
+      y0 = make_float4(p0.x, p0.y, p1.x, p1.y);
+      y1 = make_float4(p2.x, p2.y, p3.x, p3.y);
+    } else {
+      y0 = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(y_) + i));
+      y1 = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(y_) + i + 4));
+    }
+    const float s = row_scale != nullptr ? __ldg(row_scale + i / per_sample) : 1.0f;   // per_sample % 8 == 0
+    *reinterpret_cast<float4*>(out + i) = make_float4(a.x + s * y0.x, a.y + s * y0.y, a.z + s * y0.z, a.w + s * y0.w);
+    *reinterpret_cast<float4*>(out + i + 4) = make_float4(b.x + s * y1.x, b.y + s * y1.y, b.z + s * y1.z, b.w + s * y1.w);
   }
 }
 
@@ -510,10 +528,12 @@ extern "C" int mmae_cast_f32_to_bf16(const float* src, void* dst_bf16, int64_t n
   return MMAE_OK;
 }
 
-extern "C" int mmae_cast_colsum_f32(const float* src, int64_t ld_src, void* dst_bf16, int64_t ld_dst, float* colsum,
-                                    int M, int N, void* stream) {
+int mmae::cast_colsum_f32_scaled(const float* src, int64_t ld_src, bf16* dst_bf16, int64_t ld_dst, float* colsum,
+                                 const float* row_scale, int rows_per_sample, int M, int N, void* stream) {
   MMAE_CHECK(src && M > 0 && N > 0 && N % 4 == 0 && ld_src % 4 == 0 && (!dst_bf16 || ld_dst % 4 == 0), MMAE_ERR_ARG,
              "mmae_cast_colsum_f32: bad args (N, ld must be multiples of 4)");
+  MMAE_CHECK(!row_scale || (rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
+             "mmae_cast_colsum_f32: rows-per-sample must divide M=%d", M);
   cudaStream_t cst = reinterpret_cast<cudaStream_t>(stream);
   const int rpb = colsum_rows_per_block(M, ceil_div(N, 128), 4);
   dim3 grid(ceil_div(N, 128), ceil_div(M, rpb)), block(32, 8);
@@ -522,12 +542,18 @@ extern "C" int mmae_cast_colsum_f32(const float* src, int64_t ld_src, void* dst_
     partial = colred_scratch(size_t(grid.y) * N, cst);
     if (!partial) return MMAE_ERR_CUDA;
   }
-  launch_k(cast_colsum_kernel<false>, grid, block, 0, cst, src, ld_src, reinterpret_cast<bf16*>(dst_bf16), ld_dst, colsum, partial,
-                                                     g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb);
+  launch_k(cast_colsum_kernel<false>, grid, block, 0, cst, src, ld_src, dst_bf16, ld_dst, colsum, partial,
+                                                     g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb, row_scale,
+                                                     rows_per_sample);
   count_launch();
   MMAE_LAUNCH_OK();
   if (partial && !g_colred_fold) return colred_finalize(partial, grid.y, N, N, colsum, nullptr, nullptr, cst);
   return MMAE_OK;
+}
+
+extern "C" int mmae_cast_colsum_f32(const float* src, int64_t ld_src, void* dst_bf16, int64_t ld_dst, float* colsum,
+                                    int M, int N, void* stream) {
+  return cast_colsum_f32_scaled(src, ld_src, reinterpret_cast<bf16*>(dst_bf16), ld_dst, colsum, nullptr, 1, M, N, stream);
 }
 
 extern "C" int mmae_colsum_bf16(const void* src_bf16, int64_t ld_src, float* colsum, int M, int N, void* stream) {
@@ -548,7 +574,8 @@ extern "C" int mmae_colsum_bf16(const void* src_bf16, int64_t ld_src, float* col
                                                 g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb);
   else
     launch_k(cast_colsum_kernel<true>, grid, block, 0, cst, src_bf16, ld_src, nullptr, 0, colsum, partial,
-                                                      g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb);
+                                                      g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb,
+                                                      nullptr, 1);
   count_launch();
   MMAE_LAUNCH_OK();
   if (partial && !g_colred_fold) return colred_finalize(partial, grid.y, N, N, colsum, nullptr, nullptr, cst);
@@ -583,16 +610,29 @@ extern "C" int mmae_gelu_bf16(const void* z, void* io, int64_t n, int backward, 
   return MMAE_OK;
 }
 
-extern "C" int mmae_add_bf16_f32(const float* x, const void* y_bf16, float* out, int64_t n, void* stream) {
-  MMAE_CHECK(x && y_bf16 && out && n >= 0 && n % 8 == 0, MMAE_ERR_ARG, "mmae_add_bf16_f32: bad args (n %% 8)");
+int mmae::add_scaled_f32(const float* x, const void* y, int y_is_bf16, const float* row_scale, int64_t per_sample, float* out,
+                         int64_t n, void* stream) {
+  MMAE_CHECK(y && out && n >= 0 && n % 8 == 0, MMAE_ERR_ARG, "mmae_add_bf16_f32: bad args (n %% 8)");
+  MMAE_CHECK(x || row_scale, MMAE_ERR_ARG, "mmae_add_bf16_f32: null x");
+  MMAE_CHECK(!row_scale || (per_sample > 0 && per_sample % 8 == 0 && n % per_sample == 0), MMAE_ERR_ARG,
+             "mmae_add_bf16_f32: a row scale needs a multiple of 8 elements per sample dividing n");
   if (n == 0) return MMAE_OK;
   int64_t blocks = (n / 8 + 255) / 256;
   const int64_t cap = int64_t(sm_count()) * 16;
   if (blocks > cap) blocks = cap;
-  launch_k(add_bf16_f32_kernel, (unsigned)blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream), x, reinterpret_cast<const bf16*>(y_bf16), out, n);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (y_is_bf16)
+    launch_k(add_bf16_f32_kernel<true>, (unsigned)blocks, 256, 0, st, x, y, out, n, row_scale, per_sample);
+  else
+    launch_k(add_bf16_f32_kernel<false>, (unsigned)blocks, 256, 0, st, x, y, out, n, row_scale, per_sample);
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;
+}
+
+extern "C" int mmae_add_bf16_f32(const float* x, const void* y_bf16, float* out, int64_t n, void* stream) {
+  MMAE_CHECK(x, MMAE_ERR_ARG, "mmae_add_bf16_f32: bad args (n %% 8)");
+  return add_scaled_f32(x, y_bf16, 1, nullptr, 1, out, n, stream);
 }
 
 extern "C" int mmae_dgelu_colsum_bf16(const void* z, void* dz, int64_t ld, float* colsum, int M, int N, void* stream) {

@@ -21,13 +21,17 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
                                                                const float* __restrict__ beta, bf16* __restrict__ y_bf16,
                                                                int64_t ldy, float* __restrict__ y_f32, int64_t ldyf,
                                                                float* __restrict__ mean_out,
-                                                               float* __restrict__ rstd_out, int M, float eps) {
+                                                               float* __restrict__ rstd_out,
+                                                               const float* __restrict__ add_scale, int rows_per_sample,
+                                                               int M, float eps) {
   pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * LN_WARPS + warp;
   if (row >= M) return;
   constexpr int D = NVEC * 128;
   const float* xr = x + int64_t(row) * ldx;
+  // per-sample factor of the addend (stochastic depth: 0 or 1/keep); 1 when none is given, which leaves x + a exact
+  const float sc = add_scale != nullptr ? __ldg(add_scale + row / rows_per_sample) : 1.0f;
   float4 v[NVEC];
   float s = 0.f;
 #pragma unroll
@@ -37,7 +41,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
     if (addend != nullptr) {   // residual add fused in front of the normalisation: x <- x + bf16 branch output
       const uint2 u = __ldg(reinterpret_cast<const uint2*>(addend + int64_t(row) * ldadd + c));
       const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-      v[i].x += a.x; v[i].y += a.y; v[i].z += b.x; v[i].w += b.y;
+      v[i].x += sc * a.x; v[i].y += sc * a.y; v[i].z += sc * b.x; v[i].w += sc * b.y;
       if (x_sum != nullptr) *reinterpret_cast<float4*>(x_sum + int64_t(row) * ldsum + c) = v[i];
     }
     s += v[i].x + v[i].y + v[i].z + v[i].w;
@@ -126,7 +130,9 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
                                                                const float* __restrict__ dx_resid, int64_t ldr,
                                                                float* __restrict__ dx, int64_t lddx,
                                                                float* __restrict__ partial, bool want_colsum,
-                                                               bf16* __restrict__ dx_bf16, int64_t lddxb, int M) {
+                                                               bf16* __restrict__ dx_bf16, int64_t lddxb,
+                                                               const float* __restrict__ out_scale, int rows_per_sample,
+                                                               int M) {
   pdl_prologue();
   constexpr int D = NVEC * 128;
   __shared__ float4 red[LN_WARPS][32];
@@ -171,6 +177,8 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
       db[i].x += d.x; db[i].y += d.y; db[i].z += d.z; db[i].w += d.w;
     }
     const float c1 = warp_sum(s1) * (1.0f / D), c2 = warp_sum(s2) * (1.0f / D);
+    // per-sample factor of the bf16 copy and its column sums (the gradient entering a drop-path branch); dx stays unscaled
+    const float sc = out_scale != nullptr ? __ldg(out_scale + row / rows_per_sample) : 1.0f;
 #pragma unroll
     for (int i = 0; i < NVEC; ++i) {
       const int c = (i * 32 + lane) * 4;
@@ -190,10 +198,11 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
       *reinterpret_cast<float4*>(dx + int64_t(row) * lddx + c) = o;
       if (dx_bf16 != nullptr) {   // bf16 copy of dx (next GEMM operand) and its column sums (next bias gradient)
         uint2 pk;
-        pk.x = pack_bf16x2(o.x, o.y);
-        pk.y = pack_bf16x2(o.z, o.w);
+        const float4 os = make_float4(sc * o.x, sc * o.y, sc * o.z, sc * o.w);
+        pk.x = pack_bf16x2(os.x, os.y);
+        pk.y = pack_bf16x2(os.z, os.w);
         *reinterpret_cast<uint2*>(dx_bf16 + int64_t(row) * lddxb + c) = pk;
-        cs[i].x += o.x; cs[i].y += o.y; cs[i].z += o.z; cs[i].w += o.w;
+        cs[i].x += os.x; cs[i].y += os.y; cs[i].z += os.z; cs[i].w += os.w;
       }
     }
     cur = nxt;
@@ -232,8 +241,11 @@ using namespace mmae;
 
 static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, float* x_sum, int64_t ldsum,
                            const float* gamma, const float* beta, void* y_bf16, int64_t ldy, float* y_f32, int64_t ldyf,
-                           float* mean, float* rstd, int M, int D, float eps, void* stream) {
+                           float* mean, float* rstd, const float* add_scale, int rows_per_sample, int M, int D, float eps,
+                           void* stream) {
   MMAE_CHECK(x && gamma && beta && (y_bf16 || y_f32) && M > 0, MMAE_ERR_ARG, "mmae_layernorm_forward: bad args");
+  MMAE_CHECK(!add_scale || (addend && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
+             "mmae_add_layernorm_forward: a row scale needs an addend and rows-per-sample dividing M=%d", M);
   MMAE_CHECK(D % 128 == 0 && D <= 1024 && ldx % 4 == 0 && ldy % 4 == 0 && ldyf % 4 == 0, MMAE_ERR_UNSUPPORTED,
              "mmae_layernorm_forward: D=%d must be a multiple of 128 and <= 1024", D);
   dim3 grid(ceil_div(M, LN_WARPS)), block(LN_WARPS * 32);
@@ -242,7 +254,7 @@ static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int6
 #define LN_CASE(NV)                                                                                            \
   case NV:                                                                                                     \
     launch_k(ln_fwd_kernel<NV>, grid, block, 0, st, x, ldx, addend, ldadd, x_sum, ldsum, gamma, beta, yb, ldy, y_f32, ldyf, \
-                                              mean, rstd, M, eps);                                            \
+                                              mean, rstd, add_scale, rows_per_sample, M, eps);                                          \
     break;
   switch (D / 128) {
     LN_CASE(1) LN_CASE(2) LN_CASE(3) LN_CASE(4) LN_CASE(5) LN_CASE(6) LN_CASE(7) LN_CASE(8)
@@ -257,24 +269,36 @@ static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int6
 extern "C" int mmae_layernorm_forward(const float* x, int64_t ldx, const float* gamma, const float* beta, void* y_bf16,
                                       int64_t ldy, float* y_f32, int64_t ldyf, float* mean, float* rstd, int M, int D,
                                       float eps, void* stream) {
-  return ln_forward_impl(x, ldx, nullptr, 0, nullptr, 0, gamma, beta, y_bf16, ldy, y_f32, ldyf, mean, rstd, M, D, eps, stream);
+  return ln_forward_impl(x, ldx, nullptr, 0, nullptr, 0, gamma, beta, y_bf16, ldy, y_f32, ldyf, mean, rstd, nullptr, 1, M, D,
+                         eps, stream);
 }
 
 // x_sum = x + addend (fp32, written when non-NULL), then LayerNorm of x_sum: the residual add of
 // `x = x + attn(...)` (multimae/multimae_utils.py:230) fused in front of the next norm (:231)
+// x_sum = x + row_scale[row / rows_per_sample] * addend: the same with a per-sample factor on the branch (stochastic depth)
+int mmae::add_layernorm_forward_scaled(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, const float* row_scale,
+                                       int rows_per_sample, float* x_sum, int64_t ldsum, const float* gamma, const float* beta,
+                                       bf16* y_bf16, int64_t ldy, float* mean, float* rstd, int M, int D, float eps,
+                                       void* stream) {
+  MMAE_CHECK(addend && ldadd % 4 == 0 && (!x_sum || ldsum % 4 == 0), MMAE_ERR_ARG, "mmae_add_layernorm_forward: bad args");
+  return ln_forward_impl(x, ldx, addend, ldadd, x_sum, ldsum, gamma, beta, y_bf16, ldy, nullptr, 0, mean, rstd, row_scale,
+                         rows_per_sample, M, D, eps, stream);
+}
+
 extern "C" int mmae_add_layernorm_forward(const float* x, int64_t ldx, const void* addend_bf16, int64_t ldadd, float* x_sum,
                                           int64_t ldsum, const float* gamma, const float* beta, void* y_bf16, int64_t ldy,
                                           float* mean, float* rstd, int M, int D, float eps, void* stream) {
-  MMAE_CHECK(addend_bf16 && ldadd % 4 == 0 && (!x_sum || ldsum % 4 == 0), MMAE_ERR_ARG, "mmae_add_layernorm_forward: bad args");
-  return ln_forward_impl(x, ldx, reinterpret_cast<const bf16*>(addend_bf16), ldadd, x_sum, ldsum, gamma, beta, y_bf16, ldy,
-                         nullptr, 0, mean, rstd, M, D, eps, stream);
+  return add_layernorm_forward_scaled(x, ldx, reinterpret_cast<const bf16*>(addend_bf16), ldadd, nullptr, 1, x_sum, ldsum,
+                                      gamma, beta, reinterpret_cast<bf16*>(y_bf16), ldy, mean, rstd, M, D, eps, stream);
 }
 
 static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx, const float* mean,
                             const float* rstd, const float* gamma, const float* dx_resid, int64_t ldr, float* dx,
-                            int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16, int64_t lddxb, float* dx_colsum, int M,
-                            int D, void* stream) {
+                            int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16, int64_t lddxb, float* dx_colsum,
+                            const float* out_scale, int rows_per_sample, int M, int D, void* stream) {
   MMAE_CHECK(dy && x && mean && rstd && gamma && dx && M > 0, MMAE_ERR_ARG, "mmae_layernorm_backward: bad args");
+  MMAE_CHECK(!out_scale || (dx_bf16 && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
+             "mmae_layernorm_backward_ex: a row scale needs the bf16 output and rows-per-sample dividing M=%d", M);
   MMAE_CHECK(D % 128 == 0 && D <= 1024 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0 && ldr % 4 == 0,
              MMAE_ERR_UNSUPPORTED, "mmae_layernorm_backward: D=%d must be a multiple of 128 and <= 1024", D);
   // one wave: resident blocks per SM follow from the register footprint of the per-lane column accumulators
@@ -293,10 +317,12 @@ static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const 
   case NV:                                                                                                        \
     if (dy_is_bf16)                                                                                               \
       launch_k(ln_bwd_kernel<NV, true>, grid, block, 0, st, dy, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx,     \
-                                                      lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb, M);   \
+                                                      lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb,     \
+                                                      out_scale, rows_per_sample, M);                            \
     else                                                                                                          \
       launch_k(ln_bwd_kernel<NV, false>, grid, block, 0, st, dy, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx,    \
-                                                       lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb, M);  \
+                                                       lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb,     \
+                                                       out_scale, rows_per_sample, M);                           \
     break;
   switch (D / 128) {
     LNB_CASE(1) LNB_CASE(2) LNB_CASE(3) LNB_CASE(4) LNB_CASE(5) LNB_CASE(6) LNB_CASE(7) LNB_CASE(8)
@@ -314,7 +340,19 @@ extern "C" int mmae_layernorm_backward(const void* dy, int dy_is_bf16, int64_t l
                                        int64_t ldr, float* dx, int64_t lddx, float* dgamma, float* dbeta, int M, int D,
                                        void* stream) {
   return ln_backward_impl(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta, nullptr, 0,
-                          nullptr, M, D, stream);
+                          nullptr, nullptr, 1, M, D, stream);
+}
+
+// the _ex form with bf16(dx) and its column sums multiplied by row_scale[row / rows_per_sample] (the fp32 dx is not): the
+// gradient entering a branch that stochastic depth scaled per sample, while dx itself continues down the residual path
+int mmae::layernorm_backward_ex_scaled(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx,
+                                       const float* mean, const float* rstd, const float* gamma, const float* dx_resid,
+                                       int64_t ldr, float* dx, int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16,
+                                       int64_t lddxb, float* dx_colsum, const float* row_scale, int rows_per_sample, int M,
+                                       int D, void* stream) {
+  MMAE_CHECK(!dx_bf16 || lddxb % 4 == 0, MMAE_ERR_ARG, "mmae_layernorm_backward_ex: bad bf16 leading dimension");
+  return ln_backward_impl(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta, dx_bf16,
+                          lddxb, dx_colsum, row_scale, rows_per_sample, M, D, stream);
 }
 
 // same, additionally emitting bf16(dx) and colsum += sum_rows(dx): the operand and bias gradient of the next Linear backward
@@ -322,7 +360,6 @@ extern "C" int mmae_layernorm_backward_ex(const void* dy, int dy_is_bf16, int64_
                                           const float* mean, const float* rstd, const float* gamma, const float* dx_resid,
                                           int64_t ldr, float* dx, int64_t lddx, float* dgamma, float* dbeta, void* dx_bf16,
                                           int64_t lddxb, float* dx_colsum, int M, int D, void* stream) {
-  MMAE_CHECK(!dx_bf16 || lddxb % 4 == 0, MMAE_ERR_ARG, "mmae_layernorm_backward_ex: bad bf16 leading dimension");
-  return ln_backward_impl(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta,
-                          reinterpret_cast<bf16*>(dx_bf16), lddxb, dx_colsum, M, D, stream);
+  return layernorm_backward_ex_scaled(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta,
+                                      reinterpret_cast<bf16*>(dx_bf16), lddxb, dx_colsum, nullptr, 1, M, D, stream);
 }

@@ -336,11 +336,14 @@ extern "C" int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hi
 // pass of its own.  `x_add` (bf16) != null: the block input is x_in + x_add, formed inside the first LayerNorm kernel and
 // written to `x_sum` (what backward gets as x_in).  `y_out` (bf16) != null: the MLP branch output goes there, x_out is not
 // written, and the block's output is x_mid (mmae_block_saved_x_mid) + y_out - the next block's (x_in, x_add).
+// Stochastic depth (mmae_block_forward_dp): s_attn / s_mlp [B] multiply the attention / MLP branch of each sample inside the
+// residual adds, s_prev [B] multiplies x_add (the previous block's MLP branch).  Null: factor 1, the plain block.
 static int block_forward_impl(const float* x_in, const bf16* x_add, float* x_sum, float* x_out, bf16* y_out, int B, int N,
-                              int D, int H, int hidden, float eps, const mmae_block_params* p, void* saved, void* ws,
-                              void* st) {
+                              int D, int H, int hidden, float eps, const float* s_attn, const float* s_mlp,
+                              const float* s_prev, const mmae_block_params* p, void* saved, void* ws, void* st) {
   MMAE_CHECK(x_in && (x_out || y_out) && (!x_add || x_sum) && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0,
              MMAE_ERR_ARG, "mmae_block_forward: bad args");
+  MMAE_CHECK(!s_prev || x_add, MMAE_ERR_ARG, "mmae_block_forward_dp: the previous block's scale needs x_add");
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(saved, B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, int64_t(3) * D * D, true, st));
@@ -353,7 +356,8 @@ static int block_forward_impl(const float* x_in, const bf16* x_add, float* x_sum
   bf16* y = w.g;   // [M, D] bf16 scratch (forward only)
   // x = x + attn(norm1(x))                                       multimae_utils.py:230
   if (x_add) {   // the previous block's `x = x + mlp(..)` (multimae_utils.py:231) fused in front of this block's norm1
-    RUN(mmae_add_layernorm_forward(x_in, D, x_add, D, x_sum, D, p->norm1_w, p->norm1_b, s.h1, D, s.mean1, s.rstd1, M, D, eps, st));
+    RUN(add_layernorm_forward_scaled(x_in, D, x_add, D, s_prev, N, x_sum, D, p->norm1_w, p->norm1_b, s.h1, D, s.mean1, s.rstd1,
+                                     M, D, eps, st));
     x_in = x_sum;
   } else {
     RUN(mmae_layernorm_forward(x_in, D, p->norm1_w, p->norm1_b, s.h1, D, nullptr, 0, s.mean1, s.rstd1, M, D, eps, st));
@@ -363,24 +367,33 @@ static int block_forward_impl(const float* x_in, const bf16* x_add, float* x_sum
                              1.0f / sqrtf((float)dh), st));
   RUN(linear_bf16(s.o, s.wproj, p->proj_b, y, M, D, D, st));
   // x = x + mlp(norm2(x))                                        multimae_utils.py:231  (add fused in front of norm2)
-  RUN(mmae_add_layernorm_forward(x_in, D, y, D, s.x_mid, D, p->norm2_w, p->norm2_b, s.h2, D, s.mean2, s.rstd2, M, D, eps, st));
+  RUN(add_layernorm_forward_scaled(x_in, D, y, D, s_attn, N, s.x_mid, D, p->norm2_w, p->norm2_b, s.h2, D, s.mean2, s.rstd2, M,
+                                   D, eps, st));
   RUN(linear_gelu(s.h2, s.w1, p->fc1_b, s.z, s.a, M, hidden, D, st));
   if (y_out) return linear_bf16(s.a, s.w2, p->fc2_b, y_out, M, D, hidden, st);   // the add is the next block's first kernel
   RUN(linear_bf16(s.a, s.w2, p->fc2_b, y, M, D, hidden, st));
-  RUN(mmae_add_bf16_f32(s.x_mid, y, x_out, int64_t(M) * D, st));
+  RUN(add_scaled_f32(s.x_mid, y, 1, s_mlp, int64_t(N) * D, x_out, int64_t(M) * D, st));
   return MMAE_OK;
 }
 
 extern "C" int mmae_block_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
                                   const mmae_block_params* p, void* saved, void* ws, void* st) {
   MMAE_CHECK(x_out, MMAE_ERR_ARG, "mmae_block_forward: bad args");
-  return block_forward_impl(x_in, nullptr, nullptr, x_out, nullptr, B, N, D, H, hidden, eps, p, saved, ws, st);
+  return block_forward_impl(x_in, nullptr, nullptr, x_out, nullptr, B, N, D, H, hidden, eps, nullptr, nullptr, nullptr, p,
+                            saved, ws, st);
 }
 extern "C" int mmae_block_forward_chain(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out,
                                         void* y_out_bf16, int B, int N, int D, int H, int hidden, float eps,
                                         const mmae_block_params* p, void* saved, void* ws, void* st) {
   return block_forward_impl(x_in, reinterpret_cast<const bf16*>(x_add_bf16), x_sum, x_out, reinterpret_cast<bf16*>(y_out_bf16),
-                            B, N, D, H, hidden, eps, p, saved, ws, st);
+                            B, N, D, H, hidden, eps, nullptr, nullptr, nullptr, p, saved, ws, st);
+}
+extern "C" int mmae_block_forward_dp(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
+                                     int B, int N, int D, int H, int hidden, float eps, const float* scale_attn,
+                                     const float* scale_mlp, const float* scale_prev, const mmae_block_params* p, void* saved,
+                                     void* ws, void* st) {
+  return block_forward_impl(x_in, reinterpret_cast<const bf16*>(x_add_bf16), x_sum, x_out, reinterpret_cast<bf16*>(y_out_bf16),
+                            B, N, D, H, hidden, eps, scale_attn, scale_mlp, scale_prev, p, saved, ws, st);
 }
 extern "C" float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H, int hidden) {
   return saved ? block_saved(saved, B, N, D, H, hidden).x_mid : nullptr;
@@ -390,11 +403,16 @@ extern "C" float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H
 // which also added its column sums to this block's fc2 bias gradient: the cast + column-sum pass is skipped.
 // `dx_in_b` (bf16) != null: the first LayerNorm's backward also writes bf16(dx_in) there and adds colsum(dx_in) to
 // `dx_in_colsum` - the PREVIOUS block's fc2 bias gradient - for that block's backward to start from.
+// Stochastic depth: the gradient entering a branch is s * (gradient of the residual stream), so s_mlp scales the MLP branch's
+// bf16 operand and fc2 bias gradient, s_attn the proj operand and bias gradient that LN2's backward emits, s_prev what LN1's
+// backward hands to the previous block.  The fp32 residual-path gradients (dx_mid, dx_in) are never scaled.
 static int block_backward_impl(const float* x_in, const float* dx_out, const bf16* dx_out_b, float* dx_in, bf16* dx_in_b,
-                               float* dx_in_colsum, int B, int N, int D, int H, int hidden, const mmae_block_params* p,
+                               float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* s_attn,
+                               const float* s_mlp, const float* s_prev, const mmae_block_params* p,
                                const mmae_block_grads* g, const void* saved, void* ws, void* st) {
   MMAE_CHECK(x_in && dx_out && dx_in && (!dx_in_b || dx_in_colsum) && p && g && saved && ws, MMAE_ERR_ARG,
              "mmae_block_backward: bad args");
+  MMAE_CHECK(!s_prev || dx_in_b, MMAE_ERR_ARG, "mmae_block_backward_dp: the previous block's scale needs dx_in_bf16");
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(const_cast<void*>(saved), B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, 0, false, st));
@@ -409,7 +427,7 @@ static int block_backward_impl(const float* x_in, const float* dx_out, const bf1
   // ---- MLP branch
   const bf16* gout = dx_out_b;
   if (!gout) {
-    RUN(mmae_cast_colsum_f32(dx_out, D, w.g, D, g->fc2_b, M, D, st));
+    RUN(cast_colsum_f32_scaled(dx_out, D, w.g, D, g->fc2_b, s_mlp, N, M, D, st));
     gout = w.g;
   }
   if (side) RUN(side_fork(st, 0));
@@ -419,8 +437,8 @@ static int block_backward_impl(const float* x_in, const float* dx_out, const bf1
   RUN(wgrad(w.big, hidden, s.h2, D, g->fc1_w, M, hidden, D, ws_st));
   RUN(dgrad_bf16(w.big, hidden, s.w1, nullptr, w.dh, M, hidden, D, st));
   // LN2 backward also emits bf16(dx_mid) and its column sums = operand and bias gradient of the proj backward
-  RUN(mmae_layernorm_backward_ex(w.dh, 1, D, s.x_mid, D, s.mean2, s.rstd2, p->norm2_w, dx_out, D, w.dx_mid, D, g->norm2_w,
-                                 g->norm2_b, g2, D, g->proj_b, M, D, st));
+  RUN(layernorm_backward_ex_scaled(w.dh, 1, D, s.x_mid, D, s.mean2, s.rstd2, p->norm2_w, dx_out, D, w.dx_mid, D, g->norm2_w,
+                                   g->norm2_b, g2, D, g->proj_b, s_attn, N, M, D, st));
   // ---- attention branch
   if (side) RUN(side_fork(st, 2));
   RUN(wgrad(g2, D, s.o, D, g->proj_w, M, D, D, ws_st));
@@ -433,8 +451,8 @@ static int block_backward_impl(const float* x_in, const float* dx_out, const bf1
   RUN(wgrad(dqkv, 3 * D, s.h1, D, g->qkv_w, M, 3 * D, D, ws_st));
   RUN(dgrad_bf16(dqkv, 3 * D, s.wqkv, nullptr, w.dh, M, 3 * D, D, st));
   if (dx_in_b)
-    RUN(mmae_layernorm_backward_ex(w.dh, 1, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
-                                   g->norm1_b, dx_in_b, D, dx_in_colsum, M, D, st));
+    RUN(layernorm_backward_ex_scaled(w.dh, 1, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
+                                     g->norm1_b, dx_in_b, D, dx_in_colsum, s_prev, N, M, D, st));
   else
     RUN(mmae_layernorm_backward(w.dh, 1, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
                                 g->norm1_b, M, D, st));
@@ -445,14 +463,25 @@ static int block_backward_impl(const float* x_in, const float* dx_out, const bf1
 extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H,
                                    int hidden, const mmae_block_params* p, const mmae_block_grads* g, const void* saved,
                                    void* ws, void* st) {
-  return block_backward_impl(x_in, dx_out, nullptr, dx_in, nullptr, nullptr, B, N, D, H, hidden, p, g, saved, ws, st);
+  return block_backward_impl(x_in, dx_out, nullptr, dx_in, nullptr, nullptr, B, N, D, H, hidden, nullptr, nullptr, nullptr, p,
+                             g, saved, ws, st);
 }
 extern "C" int mmae_block_backward_chain(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
                                          void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
                                          const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
                                          void* st) {
   return block_backward_impl(x_in, dx_out, reinterpret_cast<const bf16*>(dx_out_bf16), dx_in,
-                             reinterpret_cast<bf16*>(dx_in_bf16), dx_in_colsum, B, N, D, H, hidden, p, g, saved, ws, st);
+                             reinterpret_cast<bf16*>(dx_in_bf16), dx_in_colsum, B, N, D, H, hidden, nullptr, nullptr, nullptr,
+                             p, g, saved, ws, st);
+}
+extern "C" int mmae_block_backward_dp(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
+                                      void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
+                                      const float* scale_attn, const float* scale_mlp, const float* scale_prev,
+                                      const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
+                                      void* st) {
+  return block_backward_impl(x_in, dx_out, reinterpret_cast<const bf16*>(dx_out_bf16), dx_in,
+                             reinterpret_cast<bf16*>(dx_in_bf16), dx_in_colsum, B, N, D, H, hidden, scale_attn, scale_mlp,
+                             scale_prev, p, g, saved, ws, st);
 }
 
 extern "C" int mmae_set_wgrad_stream(int enable) {

@@ -177,10 +177,14 @@ extern "C" int64_t mmae_block_f32_workspace_bytes(int B, int N, int D, int H, in
   return (int64_t)block_ws_f(nullptr, B, N, D, H, hidden).bytes;
 }
 
-extern "C" int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                                      const mmae_block_params* p, void* saved, void* ws, void* st) {
+// Stochastic depth (the *_dp forms): s_attn / s_mlp [B] multiply each sample's attention / MLP branch.  With a factor the
+// branch GEMM writes the branch alone (w.g, unused otherwise in forward) and a row-scaled add forms the residual sum.
+static int block_f32_forward_impl(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
+                                  const float* s_attn, const float* s_mlp, const mmae_block_params* p, void* saved, void* ws,
+                                  void* st) {
   MMAE_CHECK(x_in && x_out && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0, MMAE_ERR_ARG, "mmae_block_f32_forward: bad args");
   const int M = B * N, dh = D / H;
+  const int64_t MD = int64_t(M) * D, ND = int64_t(N) * D;
   BlockSavedF s = block_saved_f(saved, B, N, D, H, hidden);
   BlockWsF w = block_ws_f(ws, B, N, D, H, hidden);
   // x = x + attn(norm1(x))                                        multimae_utils.py:230
@@ -188,32 +192,65 @@ extern "C" int mmae_block_f32_forward(const float* x_in, float* x_out, int B, in
   RUN(linear_f32x3_forward(s.h1, p->qkv_w, p->qkv_b, nullptr, s.qkv, M, 3 * D, D, w.sp.A, w.sp.B, st));
   RUN(mmae_attention_f32_forward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, s.lse, B, H, N, N, dh,
                                  1.0f / sqrtf((float)dh), st));
-  RUN(linear_f32x3_forward(s.o, p->proj_w, p->proj_b, x_in, s.x_mid, M, D, D, w.sp.A, w.sp.B, st));
+  if (s_attn) {
+    RUN(linear_f32x3_forward(s.o, p->proj_w, p->proj_b, nullptr, w.g, M, D, D, w.sp.A, w.sp.B, st));
+    RUN(add_scaled_f32(x_in, w.g, 0, s_attn, ND, s.x_mid, MD, st));
+  } else {
+    RUN(linear_f32x3_forward(s.o, p->proj_w, p->proj_b, x_in, s.x_mid, M, D, D, w.sp.A, w.sp.B, st));
+  }
   // x = x + mlp(norm2(x))                                         multimae_utils.py:231
   RUN(mmae_layernorm_forward(s.x_mid, D, p->norm2_w, p->norm2_b, nullptr, 0, s.h2, D, s.mean2, s.rstd2, M, D, eps, st));
   RUN(linear_f32x3_forward(s.h2, p->fc1_w, p->fc1_b, nullptr, s.z, M, hidden, D, w.sp.A, w.sp.B, st));
   RUN(gelu_f32(s.z, s.a, int64_t(M) * hidden, 0, st));
+  if (s_mlp) {
+    RUN(linear_f32x3_forward(s.a, p->fc2_w, p->fc2_b, nullptr, w.g, M, D, hidden, w.sp.A, w.sp.B, st));
+    return add_scaled_f32(s.x_mid, w.g, 0, s_mlp, ND, x_out, MD, st);
+  }
   RUN(linear_f32x3_forward(s.a, p->fc2_w, p->fc2_b, s.x_mid, x_out, M, D, hidden, w.sp.A, w.sp.B, st));
   return MMAE_OK;
 }
 
-extern "C" int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                                       const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+extern "C" int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
+                                      const mmae_block_params* p, void* saved, void* ws, void* st) {
+  return block_f32_forward_impl(x_in, x_out, B, N, D, H, hidden, eps, nullptr, nullptr, p, saved, ws, st);
+}
+extern "C" int mmae_block_f32_forward_dp(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
+                                         const float* scale_attn, const float* scale_mlp, const mmae_block_params* p,
+                                         void* saved, void* ws, void* st) {
+  return block_f32_forward_impl(x_in, x_out, B, N, D, H, hidden, eps, scale_attn, scale_mlp, p, saved, ws, st);
+}
+
+// Backward with factors: the branch's weight / input gradients are taken from a row-scaled copy of the residual-stream
+// gradient (w.g, unused otherwise in backward); the residual path itself carries the unscaled gradient.
+static int block_f32_backward_impl(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
+                                   const float* s_attn, const float* s_mlp, const mmae_block_params* p,
+                                   const mmae_block_grads* g, const void* saved, void* ws, void* st) {
   MMAE_CHECK(x_in && dx_out && dx_in && p && g && saved && ws, MMAE_ERR_ARG, "mmae_block_f32_backward: bad args");
   const int M = B * N, dh = D / H;
+  const int64_t MD = int64_t(M) * D, ND = int64_t(N) * D;
   BlockSavedF s = block_saved_f(const_cast<void*>(saved), B, N, D, H, hidden);
   BlockWsF w = block_ws_f(ws, B, N, D, H, hidden);
   // ---- MLP branch
-  RUN(linear_f32x3_wgrad(dx_out, s.a, g->fc2_w, g->fc2_b, M, D, hidden, w.sp.A, w.sp.B, st));
-  RUN(linear_f32x3_dgrad(dx_out, p->fc2_w, w.big, M, D, hidden, 0, w.sp.A, w.sp.B, st));        // d a  [M, hidden]
+  const float* g_mlp = dx_out;
+  if (s_mlp) {
+    RUN(add_scaled_f32(nullptr, dx_out, 0, s_mlp, ND, w.g, MD, st));
+    g_mlp = w.g;
+  }
+  RUN(linear_f32x3_wgrad(g_mlp, s.a, g->fc2_w, g->fc2_b, M, D, hidden, w.sp.A, w.sp.B, st));
+  RUN(linear_f32x3_dgrad(g_mlp, p->fc2_w, w.big, M, D, hidden, 0, w.sp.A, w.sp.B, st));         // d a  [M, hidden]
   RUN(gelu_f32(s.z, w.big, int64_t(M) * hidden, 1, st));                                          // dz = da * gelu'(z)
   RUN(linear_f32x3_wgrad(w.big, s.h2, g->fc1_w, g->fc1_b, M, hidden, D, w.sp.A, w.sp.B, st));
   RUN(linear_f32x3_dgrad(w.big, p->fc1_w, w.dh, M, hidden, D, 0, w.sp.A, w.sp.B, st));
   RUN(mmae_layernorm_backward(w.dh, 0, D, s.x_mid, D, s.mean2, s.rstd2, p->norm2_w, dx_out, D, w.dx_mid, D, g->norm2_w,
                               g->norm2_b, M, D, st));
   // ---- attention branch
-  RUN(linear_f32x3_wgrad(w.dx_mid, s.o, g->proj_w, g->proj_b, M, D, D, w.sp.A, w.sp.B, st));
-  RUN(linear_f32x3_dgrad(w.dx_mid, p->proj_w, w.d_o, M, D, D, 0, w.sp.A, w.sp.B, st));
+  const float* g_attn = w.dx_mid;
+  if (s_attn) {
+    RUN(add_scaled_f32(nullptr, w.dx_mid, 0, s_attn, ND, w.g, MD, st));
+    g_attn = w.g;
+  }
+  RUN(linear_f32x3_wgrad(g_attn, s.o, g->proj_w, g->proj_b, M, D, D, w.sp.A, w.sp.B, st));
+  RUN(linear_f32x3_dgrad(g_attn, p->proj_w, w.d_o, M, D, D, 0, w.sp.A, w.sp.B, st));
   RUN(mmae_attention_f32_backward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, w.d_o, D, s.lse, w.delta, w.big,
                                   3 * D, w.big + D, 3 * D, w.big + 2 * D, 3 * D, B, H, N, N, dh, 1.0f / sqrtf((float)dh), st));
   RUN(linear_f32x3_wgrad(w.big, s.h1, g->qkv_w, g->qkv_b, M, 3 * D, D, w.sp.A, w.sp.B, st));
@@ -221,6 +258,17 @@ extern "C" int mmae_block_f32_backward(const float* x_in, const float* dx_out, f
   RUN(mmae_layernorm_backward(w.dh, 0, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
                               g->norm1_b, M, D, st));
   return MMAE_OK;
+}
+
+extern "C" int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
+                                       const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+  return block_f32_backward_impl(x_in, dx_out, dx_in, B, N, D, H, hidden, nullptr, nullptr, p, g, saved, ws, st);
+}
+extern "C" int mmae_block_f32_backward_dp(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H,
+                                          int hidden, const float* scale_attn, const float* scale_mlp,
+                                          const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
+                                          void* st) {
+  return block_f32_backward_impl(x_in, dx_out, dx_in, B, N, D, H, hidden, scale_attn, scale_mlp, p, g, saved, ws, st);
 }
 
 // ================================================================================================ decoder head

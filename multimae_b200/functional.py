@@ -133,16 +133,45 @@ def _ret_grads(arena, names, params):
 # ---------------------------------------------------------------------------------------------------------------------
 # transformer block
 # ---------------------------------------------------------------------------------------------------------------------
+def drop_path_prob(block):
+    """Stochastic-depth rate that applies to `block` in this call: its DropPath rate in training mode, else 0."""
+    dp = getattr(block, "drop_path", None)
+    return float(dp.drop_prob or 0.0) if block.training and hasattr(dp, "drop_prob") else 0.0
+
+
+def drop_path_scales(blocks, batch, device):
+    """Per-sample factors of stochastic depth for one run of consecutive Blocks (multimae/multimae_utils.py:105-132).
+
+    Returns one entry per block: None when the block drops nothing in this call (eval mode or rate 0), else the pair
+    (s_attn, s_mlp) of fp32 [batch] tensors, s = floor(keep + u) / keep with keep = 1 - p and u ~ U[0, 1): 0 for a dropped
+    sample, 1/keep for a kept one.  All draws come from ONE torch.rand on `device` (torch's CUDA generator), block by block,
+    the attention branch before the MLP branch; no host synchronisation, so it can be captured in a CUDA graph and every
+    replay draws anew."""
+    probs = [drop_path_prob(b) for b in blocks]
+    live = [i for i, p in enumerate(probs) if p > 0.0]
+    out = [None] * len(probs)
+    if not live:
+        return out
+    u = torch.rand((len(live), 2, batch), dtype=torch.float32, device=device)
+    for j, i in enumerate(live):
+        keep = 1.0 - probs[i]
+        s = u[j].add_(keep).floor_().div_(keep)
+        out[i] = (s[0], s[1])
+    return out
+
+
 BLOCK_PARAM_NAMES = ["norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight",
                      "attn.proj.bias", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias", "mlp.fc2.weight",
                      "mlp.fc2.bias"]
 
 
 class BlockFunction(torch.autograd.Function):
-    """Block.forward (multimae/multimae_utils.py:229-232) as one fused sequence of kernels."""
+    """Block.forward (multimae/multimae_utils.py:229-232) as one fused sequence of kernels.
+
+    `scales`: None, or the (s_attn, s_mlp) pair of drop_path_scales - then the *_dp entry points apply stochastic depth."""
 
     @staticmethod
-    def forward(ctx, x, meta, *params):
+    def forward(ctx, x, meta, scales, *params):
         _require_cuda(x, "Block")
         B, N, D = x.shape
         H, hidden, eps = meta["heads"], meta["hidden"], meta["eps"]
@@ -155,11 +184,21 @@ class BlockFunction(torch.autograd.Function):
         ws = Workspace.get(getattr(lib, "mmae_block%s_workspace_bytes" % f32)(B, N, D, H, hidden), x.device)
         out = torch.empty_like(x)
         prm = L.BlockParams(*[p.data_ptr() for p in params])
-        L.check(getattr(lib, "mmae_block%s_forward" % f32)(x.data_ptr(), out.data_ptr(), B, N, D, H, hidden, eps,
-                                                           ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                                           L.current_stream()), "mmae_block%s_forward" % f32)
+        if scales is None:
+            L.check(getattr(lib, "mmae_block%s_forward" % f32)(x.data_ptr(), out.data_ptr(), B, N, D, H, hidden, eps,
+                                                               ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
+                                                               L.current_stream()), "mmae_block%s_forward" % f32)
+        elif f32:
+            L.check(lib.mmae_block_f32_forward_dp(x.data_ptr(), out.data_ptr(), B, N, D, H, hidden, eps, scales[0].data_ptr(),
+                                                  scales[1].data_ptr(), ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
+                                                  L.current_stream()), "mmae_block_f32_forward_dp")
+        else:
+            L.check(lib.mmae_block_forward_dp(x.data_ptr(), None, None, out.data_ptr(), None, B, N, D, H, hidden, eps,
+                                              scales[0].data_ptr(), scales[1].data_ptr(), None, ctypes.byref(prm),
+                                              saved.data_ptr(), ws.data_ptr(), L.current_stream()), "mmae_block_forward_dp")
         ctx.meta = meta
         ctx.params = params
+        ctx.scales = scales
         ctx.save_for_backward(x, saved)
         return out
 
@@ -178,12 +217,25 @@ class BlockFunction(torch.autograd.Function):
         dx = torch.empty_like(x)
         prm = L.BlockParams(*[p.data_ptr() for p in params])
         grd = L.BlockGrads(*[_grad_ptr(arena, n) for n in names])
-        L.check(getattr(lib, "mmae_block%s_backward" % f32)(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), B, N, D, H, hidden,
-                                                            ctypes.byref(prm), ctypes.byref(grd), saved.data_ptr(),
-                                                            ws.data_ptr(), L.current_stream()), "mmae_block%s_backward" % f32)
+        sc = ctx.scales
+        if sc is None:
+            L.check(getattr(lib, "mmae_block%s_backward" % f32)(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), B, N, D, H,
+                                                                hidden, ctypes.byref(prm), ctypes.byref(grd),
+                                                                saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                    "mmae_block%s_backward" % f32)
+        elif f32:
+            L.check(lib.mmae_block_f32_backward_dp(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), B, N, D, H, hidden,
+                                                   sc[0].data_ptr(), sc[1].data_ptr(), ctypes.byref(prm), ctypes.byref(grd),
+                                                   saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                    "mmae_block_f32_backward_dp")
+        else:
+            L.check(lib.mmae_block_backward_dp(x.data_ptr(), dout.data_ptr(), None, dx.data_ptr(), None, None, B, N, D, H,
+                                               hidden, sc[0].data_ptr(), sc[1].data_ptr(), None, ctypes.byref(prm),
+                                               ctypes.byref(grd), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                    "mmae_block_backward_dp")
         if meta.get("on_grads_ready") is not None:
             meta["on_grads_ready"](names)
-        return (dx, None) + tuple(_ret_grads(arena, names, params))
+        return (dx, None, None) + tuple(_ret_grads(arena, names, params))
 
 
 class BlockStackFunction(torch.autograd.Function):
@@ -193,10 +245,15 @@ class BlockStackFunction(torch.autograd.Function):
     bf16 copy of the gradient and the fc2 bias gradient that block i's backward starts from.  n - 1 add passes and n - 1
     cast + column-sum passes less than n BlockFunctions; same arithmetic.
 
-    args: x, metas (one dict per block, as for BlockFunction), then the 12 BLOCK_PARAM_NAMES tensors of every block."""
+    Stochastic depth: `scales` holds one drop_path_scales entry per block.  When any is set, every block runs through
+    mmae_block_*_dp, block i+1 also receiving block i's s_mlp - the factor of the MLP branch it adds in front of its first
+    LayerNorm (forward) and of the bf16 gradient it hands down (backward); otherwise the calls are the plain _chain ones.
+
+    args: x, metas (one dict per block, as for BlockFunction), scales, then the 12 BLOCK_PARAM_NAMES tensors of every
+    block."""
 
     @staticmethod
-    def forward(ctx, x, metas, *params):
+    def forward(ctx, x, metas, scales, *params):
         _require_cuda(x, "Block")
         lib = L.lib()
         n, P = len(metas), len(BLOCK_PARAM_NAMES)
@@ -210,20 +267,28 @@ class BlockStackFunction(torch.autograd.Function):
         out = torch.empty_like(x)
         xs, saveds = [], []
         x_ptr, add_ptr = x.data_ptr(), None
+        dp = any(sc is not None for sc in scales)
         for i in range(n):
             last = i == n - 1
             saved = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             x_sum = torch.empty_like(x) if add_ptr is not None else None
             prm = L.BlockParams(*[p.data_ptr() for p in params[i * P:(i + 1) * P]])
-            L.check(lib.mmae_block_forward_chain(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
-                                                 None if last else y.data_ptr(), B, N, D, H, hidden, eps, ctypes.byref(prm),
-                                                 saved.data_ptr(), ws.data_ptr(), L.current_stream()),
-                    "mmae_block_forward_chain")
+            if dp:
+                s_attn, s_mlp, s_prev = _stack_scale_ptrs(scales, i)
+                L.check(lib.mmae_block_forward_dp(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
+                                                  None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
+                                                  s_prev, ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
+                                                  L.current_stream()), "mmae_block_forward_dp")
+            else:
+                L.check(lib.mmae_block_forward_chain(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
+                                                     None if last else y.data_ptr(), B, N, D, H, hidden, eps,
+                                                     ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
+                                                     L.current_stream()), "mmae_block_forward_chain")
             xs.append(x if x_sum is None else x_sum)
             saveds.append(saved)
             if not last:       # the next block's input: this block's x_mid (inside `saved`) + y
                 x_ptr, add_ptr = lib.mmae_block_saved_x_mid(saved.data_ptr(), B, N, D, H, hidden), y.data_ptr()
-        ctx.metas, ctx.params, ctx.dims = metas, params, (B, N, D, H, hidden)
+        ctx.metas, ctx.params, ctx.dims, ctx.scales = metas, params, (B, N, D, H, hidden), (scales if dp else None)
         ctx.save_for_backward(*xs, *saveds)
         return out
 
@@ -251,34 +316,51 @@ class BlockStackFunction(torch.autograd.Function):
             if i > 0:      # bf16(dx) + the fc2 bias gradient of the block below, from this block's first-LayerNorm backward
                 g_out = g_bufs[i % len(g_bufs)]
                 below_bias = _grad_ptr(metas[i - 1]["arena"], metas[i - 1]["prefix"] + "mlp.fc2.bias")
-            L.check(lib.mmae_block_backward_chain(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
-                                                  below_bias, B, N, D, H, hidden, ctypes.byref(prm), ctypes.byref(grd),
-                                                  saveds[i].data_ptr(), ws.data_ptr(), L.current_stream()),
-                    "mmae_block_backward_chain")
+            if ctx.scales is not None:
+                s_attn, s_mlp, s_prev = _stack_scale_ptrs(ctx.scales, i)
+                L.check(lib.mmae_block_backward_dp(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
+                                                   below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev, ctypes.byref(prm),
+                                                   ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
+                                                   L.current_stream()), "mmae_block_backward_dp")
+            else:
+                L.check(lib.mmae_block_backward_chain(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(),
+                                                      L.ptr(g_out), below_bias, B, N, D, H, hidden, ctypes.byref(prm),
+                                                      ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
+                                                      L.current_stream()), "mmae_block_backward_chain")
             if metas[i].get("on_grads_ready") is not None:
                 metas[i]["on_grads_ready"](names)       # fc2.bias of block i is complete: its column sums came from block i+1
             grads[i * P:(i + 1) * P] = _ret_grads(arena, names, blk)
             d, g_in = dx, g_out
-        return (d, None) + tuple(grads)
+        return (d, None, None) + tuple(grads)
 
 
-def block_stack(blocks, x):
+def _stack_scale_ptrs(scales, i):
+    """(s_attn, s_mlp, s_prev) device pointers of block i of a stack (None = factor 1); s_prev is block i-1's s_mlp."""
+    own = scales[i]
+    prev = scales[i - 1] if i > 0 else None
+    return (None if own is None else own[0].data_ptr(), None if own is None else own[1].data_ptr(),
+            None if prev is None else prev[1].data_ptr())
+
+
+def block_stack(blocks, x, fp32=False):
     """Run an nn.Sequential of multimae_utils.Block through BlockStackFunction when it applies (CUDA path, >= 2 blocks of
-    one shape bound to an arena, BLOCK_CHAIN on), else block by block."""
+    one shape bound to an arena, BLOCK_CHAIN on), else block by block (`fp32`: in the fp32 tier, always block by block).
+    The stochastic-depth factors of all blocks are drawn once, up front (drop_path_scales)."""
     blocks = list(blocks)
+    scales = drop_path_scales(blocks, x.shape[0], x.device)
     metas = [getattr(b, "_meta", None) for b in blocks]
-    ok = (BLOCK_CHAIN and len(blocks) >= 2 and all(m is not None and m["arena"].flat.device == x.device for m in metas)
+    ok = (BLOCK_CHAIN and not fp32 and len(blocks) >= 2
+          and all(m is not None and m["arena"].flat.device == x.device for m in metas)
           and not any(getattr(b, "_own_arena", False) for b in blocks)
-          and len({(b.dim, b.num_heads, b.hidden, b.norm1.eps) for b in blocks}) == 1
-          and all(b.chainable() for b in blocks))
+          and len({(b.dim, b.num_heads, b.hidden, b.norm1.eps) for b in blocks}) == 1)
     if not ok:
-        for b in blocks:
-            x = b(x)
+        for b, sc in zip(blocks, scales):
+            x = b.run(x, fp32=fp32, scales=sc)
         return x
     flat = []
     for b in blocks:
         flat += list(b._params())
-    return BlockStackFunction.apply(x, metas, *flat)
+    return BlockStackFunction.apply(x, metas, scales, *flat)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -1,5 +1,5 @@
 """Transformer building blocks with the reference's module / parameter names (multimae/multimae_utils.py), executing on
-the sm_90a kernels.  `Block` is the unit of execution (one fused forward / backward sequence); `Attention`, `Mlp` and
+the sm_90a kernels.  `Block` is the unit of execution (one fused forward / backward sequence, stochastic depth included); `Attention`, `Mlp` and
 `CrossAttention` are parameter containers with the reference constructor signatures so that `state_dict()` keys match
 (SURVEY.md §A.1)."""
 import math
@@ -36,8 +36,9 @@ def trunc_normal_(tensor, mean=0.0, std=1.0, a=-2.0, b=2.0):
 
 
 class DropPath(nn.Module):
-    """Stochastic depth.  Pre-training runs with drop_path = 0 (run_pretraining_multimae.py:162,289); a non-zero rate in
-    training mode is not on the accelerated path."""
+    """Stochastic depth (multimae/multimae_utils.py:105-132): holds `drop_prob` for its Block, which applies it per sample
+    inside the fused block kernels (residual adds and branch-gradient casts, functional.drop_path_scales).  No parameters;
+    repr and state_dict as the reference's."""
 
     def __init__(self, drop_prob=None):
         super().__init__()
@@ -46,7 +47,8 @@ class DropPath(nn.Module):
     def forward(self, x):
         if not self.drop_prob or not self.training:
             return x
-        raise NotImplementedError("multimae_b200: DropPath > 0 in training is outside the pre-training hot path")
+        raise NotImplementedError("multimae_b200: drop path is applied inside Block (the fused block kernels); "
+                                  "a stand-alone DropPath in training mode is not supported")
 
     def extra_repr(self):
         return "p={}".format(self.drop_prob)
@@ -121,14 +123,13 @@ class Block(nn.Module):
                 self.attn.proj.bias, self.norm2.weight, self.norm2.bias, self.mlp.fc1.weight, self.mlp.fc1.bias,
                 self.mlp.fc2.weight, self.mlp.fc2.bias)
 
-    def chainable(self):
-        """May this block run inside functional.BlockStackFunction (no stochastic depth to apply between the blocks)?"""
-        return not isinstance(self.drop_path, DropPath)
-
     def forward(self, x, fp32=False):
-        """`fp32`: run this block in the fp32 tier (a decoder block of an adapter listed in fp32_output_adapters)."""
-        if isinstance(self.drop_path, DropPath):
-            self.drop_path(x)  # raises in training when p > 0
+        """`fp32`: run this block in the fp32 tier (a decoder block of an adapter listed in fp32_output_adapters).  In
+        training mode with drop_path > 0 each call draws the per-sample factors of both residual branches."""
+        return self.run(x, fp32=fp32, scales=Fn.drop_path_scales([self], x.shape[0], x.device)[0])
+
+    def run(self, x, fp32=False, scales=None):
+        """One BlockFunction; `scales`: this block's entry of functional.drop_path_scales (None: no stochastic depth)."""
         if self._meta is None or self._meta["arena"].flat.device != x.device:
             # stand-alone use (outside MultiMAE): private gradient arena, zeroed on every forward
             self.bind(Fn.GradArena(list(self.named_parameters()), x.device), "")
@@ -136,4 +137,4 @@ class Block(nn.Module):
         if getattr(self, "_own_arena", False) and torch.is_grad_enabled():
             self._meta["arena"].zero_()
         meta = dict(self._meta, fp32=True) if fp32 else self._meta
-        return Fn.BlockFunction.apply(x, meta, *self._params())
+        return Fn.BlockFunction.apply(x, meta, scales, *self._params())

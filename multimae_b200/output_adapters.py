@@ -158,11 +158,8 @@ class SpatialOutputAdapter(nn.Module, _PosEmbCache):
             head_in = shared_ctx["ctx"]
             head_params = (None,) + head_params[1:]          # proj_context.weight: used and differentiated by the shared GEMM
         x = Fn.DecoderHeadFunction.apply(head_in, head_meta, ids_keep, ids_restore, *head_params, *task_embs)
-        if fp32 and isinstance(self.decoder_transformer, nn.Sequential):
-            for blk in self.decoder_transformer:
-                x = blk(x, fp32=True)
-        elif isinstance(self.decoder_transformer, nn.Sequential):
-            x = Fn.block_stack(self.decoder_transformer, x)
+        if isinstance(self.decoder_transformer, nn.Sequential):
+            x = Fn.block_stack(self.decoder_transformer, x, fp32=bool(fp32))
         else:
             x = self.decoder_transformer(x)
         tail_meta = dict(self._bound, nh=nh, nw=nw, channels=self.num_channels, patch=self.P_H, fp32=bool(fp32))
