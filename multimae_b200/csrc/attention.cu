@@ -141,6 +141,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __res
   for (int j = 0; j < DH / 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const float sl2 = scale * LOG2E;
+  const bool live = q0 + warp * 16 < Nq;
 
   for (int k0 = 0, it = 0; k0 < Nk; k0 += ATT_CHUNK, ++it) {
     const bf16* sK = sKb[it & 1];
@@ -155,66 +156,69 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __res
     }
     __syncthreads();
 
-    float s[ATT_CHUNK / 8][4];
+    // a warp whose 16 query rows all lie past Nq only stages chunks (decoder 196 queries: 3 of the last CTA's 4 warps)
+    if (live) {
+      float s[ATT_CHUNK / 8][4];
 #pragma unroll
-    for (int j = 0; j < ATT_CHUNK / 8; ++j) {
-      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+      for (int j = 0; j < ATT_CHUNK / 8; ++j) {
+        s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
 #pragma unroll
-      for (int kk = 0; kk < DH / 16; ++kk) {
-        uint32_t bfr[2];
-        load_b_frag(bfr, sK, LDS, j * 8, kk * 16, g, t);
-        mma_bf16_16816(s[j], qa[kk], bfr);
+        for (int kk = 0; kk < DH / 16; ++kk) {
+          uint32_t bfr[2];
+          load_b_frag(bfr, sK, LDS, j * 8, kk * 16, g, t);
+          mma_bf16_16816(s[j], qa[kk], bfr);
+        }
       }
-    }
-    // mask padded keys, running max
-    float mx[2] = {m_run[0], m_run[1]};
+      // mask padded keys, running max
+      float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
-    for (int j = 0; j < ATT_CHUNK / 8; ++j) {
-      const int key = k0 + j * 8 + 2 * t;
-      if (key >= Nk) s[j][0] = s[j][2] = -INFINITY;
-      if (key + 1 >= Nk) s[j][1] = s[j][3] = -INFINITY;
-      mx[0] = fmaxf(mx[0], fmaxf(s[j][0], s[j][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[j][2], s[j][3]));
-    }
+      for (int j = 0; j < ATT_CHUNK / 8; ++j) {
+        const int key = k0 + j * 8 + 2 * t;
+        if (key >= Nk) s[j][0] = s[j][2] = -INFINITY;
+        if (key + 1 >= Nk) s[j][1] = s[j][3] = -INFINITY;
+        mx[0] = fmaxf(mx[0], fmaxf(s[j][0], s[j][1]));
+        mx[1] = fmaxf(mx[1], fmaxf(s[j][2], s[j][3]));
+      }
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-    }
-    const float alpha0 = fast_exp2((m_run[0] - mx[0]) * sl2), alpha1 = fast_exp2((m_run[1] - mx[1]) * sl2);
-    m_run[0] = mx[0];
-    m_run[1] = mx[1];
-    const float mo0 = mx[0] * sl2, mo1 = mx[1] * sl2;
-    float rs0 = 0.f, rs1 = 0.f;
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      }
+      const float alpha0 = fast_exp2((m_run[0] - mx[0]) * sl2), alpha1 = fast_exp2((m_run[1] - mx[1]) * sl2);
+      m_run[0] = mx[0];
+      m_run[1] = mx[1];
+      const float mo0 = mx[0] * sl2, mo1 = mx[1] * sl2;
+      float rs0 = 0.f, rs1 = 0.f;
 #pragma unroll
-    for (int j = 0; j < ATT_CHUNK / 8; ++j) {
-      s[j][0] = fast_exp2(s[j][0] * sl2 - mo0);
-      s[j][1] = fast_exp2(s[j][1] * sl2 - mo0);
-      s[j][2] = fast_exp2(s[j][2] * sl2 - mo1);
-      s[j][3] = fast_exp2(s[j][3] * sl2 - mo1);
-      rs0 += s[j][0] + s[j][1];
-      rs1 += s[j][2] + s[j][3];
-    }
-    l_run[0] = l_run[0] * alpha0 + rs0;
-    l_run[1] = l_run[1] * alpha1 + rs1;
+      for (int j = 0; j < ATT_CHUNK / 8; ++j) {
+        s[j][0] = fast_exp2(s[j][0] * sl2 - mo0);
+        s[j][1] = fast_exp2(s[j][1] * sl2 - mo0);
+        s[j][2] = fast_exp2(s[j][2] * sl2 - mo1);
+        s[j][3] = fast_exp2(s[j][3] * sl2 - mo1);
+        rs0 += s[j][0] + s[j][1];
+        rs1 += s[j][2] + s[j][3];
+      }
+      l_run[0] = l_run[0] * alpha0 + rs0;
+      l_run[1] = l_run[1] * alpha1 + rs1;
 #pragma unroll
-    for (int j = 0; j < DH / 8; ++j) {
-      acc[j][0] *= alpha0; acc[j][1] *= alpha0;
-      acc[j][2] *= alpha1; acc[j][3] *= alpha1;
-    }
-    // O += P V
+      for (int j = 0; j < DH / 8; ++j) {
+        acc[j][0] *= alpha0; acc[j][1] *= alpha0;
+        acc[j][2] *= alpha1; acc[j][3] *= alpha1;
+      }
+      // O += P V
 #pragma unroll
-    for (int ks = 0; ks < ATT_CHUNK / 16; ++ks) {
-      uint32_t pa[4];
-      pa[0] = pack_bf16x2(s[2 * ks][0], s[2 * ks][1]);
-      pa[1] = pack_bf16x2(s[2 * ks][2], s[2 * ks][3]);
-      pa[2] = pack_bf16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
-      pa[3] = pack_bf16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
+      for (int ks = 0; ks < ATT_CHUNK / 16; ++ks) {
+        uint32_t pa[4];
+        pa[0] = pack_bf16x2(s[2 * ks][0], s[2 * ks][1]);
+        pa[1] = pack_bf16x2(s[2 * ks][2], s[2 * ks][3]);
+        pa[2] = pack_bf16x2(s[2 * ks + 1][0], s[2 * ks + 1][1]);
+        pa[3] = pack_bf16x2(s[2 * ks + 1][2], s[2 * ks + 1][3]);
 #pragma unroll
-      for (int jd = 0; jd < DH / 8; ++jd) {
-        uint32_t bfr[2];
-        load_b_frag_t(bfr, sV, LDS, ks * 16, jd * 8, g, t);
-        mma_bf16_16816(acc[jd], pa, bfr);
+        for (int jd = 0; jd < DH / 8; ++jd) {
+          uint32_t bfr[2];
+          load_b_frag_t(bfr, sV, LDS, ks * 16, jd * 8, g, t);
+          mma_bf16_16816(acc[jd], pa, bfr);
+        }
       }
     }
     __syncthreads();   // every warp is done with this buffer before the next iteration's prefetch overwrites it
@@ -511,7 +515,244 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const bf16* _
   }
 }
 
+// =====================================================================================================================
+// fused backward for Nk <= 256: one CTA per (b, h) owns every key, so each score tile is computed once (5 matmuls instead
+// of the 7 of the dQ + dK/dV pair above, and half the exp2) and dQ is written without atomics.
+//
+// Warp w owns keys [16w, 16w + 16) (keys padded to a multiple of 16, not 64); all of the head's K stays in shared memory
+// and the warp's V rows are held as A fragments.  Query
+// chunks of ATT_CHUNK rows (Q, dO, O, lse) stream through a cp.async double buffer.  Per chunk:
+//   A  delta = rowsum(dO * O) from the staged chunk (replaces attn_delta_kernel)
+//   B  every warp: S^T, dP^T for its keys, P and dS in registers, dV += P^T dO, dK += dS^T Q; dS^T (bf16) -> smem
+//   C  dQ(chunk) = dS K from smem, spread over the warps in 16 x 16 output tiles, stored straight to global
+// 16-query sub-tiles wholly past Nq are skipped.  Rows past Nq are zero-filled (Q = dO = O = 0, lse = 0): their P
+// multiplies dO = 0 and their dS is 0.  Keys past Nk have K = V = 0 and P forced to 0.
+// ptxas (sm_90a): 128 registers at dh 64, 124 at dh 32, no spills; the K A fragments are re-read from sK (which dQ needs
+// anyway) instead of being held, which is what keeps dh 64 within 128.  At the bench shapes the dynamic shared memory is
+// 88 KB (encoder, 7 warps: 2 CTAs per SM), 57 KB (decoder cross, 7 warps: 2) and 78 KB (decoder self, 13 warps: 1 CTA
+// per SM, register-bound; capping dh 32 at 72 registers for 2 spills, see the table below).
+// =====================================================================================================================
+constexpr int FB_MAX_KEYS = 256;
+constexpr int FB_LDD = ATT_CHUNK + 8;   // pitch of the dS^T tile [key][query] (144-byte rows: conflict-free ldmatrix)
+
+template <int DH>
+__host__ __device__ constexpr int fb_stream_elems() { return ATT_CHUNK * (DH + 8); }
+// dynamic shared memory: sK [Nkp][DH+8] | sdS [Nkp][FB_LDD] (V is staged here first) | 2 x (Q, dO, O) | 2 x lse | delta
+template <int DH>
+__host__ __device__ constexpr size_t fb_smem_bytes(int Nkp) {
+  return size_t(Nkp) * (DH + 8 + FB_LDD) * sizeof(bf16) + 6 * fb_stream_elems<DH>() * sizeof(bf16) +
+         3 * ATT_CHUNK * sizeof(float);
+}
+
+template <int DH>
+__device__ __forceinline__ void load_rows_async(bf16* s, const bf16* gbase, int64_t ld, int row0, int nrows, int rows_valid) {
+  constexpr int LDS = DH + 8, VPR = DH / 8;
+  for (int idx = threadIdx.x; idx < nrows * VPR; idx += blockDim.x) {
+    const int r = idx / VPR, cv = idx % VPR;
+    const bool ok = row0 + r < rows_valid;
+    cp_async_16(s + r * LDS + cv * 8, gbase + int64_t(ok ? row0 + r : 0) * ld + cv * 8, ok);
+  }
+}
+
+// A fragment (16 rows x 16 k) from smem stored transposed, s[k][row] (row contiguous)
+__device__ __forceinline__ void load_a_frag_t(uint32_t (&a)[4], const bf16* s, int ld, int row0, int k0, int lane) {
+  const int m = lane >> 3;
+  const bf16* p = s + (k0 + (lane & 7) + (m >> 1) * 8) * ld + row0 + (m & 1) * 8;
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3])
+               : "r"(smem_u32(p)));
+}
+
+template <int DH>
+__global__ void __launch_bounds__(FB_MAX_KEYS / 16 * 32) attn_bwd_fused_kernel(
+    const bf16* __restrict__ Q, int64_t ldq, const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V,
+    int64_t ldv, const bf16* __restrict__ O, int64_t ldo, const bf16* __restrict__ dO, int64_t lddo,
+    const float* __restrict__ lse, bf16* __restrict__ dQ, int64_t lddq, bf16* __restrict__ dK, int64_t lddk,
+    bf16* __restrict__ dV, int64_t lddv, int Nq, int Nk, int H, float scale) {
+  pdl_prologue();
+  constexpr int LDS = DH + 8, SE = fb_stream_elems<DH>();
+  static_assert(LDS <= FB_LDD, "V is staged in the dS^T tile");
+  extern __shared__ __align__(16) unsigned char fb_smem[];
+  const int nwarps = blockDim.x >> 5, Nkp = nwarps * 16;
+  bf16* sK = reinterpret_cast<bf16*>(fb_smem);
+  bf16* sdS = sK + Nkp * LDS;
+  bf16* sStream = sdS + Nkp * FB_LDD;               // [buf][Q | dO | O]
+  float* sLse = reinterpret_cast<float*>(sStream + 6 * SE);   // [buf][ATT_CHUNK]
+  float* sDel = sLse + 2 * ATT_CHUNK;
+
+  const int h = blockIdx.x % H, b = blockIdx.x / H;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const bf16* Qb = Q + int64_t(b) * Nq * ldq + h * DH;
+  const bf16* Kb = K + int64_t(b) * Nk * ldk + h * DH;
+  const bf16* Vb = V + int64_t(b) * Nk * ldv + h * DH;
+  const bf16* Ob = O + int64_t(b) * Nq * ldo + h * DH;
+  const bf16* dOb = dO + int64_t(b) * Nq * lddo + h * DH;
+  const float* Lp = lse + (int64_t(b) * H + h) * Nq;
+
+  auto issue_chunk = [&](int buf, int q0) {
+    bf16* s = sStream + buf * 3 * SE;
+    load_rows_async<DH>(s, Qb, ldq, q0, ATT_CHUNK, Nq);
+    load_rows_async<DH>(s + SE, dOb, lddo, q0, ATT_CHUNK, Nq);
+    load_rows_async<DH>(s + 2 * SE, Ob, ldo, q0, ATT_CHUNK, Nq);
+    for (int i = threadIdx.x; i < ATT_CHUNK; i += blockDim.x) {
+      const bool ok = q0 + i < Nq;
+      cp_async_4(&sLse[buf * ATT_CHUNK + i], Lp + (ok ? q0 + i : 0), ok);
+    }
+    cp_async_commit();
+  };
+  load_rows_async<DH>(sK, Kb, ldk, 0, Nkp, Nk);
+  load_rows_async<DH>(sdS, Vb, ldv, 0, Nkp, Nk);    // rows of pitch LDS inside the dS^T area, read once below
+  issue_chunk(0, 0);
+  cp_async_wait<0>();
+  __syncthreads();
+  uint32_t va[DH / 16][4];
+#pragma unroll
+  for (int kk = 0; kk < DH / 16; ++kk) load_a_frag(va[kk], sdS, LDS, warp * 16, kk * 16, g, t);
+  float dk[DH / 8][4], dv[DH / 8][4];
+#pragma unroll
+  for (int j = 0; j < DH / 8; ++j) {
+    dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = 0.f;
+    dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f;
+  }
+  const float sl2 = scale * LOG2E;
+  const bool key_a = warp * 16 + g < Nk, key_b = warp * 16 + g + 8 < Nk;
+
+  for (int q0 = 0, it = 0; q0 < Nq; q0 += ATT_CHUNK, ++it) {
+    const int buf = it & 1;
+    // the other buffer was last read before the previous chunk's dS^T barrier, and V before the first one
+    if (q0 + ATT_CHUNK < Nq) {
+      issue_chunk(buf ^ 1, q0 + ATT_CHUNK);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();   // chunk landed; every warp is done with the previous chunk's dS^T and delta
+    const bf16* sQ = sStream + buf * 3 * SE;
+    const bf16* sdO = sQ + SE;
+    const float* sL = sLse + buf * ATT_CHUNK;
+    // A: delta
+    for (int r = threadIdx.x; r < ATT_CHUNK; r += blockDim.x) {
+      const bf16* o = sQ + 2 * SE + r * LDS;
+      const bf16* d = sdO + r * LDS;
+      float p = 0.f;
+#pragma unroll
+      for (int c = 0; c < DH; c += 8) {
+        const uint4 ov = *reinterpret_cast<const uint4*>(o + c), dv4 = *reinterpret_cast<const uint4*>(d + c);
+        const uint32_t* ou = reinterpret_cast<const uint32_t*>(&ov);
+        const uint32_t* du = reinterpret_cast<const uint32_t*>(&dv4);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 x = unpack_bf16x2(ou[i]), y = unpack_bf16x2(du[i]);
+          p += x.x * y.x + x.y * y.y;
+        }
+      }
+      sDel[r] = p;
+    }
+    __syncthreads();
+    // B: S^T, dP^T, dV, dK for this warp's keys
+#pragma unroll
+    for (int qs = 0; qs < ATT_CHUNK / 16; ++qs) {
+      if (q0 + qs * 16 >= Nq) break;
+      uint32_t pa[4], dsa[4];
+      float s[2][4] = {}, dp[2][4] = {};
+#pragma unroll
+      for (int kk = 0; kk < DH / 16; ++kk) {
+        uint32_t ka[4];   // K fragments come from sK (kept for dQ) rather than registers: no spills at dh 64
+        load_a_frag(ka, sK, LDS, warp * 16, kk * 16, g, t);
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          uint32_t bq[2], bd[2];
+          load_b_frag(bq, sQ, LDS, qs * 16 + half * 8, kk * 16, g, t);
+          load_b_frag(bd, sdO, LDS, qs * 16 + half * 8, kk * 16, g, t);
+          mma_bf16_16816(s[half], ka, bq);       // S^T[key, q]
+          mma_bf16_16816(dp[half], va[kk], bd);  // dP^T[key, q]
+        }
+      }
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int qc = qs * 16 + half * 8 + 2 * t;
+        const float l0 = sL[qc] * LOG2E, l1 = sL[qc + 1] * LOG2E, d0 = sDel[qc], d1 = sDel[qc + 1];
+        const float p0 = key_a ? fast_exp2(s[half][0] * sl2 - l0) : 0.f, p1 = key_a ? fast_exp2(s[half][1] * sl2 - l1) : 0.f;
+        const float p2 = key_b ? fast_exp2(s[half][2] * sl2 - l0) : 0.f, p3 = key_b ? fast_exp2(s[half][3] * sl2 - l1) : 0.f;
+        pa[half * 2 + 0] = pack_bf16x2(p0, p1);
+        pa[half * 2 + 1] = pack_bf16x2(p2, p3);
+        dsa[half * 2 + 0] = pack_bf16x2(p0 * (dp[half][0] - d0), p1 * (dp[half][1] - d1));
+        dsa[half * 2 + 1] = pack_bf16x2(p2 * (dp[half][2] - d0), p3 * (dp[half][3] - d1));
+      }
+#pragma unroll
+      for (int jd = 0; jd < DH / 8; ++jd) {
+        uint32_t b1[2], b2[2];
+        load_b_frag_t(b1, sdO, LDS, qs * 16, jd * 8, g, t);
+        load_b_frag_t(b2, sQ, LDS, qs * 16, jd * 8, g, t);
+        mma_bf16_16816(dv[jd], pa, b1);    // dV += P^T dO
+        mma_bf16_16816(dk[jd], dsa, b2);   // dK += dS^T Q
+      }
+      bf16* r0 = sdS + (warp * 16 + g) * FB_LDD + qs * 16 + 2 * t;
+      *reinterpret_cast<uint32_t*>(r0) = dsa[0];
+      *reinterpret_cast<uint32_t*>(r0 + 8 * FB_LDD) = dsa[1];
+      *reinterpret_cast<uint32_t*>(r0 + 8) = dsa[2];
+      *reinterpret_cast<uint32_t*>(r0 + 8 * FB_LDD + 8) = dsa[3];
+    }
+    __syncthreads();
+    // C: dQ(chunk) = dS K, one 16-query x 16-column tile per warp at a time
+    for (int u = warp; u < (ATT_CHUNK / 16) * (DH / 16); u += nwarps) {
+      const int qt = u / (DH / 16), c0 = (u % (DH / 16)) * 16;
+      if (q0 + qt * 16 >= Nq) continue;
+      float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+      for (int ks = 0; ks < Nkp; ks += 16) {
+        uint32_t a[4], b0[2], b1[2];
+        load_a_frag_t(a, sdS, FB_LDD, qt * 16, ks, lane);
+        load_b_frag_t(b0, sK, LDS, ks, c0, g, t);
+        load_b_frag_t(b1, sK, LDS, ks, c0 + 8, g, t);
+        mma_bf16_16816(acc[0], a, b0);
+        mma_bf16_16816(acc[1], a, b1);
+      }
+      const int row_a = q0 + qt * 16 + g, row_b = row_a + 8;
+      bf16* dQb = dQ + int64_t(b) * Nq * lddq + h * DH;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int c = c0 + j * 8 + 2 * t;
+        if (row_a < Nq) *reinterpret_cast<uint32_t*>(dQb + int64_t(row_a) * lddq + c) = pack_bf16x2(acc[j][0] * scale, acc[j][1] * scale);
+        if (row_b < Nq) *reinterpret_cast<uint32_t*>(dQb + int64_t(row_b) * lddq + c) = pack_bf16x2(acc[j][2] * scale, acc[j][3] * scale);
+      }
+    }
+  }
+  const int row_a = warp * 16 + g, row_b = row_a + 8;
+  bf16* dKb = dK + int64_t(b) * Nk * lddk + h * DH;
+  bf16* dVb = dV + int64_t(b) * Nk * lddv + h * DH;
+#pragma unroll
+  for (int jd = 0; jd < DH / 8; ++jd) {
+    const int c = jd * 8 + 2 * t;
+    if (row_a < Nk) {
+      *reinterpret_cast<uint32_t*>(dKb + int64_t(row_a) * lddk + c) = pack_bf16x2(dk[jd][0] * scale, dk[jd][1] * scale);
+      *reinterpret_cast<uint32_t*>(dVb + int64_t(row_a) * lddv + c) = pack_bf16x2(dv[jd][0], dv[jd][1]);
+    }
+    if (row_b < Nk) {
+      *reinterpret_cast<uint32_t*>(dKb + int64_t(row_b) * lddk + c) = pack_bf16x2(dk[jd][2] * scale, dk[jd][3] * scale);
+      *reinterpret_cast<uint32_t*>(dVb + int64_t(row_b) * lddv + c) = pack_bf16x2(dv[jd][2], dv[jd][3]);
+    }
+  }
+}
+
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+template <int DH>
+int launch_bwd_fused(const bf16* q, int64_t ldq, const bf16* k, int64_t ldk, const bf16* v, int64_t ldv, const bf16* o,
+                     int64_t ldo, const bf16* d_o, int64_t lddo, const float* lse, bf16* dq, int64_t lddq, bf16* dk,
+                     int64_t lddk, bf16* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale, cudaStream_t st) {
+  auto kern = attn_bwd_fused_kernel<DH>;
+  static bool configured = false;
+  if (!configured) {
+    MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(fb_smem_bytes<DH>(FB_MAX_KEYS))));
+    configured = true;
+  }
+  const int nwarps = ceil_div(Nk, 16);
+  launch_k(kern, dim3(B * H), dim3(nwarps * 32), fb_smem_bytes<DH>(nwarps * 16), st, q, ldq, k, ldk, v, ldv, o, ldo, d_o,
+           lddo, lse, dq, lddq, dk, lddk, dv, lddv, Nq, Nk, H, scale);
+  count_launch();
+  MMAE_LAUNCH_OK();
+  return MMAE_OK;
+}
 
 }  // namespace
 }  // namespace mmae
@@ -522,14 +763,18 @@ using namespace mmae;
 // counterpart): 1 = wgmma forward (attention_wgmma.cu) for <= 128 keys; 2 | 8 | 32 | 128 = wgmma forward for 129..256 keys;
 // 4 | 64 = wgmma backward (any length); the forward above 256 keys and the backward without those bits use the warp-level
 // mma.sync kernels of this file (bit 16 selected a persistent variant that has no Hopper kernel and is ignored).
-// 0 = mma.sync kernels everywhere.
-// Default 0 (env MMAE_ATTN_TC), from scripts/gpu_time_attention.py and bench.py on one H100 80GB HBM3 capped at 400 W,
-// MultiMAE-B bs 128, us per call (forward mma.sync / wgmma, backward mma.sync / wgmma):
-//   encoder 99 x 99, dh 64      55.3 / 77.4    165.3 / 337.9
-//   decoder 196 x 99, dh 32     46.1 / 48.1    118.9 / 198.5
-//   decoder 196 x 196, dh 32    72.7 / 122.3   193.2 / 331.5
-// and the step: 44.5 ms (0), 47.8 ms (64: wgmma backward), 48.5 ms (195: wgmma forward + backward).  The wgmma kernels
-// stage every tile with plain loads and no pipelining.  A negative value restores the start-up default.
+// 0 = mma.sync kernels everywhere; their backward is the fused kernel up to 256 keys, delta + dQ + dK/dV above.
+// Default 0 (env MMAE_ATTN_TC), from scripts/gpu_time_attention.py on one H100 80GB HBM3 at a 700 W power limit,
+// MultiMAE-B bs 128, us per call (forward mma.sync / wgmma, backward mma.sync fused / wgmma; in brackets, from the same
+// run, the forward before idle warps skipped their work and the delta + dQ + dK/dV backward the fused kernel replaced):
+//   encoder 99 x 99, dh 64      46.8 (51.8) / 77.4    109.1 (155.4) / 340.1
+//   decoder 196 x 99, dh 32     43.9 (53.0) / 48.5     74.1 (115.5) / 198.8
+//   decoder 196 x 196, dh 32    65.6 (69.0) / 125.4   127.0 (180.1) / 333.1
+// The wgmma kernels stage every tile with plain loads and no pipelining.  Also measured and not kept (400 W limit): the
+// forward skipping the 16-key groups of its last key chunk that lie wholly past Nk (6 to 9 % slower at all three
+// shapes), and the fused backward capped at 72 registers at dh 32 for 2 CTAs per SM (it spills: decoder self 4 %
+// faster, decoder cross 8 % slower).
+// A negative value restores the start-up default.
 static int g_attn_tc = []() {
   const char* e = getenv("MMAE_ATTN_TC");
   return e ? atoi(e) : 0;
@@ -592,6 +837,13 @@ extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k
     MMAE_LAUNCH_OK();
     return attn_wg_backward(q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv, B, H, Nq, Nk,
                             head_dim, scale, st);
+  }
+  if (Nk <= FB_MAX_KEYS) {   // one fused kernel per (b, h); delta_ws is not used
+    if (head_dim == 64)
+      return launch_bwd_fused<64>(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, (bf16*)dq, lddq, (bf16*)dk, lddk,
+                                  (bf16*)dv, lddv, B, H, Nq, Nk, scale, st);
+    return launch_bwd_fused<32>(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, (bf16*)dq, lddq, (bf16*)dk, lddk,
+                                (bf16*)dv, lddv, B, H, Nq, Nk, scale, st);
   }
   if (head_dim == 64) {
     launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
