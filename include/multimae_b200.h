@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 6
+#define MMAE_ABI_VERSION 7
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -363,6 +363,25 @@ int mmae_dectail_forward(const float* x, int B, int nh, int nw, int Dd, int C, i
                          const float* out_b, float* pred, void* saved, void* ws, void* stream);
 int mmae_dectail_backward(const float* dpred, int B, int nh, int nw, int Dd, int C, int P, const float* out_w,
                           float* d_out_w, float* d_out_b, float* dx, const void* saved, void* ws, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Classification head of fine-tuning: LinearOutputAdapter.forward (multimae/output_adapters.py:345-356),
+ *   pooled = mean_pool ? x.mean(1) : x[:, N-1]   (mean over all N tokens, global token included; or the global token)
+ *   out    = LayerNorm(pooled) W^T + b           (W: [C, D] head.weight, b: [C]; fp32 LayerNorm statistics)
+ * x: [B, N, D] fp32 encoder output; out: [B, C] fp32 logits, or with C = 0 (head = nn.Identity) the fp32 LayerNorm output
+ * [B, D].  D must be a multiple of 8 (at most 8192); any C >= 0.  The head GEMM takes bf16 operands (the registered
+ * weight mirror when there is one) and accumulates in fp32.  Backward WRITES dx ([B, N, D]: dpooled / N on every token,
+ * or dpooled on token N-1 and zeros elsewhere) and ACCUMULATES (+=) the four parameter gradients.  `saved` (from
+ * forward to backward) and `ws` are sized by the *_bytes queries.  head_w / d_head_w / d_head_b may be NULL when C = 0.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t mmae_clshead_saved_bytes(int B, int N, int D, int C);
+int64_t mmae_clshead_workspace_bytes(int B, int N, int D, int C);
+int mmae_clshead_forward(const float* x, int B, int N, int D, int C, int mean_pool, float eps, const float* norm_w,
+                         const float* norm_b, const float* head_w, const float* head_b, float* out, void* saved, void* ws,
+                         void* stream);
+int mmae_clshead_backward(const float* dout, int B, int N, int D, int C, int mean_pool, const float* norm_w,
+                          const float* head_w, float* d_norm_w, float* d_norm_b, float* d_head_w, float* d_head_b,
+                          float* dx, const void* saved, void* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp32 tier for `fp32_output_adapters` (multimae/multimae.py:367-377: the listed output adapters run outside autocast;

@@ -211,6 +211,12 @@ SIGNATURES = {
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "mmae_clshead_saved_bytes": (c_i64, [c_int] * 4),
+    "mmae_clshead_workspace_bytes": (c_i64, [c_int] * 4),
+    "mmae_clshead_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_clshead_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     # ---- fp32 tier (fp32_output_adapters)
     "mmae_linear_f32_workspace_bytes": (c_i64, [c_int] * 3),
     "mmae_linear_f32_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -250,7 +256,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 
 def lib():

@@ -697,6 +697,66 @@ class DecoderTailFunction(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# classification head
+# ---------------------------------------------------------------------------------------------------------------------
+CLS_PARAM_NAMES = ["norm.weight", "norm.bias", "head.weight", "head.bias"]
+
+
+class ClsHeadFunction(torch.autograd.Function):
+    """LinearOutputAdapter.forward (multimae/output_adapters.py:345-356): token pool -> LayerNorm -> Linear as one call each
+    way (mmae_clshead_forward / _backward).
+
+    args: x [B, N, D], meta, norm.weight, norm.bias, head.weight, head.bias (both None when num_classes = 0).  meta: arena,
+    prefix, on_grads_ready, num_classes, mean_pool, eps, save (False: no backward will follow - the saved tensors live in
+    the stream's scratch buffer instead of a fresh allocation)."""
+
+    @staticmethod
+    def forward(ctx, x, meta, norm_w, norm_b, head_w, head_b):
+        _require_cuda(x, "LinearOutputAdapter")
+        lib = L.lib()
+        x = x.contiguous().float()
+        B, N, D = x.shape
+        C, mean_pool = meta["num_classes"], int(bool(meta["mean_pool"]))
+        out = torch.empty((B, C if C > 0 else D), dtype=torch.float32, device=x.device)
+        nsaved = lib.mmae_clshead_saved_bytes(B, N, D, C)
+        nws = lib.mmae_clshead_workspace_bytes(B, N, D, C)
+        if meta["save"]:
+            saved = torch.empty(nsaved, dtype=torch.uint8, device=x.device)
+            ws = Workspace.get(nws, x.device)
+            saved_ptr, ws_ptr = saved.data_ptr(), ws.data_ptr()
+        else:
+            ws = Workspace.get(nws + 256 + nsaved, x.device)
+            ws_ptr = ws.data_ptr()
+            saved, saved_ptr = None, (ws_ptr + nws + 255) // 256 * 256
+        L.check(lib.mmae_clshead_forward(x.data_ptr(), B, N, D, C, mean_pool, float(meta["eps"]), norm_w.data_ptr(),
+                                         norm_b.data_ptr(), L.ptr(head_w), L.ptr(head_b), out.data_ptr(), saved_ptr,
+                                         ws_ptr, L.current_stream()), "mmae_clshead_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, (B, N, D, C, mean_pool), (norm_w, norm_b, head_w, head_b)
+            ctx.save_for_backward(saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        (saved,) = ctx.saved_tensors
+        meta, params = ctx.meta, ctx.params
+        B, N, D, C, mean_pool = ctx.dims
+        arena, prefix = meta["arena"], meta["prefix"]
+        names = [prefix + n for n in CLS_PARAM_NAMES]
+        grd = [None if p is None else _grad_ptr(arena, n) for n, p in zip(names, params)]
+        ws = Workspace.get(lib.mmae_clshead_workspace_bytes(B, N, D, C), dout.device)
+        dout = dout.contiguous().float()
+        dx = torch.empty((B, N, D), dtype=torch.float32, device=dout.device)
+        L.check(lib.mmae_clshead_backward(dout.data_ptr(), B, N, D, C, mean_pool, params[0].data_ptr(), L.ptr(params[2]),
+                                          *grd, dx.data_ptr(), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_clshead_backward")
+        if meta.get("on_grads_ready") is not None:
+            meta["on_grads_ready"]([n for n, p in zip(names, params) if p is not None])
+        return (dx, None) + tuple(_ret_grads(arena, names, params))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # masked losses
 # ---------------------------------------------------------------------------------------------------------------------
 class MaskedLossFunction(torch.autograd.Function):

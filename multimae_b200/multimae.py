@@ -441,6 +441,8 @@ class MultiViT(MultiMAE):
         ids = torch.arange(total, device=dev).unsqueeze(0).expand(B, -1).contiguous()
         arena = self.grad_arena(dev)
         if torch.is_grad_enabled() and self.training:
+            if AUTO_OWN_GRADIENTS and not arena.owned:
+                self.own_gradients(True)
             arena.begin_step()
         seq = _embed(adapters, x, ids, self.global_tokens, arena, lambda d: "input_adapters.%s." % d, self._grad_callback)
         return seq, input_info

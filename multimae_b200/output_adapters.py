@@ -1,8 +1,10 @@
-"""SpatialOutputAdapter — the pre-training decoder — with the reference's constructor / state_dict / forward contract
-(multimae/output_adapters.py:33-282), executed as DecoderHeadFunction -> Block x depth -> DecoderTailFunction.
+"""Output adapters with the reference's constructor / state_dict / forward contract (multimae/output_adapters.py):
 
-The fine-tuning heads of the reference (Linear / Segmenter / ConvNeXt / DPT adapters) are outside the pre-training hot
-path (SURVEY.md §2.1 #4) and are not provided."""
+  SpatialOutputAdapter (:33-282) - the pre-training decoder, executed as DecoderHeadFunction -> Block x depth ->
+                                   DecoderTailFunction;
+  LinearOutputAdapter (:285-356) - the classification head of fine-tuning (run_finetuning_cls.py), one ClsHeadFunction.
+
+The dense fine-tuning heads of the reference (Segmenter / ConvNeXt / DPT adapters) are not provided."""
 from functools import partial
 from typing import Dict, Optional, Tuple, Union
 
@@ -164,3 +166,83 @@ class SpatialOutputAdapter(nn.Module, _PosEmbCache):
             x = self.decoder_transformer(x)
         tail_meta = dict(self._bound, nh=nh, nw=nw, channels=self.num_channels, patch=self.P_H, fp32=bool(fp32))
         return Fn.DecoderTailFunction.apply(x, tail_meta, self.out_proj.weight, self.out_proj.bias)
+
+
+class LinearOutputAdapter(nn.Module):
+    """Linear output adapter: head(norm(pool(encoder_tokens))), the pool being the mean over all tokens (global token
+    included) or the last token (the global token).  Runs as one functional.ClsHeadFunction (mmae_clshead_*)."""
+
+    def __init__(self, num_classes: int, dim_tokens_enc: Optional[int] = None, use_mean_pooling: bool = True,
+                 norm_layer: nn.Module = partial(nn.LayerNorm, eps=1e-6), init_scale: float = 1.0):
+        super().__init__()
+        self.num_classes = num_classes
+        self.dim_tokens_enc = dim_tokens_enc
+        self.use_mean_pooling = use_mean_pooling
+        self.norm_layer = norm_layer
+        self.init_scale = init_scale
+        self._bound = None
+        if self.dim_tokens_enc is not None:
+            self.init(dim_tokens_enc=dim_tokens_enc)
+
+    def init(self, dim_tokens_enc: int = 768):
+        """Build norm / head for encoder tokens of width dim_tokens_enc (called by MultiMAE.__init__).  A model that
+        re-initialises all its modules afterwards (MultiMAE._init_all_weights, like the reference's
+        multimae/multimae.py:100) overrides this trunc_normal / init_scale initialisation."""
+        self._forbid_rebuild()
+        self._bound = None
+        self.dim_tokens_enc = dim_tokens_enc
+        self.norm = self.norm_layer(self.dim_tokens_enc)
+        assert isinstance(self.norm, nn.LayerNorm), "multimae_b200: norm_layer must build nn.LayerNorm"
+        self.head = nn.Linear(dim_tokens_enc, self.num_classes) if self.num_classes > 0 else nn.Identity()
+        self.apply(self._init_weights)
+        if self.num_classes > 0:
+            self.head.weight.data.mul_(self.init_scale)
+            self.head.bias.data.mul_(self.init_scale)
+
+    def _forbid_rebuild(self):
+        if self._bound is not None and not getattr(self, "_own_arena", False):
+            raise RuntimeError("LinearOutputAdapter: the head cannot be rebuilt once the model's gradient arena exists "
+                               "(its gradient slots have the old shapes); reset the classifier before the first forward, "
+                               "or build a new model")
+
+    def _init_weights(self, m):
+        if isinstance(m, nn.Linear):
+            trunc_normal_(m.weight, std=.02)
+            if m.bias is not None:
+                nn.init.constant_(m.bias, 0)
+        elif isinstance(m, nn.LayerNorm):
+            nn.init.constant_(m.bias, 0)
+            nn.init.constant_(m.weight, 1.0)
+
+    def get_classifier(self):
+        return self.head
+
+    def reset_classifier(self, num_classes, global_pool=''):
+        """New head (and norm) for `num_classes`; raises once the model's gradient arena has been built."""
+        self._forbid_rebuild()
+        self.num_classes = num_classes
+        self.init(dim_tokens_enc=self.dim_tokens_enc)
+
+    def bind(self, arena, prefix, on_grads_ready=None):
+        self._own_arena = False
+        self._bound = dict(arena=arena, prefix=prefix, on_grads_ready=on_grads_ready)
+
+    def forward(self, encoder_tokens: torch.Tensor, **kwargs):
+        assert self.dim_tokens_enc is not None, "Need to call init(dim_tokens_enc) function first"
+        if not torch.is_tensor(encoder_tokens):
+            raise NotImplementedError("multimae_b200: LinearOutputAdapter takes the last layer's tokens "
+                                      "(return_all_layers=False)")
+        if self._bound is None or self._bound["arena"].flat.device != encoder_tokens.device:
+            # stand-alone use (outside MultiMAE / MultiViT): private gradient arena, zeroed on every training forward
+            self.bind(Fn.GradArena([(n, p) for n, p in self.named_parameters() if p.requires_grad],
+                                   encoder_tokens.device), "")
+            self._own_arena = True
+        params = (self.norm.weight, self.norm.bias) + ((self.head.weight, self.head.bias) if self.num_classes > 0
+                                                        else (None, None))
+        save = torch.is_grad_enabled() and (encoder_tokens.requires_grad or
+                                            any(p is not None and p.requires_grad for p in params))
+        if self._own_arena and save:
+            self._bound["arena"].zero_()
+        meta = dict(self._bound, num_classes=self.num_classes, mean_pool=self.use_mean_pooling, eps=self.norm.eps,
+                    save=save)
+        return Fn.ClsHeadFunction.apply(encoder_tokens, meta, *params)
