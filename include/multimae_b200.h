@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 7
+#define MMAE_ABI_VERSION 8
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -382,6 +382,43 @@ int mmae_clshead_forward(const float* x, int B, int N, int D, int C, int mean_po
 int mmae_clshead_backward(const float* dout, int B, int N, int D, int C, int mean_pool, const float* norm_w,
                           const float* head_w, float* d_norm_w, float* d_norm_b, float* d_head_w, float* d_head_b,
                           float* dx, const void* saved, void* ws, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Semantic-segmentation head of fine-tuning: ConvNeXtAdapter (multimae/output_adapters.py:481-573, ConvNeXtBlock in
+ * multimae/output_adapter_utils.py:19-57), split like SpatialOutputAdapter: proj -> block x depth -> tail.
+ * The feature map (Hf, Wf) = (nh*s, nw*s), s = sqrt(preds_per_patch), is held as the fp32 [P, C] view of the proj_dec output
+ * (P = B*nh*nw*s*s): row (b*n + t)*s*s + a*s + c' is pixel ((t / nw)*s + a, (t % nw)*s + c') of sample b, n = nh*nw.
+ * C must be a multiple of 128, at most 1024.  GEMMs take bf16 operands (registered weight mirrors when there are any) and
+ * accumulate in fp32.  Backward WRITES the activation gradient and ACCUMULATES (+=) the parameter gradients; the activation
+ * gradients and the depthwise-conv parameter gradients are computed without atomics (bitwise repeatable).  `saved` (from
+ * forward to backward) and `ws` are sized by the *_bytes queries.
+ * ---------------------------------------------------------------------------------------------- */
+/* proj: x[P, C] = cat_t(enc[:, start_t : start_t + n]) W^T + b  (enc [B, N, D] fp32, W [E, D*num_tasks], E = s*s*C).
+ * Backward writes denc [B, N, D] in full: zeros on the tokens of other tasks and on the global tokens. */
+int64_t mmae_convnext_proj_saved_bytes(int B, int n, int D_in, int E);
+int64_t mmae_convnext_proj_workspace_bytes(int B, int n, int D_in, int E);
+int mmae_convnext_proj_forward(const float* enc, int B, int N, int D, int n, int num_tasks, const int* start_host, int E,
+                               const float* w, const float* b, float* x_out, void* saved, void* ws, void* stream);
+int mmae_convnext_proj_backward(const float* dx_out, int B, int N, int D, int n, int num_tasks, const int* start_host, int E,
+                                const float* w, float* d_w, float* d_b, float* denc, const void* saved, void* ws, void* stream);
+/* block: x_out = x_in + pwconv2(GELU(pwconv1(LN(dwconv7x7(x_in)))))  (zero padding at the map borders).
+ * params_host / grads_host: host arrays of 8 device pointers, in this order: dwconv.weight [C, 1, 7, 7], dwconv.bias [C],
+ * norm.weight [C], norm.bias [C], pwconv1.weight [4C, C], pwconv1.bias [4C], pwconv2.weight [C, 4C], pwconv2.bias [C] */
+int64_t mmae_convnext_block_saved_bytes(int B, int nh, int nw, int s, int C);
+int64_t mmae_convnext_block_workspace_bytes(int B, int nh, int nw, int s, int C);
+int mmae_convnext_block_forward(const float* x_in, float* x_out, int B, int nh, int nw, int s, int C, float eps,
+                                const float* const* params_host, void* saved, void* ws, void* stream);
+int mmae_convnext_block_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int nh, int nw, int s, int C,
+                                 const float* const* params_host, float* const* grads_host, const void* saved, void* ws,
+                                 void* stream);
+/* tail: out [B, K, H, W] fp32 = bilinear(x W^T + b) (align_corners=False; W: final_layer.weight [K, C, 1, 1]); H, W must be
+ * integer multiples of Hf, Wf.  Any K >= 1. */
+int64_t mmae_convnext_tail_saved_bytes(int B, int nh, int nw, int s, int C, int K);
+int64_t mmae_convnext_tail_workspace_bytes(int B, int nh, int nw, int s, int C, int K);
+int mmae_convnext_tail_forward(const float* x, int B, int nh, int nw, int s, int C, int K, int H, int W, const float* w,
+                               const float* b, float* out, void* saved, void* ws, void* stream);
+int mmae_convnext_tail_backward(const float* dout, int B, int nh, int nw, int s, int C, int K, int H, int W, const float* w,
+                                float* d_w, float* d_b, float* dx, const void* saved, void* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp32 tier for `fp32_output_adapters` (multimae/multimae.py:367-377: the listed output adapters run outside autocast;

@@ -217,6 +217,25 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mmae_clshead_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_convnext_proj_saved_bytes": (c_i64, [c_int] * 4),
+    "mmae_convnext_proj_workspace_bytes": (c_i64, [c_int] * 4),
+    "mmae_convnext_proj_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_convnext_proj_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_convnext_block_saved_bytes": (c_i64, [c_int] * 5),
+    "mmae_convnext_block_workspace_bytes": (c_i64, [c_int] * 5),
+    "mmae_convnext_block_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float,
+                                            ctypes.POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
+    "mmae_convnext_block_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                             ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_void_p, c_void_p,
+                                             c_void_p]),
+    "mmae_convnext_tail_saved_bytes": (c_i64, [c_int] * 6),
+    "mmae_convnext_tail_workspace_bytes": (c_i64, [c_int] * 6),
+    "mmae_convnext_tail_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_convnext_tail_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     # ---- fp32 tier (fp32_output_adapters)
     "mmae_linear_f32_workspace_bytes": (c_i64, [c_int] * 3),
     "mmae_linear_f32_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -256,7 +275,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 def lib():

@@ -198,6 +198,8 @@ __global__ void __launch_bounds__(LN_THREADS) cls_head_bwd_kernel(const float* _
   }
 }
 
+}  // namespace
+
 // dst[i] += src[i]
 __global__ void add_f32_kernel(float* __restrict__ dst, const float* __restrict__ src, int64_t n) {
   pdl_prologue();
@@ -213,6 +215,8 @@ int add_f32(float* dst, const float* src, int64_t n, cudaStream_t st) {
   MMAE_LAUNCH_OK();
   return MMAE_OK;
 }
+
+namespace {
 
 int round8(int c) { return (c + 7) / 8 * 8; }
 

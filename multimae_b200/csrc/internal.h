@@ -73,5 +73,26 @@ int cast_colsum_f32_scaled(const float* src, int64_t ld_src, bf16* dst, int64_t 
 // fp32; x may be null (out = s * y, a scaled copy)
 int add_scaled_f32(const float* x, const void* y, int y_is_bf16, const float* row_scale, int64_t per_sample, float* out,
                    int64_t n, void* stream);
+// cls_head.cu: dst[i] += src[i] over n contiguous fp32 elements (any n)
+int add_f32(float* dst, const float* src, int64_t n, cudaStream_t st);
+
+// GEMM helpers of the module-level entry points (modules.cu): bf16 operands, fp32 accumulation through mmae_gemm_bf16.
+// bf16 operand of a weight: the registered mirror of the fp32 parameter buffer, else the per-call slot *slot (cast now when
+// cast_now; in backward the forward already cast it there)
+int weight_operand(const float* w, bf16** slot, int64_t n, bool cast_now, void* st);
+mmae_gemm_epilogue ep_zero();
+// y = x W^T + b (bf16 out), W: [N, K]
+int linear_bf16(const bf16* x, const bf16* W, const float* b, bf16* y, int M, int N, int K, void* st);
+// y = x W^T + b (+ resid) (fp32 out)
+int linear_f32(const bf16* x, const bf16* W, const float* b, const float* resid, float* y, int M, int N, int K, void* st);
+// z = x W^T + b (bf16, kept for backward), a = gelu(z) (bf16)
+int linear_gelu(const bf16* x, const bf16* W, const float* b, bf16* z, bf16* a, int M, int N, int K, void* st);
+// dx[M, Kin] = dy[M, Nout] W[Nout, Kin] (bf16 out, unsplit; optional * gelu'(z))
+int dgrad_bf16(const bf16* dy, int64_t lddy, const bf16* W, const bf16* dgelu_z, bf16* dx, int M, int Nout, int Kin, void* st);
+// dz = (dy W) * gelu'(z) and db += colsum(dz)
+int dgrad_dgelu_colsum(const bf16* dy, int64_t lddy, const bf16* W, const bf16* z, bf16* dz, float* db, int M, int Nout,
+                       int Kin, void* st);
+// dW[Nout, Kin] += dy[M, Nout]^T x[M, Kin]  (split-K chosen by mmae_gemm_bf16: fp32 atomics)
+int wgrad(const bf16* dy, int64_t lddy, const bf16* x, int64_t ldx, float* dW, int M, int Nout, int Kin, void* st);
 
 }  // namespace mmae

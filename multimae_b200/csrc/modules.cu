@@ -22,6 +22,11 @@ struct Carver {
   }
 };
 
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------- GEMM helpers
+// Shared with the other module-level entry points (declared in internal.h).
+
 // split-K count of the weight-gradient GEMMs: 0 = chosen by mmae_gemm_bf16 together with the tile width
 int pick_split(int, int, int) { return 0; }
 
@@ -119,6 +124,8 @@ int wgrad(const bf16* dy, int64_t lddy, const bf16* x, int64_t ldx, float* dW, i
   ep.ld_out_f32 = Kin;
   return mmae_gemm_bf16(dy, lddy, 1, x, ldx, 1, Nout, Kin, M, pick_split(Nout, Kin, M), &ep, st);
 }
+
+namespace {
 
 #define RUN(expr)             \
   do {                        \

@@ -757,6 +757,150 @@ class ClsHeadFunction(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# semantic-segmentation head (ConvNeXtAdapter): proj -> block x depth -> tail, each one call each way
+# ---------------------------------------------------------------------------------------------------------------------
+CONVNEXT_BLOCK_PARAM_NAMES = ["dwconv.weight", "dwconv.bias", "norm.weight", "norm.bias", "pwconv1.weight", "pwconv1.bias",
+                              "pwconv2.weight", "pwconv2.bias"]
+
+
+def _saved_and_ws(meta, nsaved, nws, device):
+    """`saved` as a fresh tensor kept for backward, or - under torch.no_grad() (meta["save"] False) - carved from the stream's
+    scratch buffer behind the workspace, so that nothing outlives the call."""
+    if meta["save"]:
+        saved = torch.empty(nsaved, dtype=torch.uint8, device=device)
+        return saved, saved.data_ptr(), Workspace.get(nws, device).data_ptr()
+    ws_ptr = Workspace.get(nws + 256 + nsaved, device).data_ptr()
+    return None, (ws_ptr + nws + 255) // 256 * 256, ws_ptr
+
+
+def _report(meta, names, params):
+    if meta.get("on_grads_ready") is not None:
+        meta["on_grads_ready"]([n for n, p in zip(names, params) if p is not None])
+    return _ret_grads(meta["arena"], names, params)
+
+
+class ConvNeXtProjFunction(torch.autograd.Function):
+    """Token gather + proj_dec of ConvNeXtAdapter.forward (multimae/output_adapters.py:545-562): encoder tokens [B, N, D] ->
+    the fp32 feature map as its [B*n*s*s, C] channels-last view (mmae_convnext_proj_*).
+
+    args: enc, meta, proj_dec.weight, proj_dec.bias.  meta: arena, prefix, on_grads_ready, save, n (tokens per task),
+    starts (first token of each main task), channels (C)."""
+
+    @staticmethod
+    def forward(ctx, enc, meta, weight, bias):
+        _require_cuda(enc, "ConvNeXtAdapter")
+        lib = L.lib()
+        enc = enc.contiguous().float()
+        B, N, D = enc.shape
+        n, starts, E = meta["n"], list(meta["starts"]), weight.shape[0]
+        arr = (ctypes.c_int * len(starts))(*starts)
+        saved, saved_ptr, ws_ptr = _saved_and_ws(meta, lib.mmae_convnext_proj_saved_bytes(B, n, D * len(starts), E),
+                                                 lib.mmae_convnext_proj_workspace_bytes(B, n, D * len(starts), E), enc.device)
+        out = torch.empty((B * n * E // meta["channels"], meta["channels"]), dtype=torch.float32, device=enc.device)
+        L.check(lib.mmae_convnext_proj_forward(enc.data_ptr(), B, N, D, n, len(starts), arr, E, weight.data_ptr(),
+                                               bias.data_ptr(), out.data_ptr(), saved_ptr, ws_ptr, L.current_stream()),
+                "mmae_convnext_proj_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, (B, N, D), (weight, bias)
+            ctx.save_for_backward(saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        (saved,) = ctx.saved_tensors
+        meta, (weight, bias) = ctx.meta, ctx.params
+        B, N, D = ctx.dims
+        n, starts, E = meta["n"], list(meta["starts"]), weight.shape[0]
+        arr = (ctypes.c_int * len(starts))(*starts)
+        names = [meta["prefix"] + "proj_dec.weight", meta["prefix"] + "proj_dec.bias"]
+        ws = Workspace.get(lib.mmae_convnext_proj_workspace_bytes(B, n, D * len(starts), E), dout.device)
+        dout = dout.contiguous().float()
+        denc = torch.empty((B, N, D), dtype=torch.float32, device=dout.device)
+        L.check(lib.mmae_convnext_proj_backward(dout.data_ptr(), B, N, D, n, len(starts), arr, E, weight.data_ptr(),
+                                                _grad_ptr(meta["arena"], names[0]), _grad_ptr(meta["arena"], names[1]),
+                                                denc.data_ptr(), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_convnext_proj_backward")
+        return (denc, None) + tuple(_report(meta, names, [weight, bias]))
+
+
+class ConvNeXtBlockFunction(torch.autograd.Function):
+    """ConvNeXtBlock.forward (multimae/output_adapter_utils.py:47-57, gamma None, drop_path 0) on the [P, C] view
+    (mmae_convnext_block_*).  args: x, meta (as ConvNeXtProjFunction plus nh, nw, s, eps; prefix ends in "blocks.<i>."),
+    then the 8 CONVNEXT_BLOCK_PARAM_NAMES tensors - the order of the entry points' pointer arrays."""
+
+    @staticmethod
+    def forward(ctx, x, meta, *params):
+        _require_cuda(x, "ConvNeXtAdapter")
+        lib = L.lib()
+        x = x.contiguous().float()
+        dims = (meta["B"], meta["nh"], meta["nw"], meta["s"], x.shape[1])
+        saved, saved_ptr, ws_ptr = _saved_and_ws(meta, lib.mmae_convnext_block_saved_bytes(*dims),
+                                                 lib.mmae_convnext_block_workspace_bytes(*dims), x.device)
+        out = torch.empty_like(x)
+        prm = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
+        L.check(lib.mmae_convnext_block_forward(x.data_ptr(), out.data_ptr(), *dims, float(meta["eps"]), prm,
+                                                saved_ptr, ws_ptr, L.current_stream()), "mmae_convnext_block_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, dims, params
+            ctx.save_for_backward(x, saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        x, saved = ctx.saved_tensors
+        meta, dims, params = ctx.meta, ctx.dims, ctx.params
+        names = [meta["prefix"] + n for n in CONVNEXT_BLOCK_PARAM_NAMES]
+        ws = Workspace.get(lib.mmae_convnext_block_workspace_bytes(*dims), dout.device)
+        dout = dout.contiguous().float()
+        dx = torch.empty_like(x)
+        prm = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
+        grd = (ctypes.c_void_p * len(names))(*[_grad_ptr(meta["arena"], n) for n in names])
+        L.check(lib.mmae_convnext_block_backward(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), *dims, prm, grd,
+                                                 saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_convnext_block_backward")
+        return (dx, None) + tuple(_report(meta, names, params))
+
+
+class ConvNeXtTailFunction(torch.autograd.Function):
+    """final_layer + bilinear upsample of ConvNeXtAdapter.forward (multimae/output_adapters.py:570-573): [P, C] ->
+    [B, K, H, W] fp32 (mmae_convnext_tail_*).  args: x, meta (plus num_classes, H, W), final_layer.weight, .bias."""
+
+    @staticmethod
+    def forward(ctx, x, meta, weight, bias):
+        _require_cuda(x, "ConvNeXtAdapter")
+        lib = L.lib()
+        x = x.contiguous().float()
+        K, H, W = meta["num_classes"], meta["H"], meta["W"]
+        dims = (meta["B"], meta["nh"], meta["nw"], meta["s"], x.shape[1], K)
+        saved, saved_ptr, ws_ptr = _saved_and_ws(meta, lib.mmae_convnext_tail_saved_bytes(*dims),
+                                                 lib.mmae_convnext_tail_workspace_bytes(*dims), x.device)
+        out = torch.empty((meta["B"], K, H, W), dtype=torch.float32, device=x.device)
+        L.check(lib.mmae_convnext_tail_forward(x.data_ptr(), *dims, H, W, weight.data_ptr(), bias.data_ptr(), out.data_ptr(),
+                                               saved_ptr, ws_ptr, L.current_stream()), "mmae_convnext_tail_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, dims, (weight, bias)
+            ctx.save_for_backward(saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        (saved,) = ctx.saved_tensors
+        meta, dims, (weight, bias) = ctx.meta, ctx.dims, ctx.params
+        names = [meta["prefix"] + "final_layer.weight", meta["prefix"] + "final_layer.bias"]
+        ws = Workspace.get(lib.mmae_convnext_tail_workspace_bytes(*dims), dout.device)
+        dout = dout.contiguous().float()
+        dx = torch.empty((dims[0] * dims[1] * dims[2] * dims[3] * dims[3], dims[4]), dtype=torch.float32, device=dout.device)
+        L.check(lib.mmae_convnext_tail_backward(dout.data_ptr(), *dims, meta["H"], meta["W"], weight.data_ptr(),
+                                                _grad_ptr(meta["arena"], names[0]), _grad_ptr(meta["arena"], names[1]),
+                                                dx.data_ptr(), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_convnext_tail_backward")
+        return (dx, None) + tuple(_report(meta, names, [weight, bias]))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # masked losses
 # ---------------------------------------------------------------------------------------------------------------------
 class MaskedLossFunction(torch.autograd.Function):

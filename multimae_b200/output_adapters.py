@@ -2,11 +2,15 @@
 
   SpatialOutputAdapter (:33-282) - the pre-training decoder, executed as DecoderHeadFunction -> Block x depth ->
                                    DecoderTailFunction;
-  LinearOutputAdapter (:285-356) - the classification head of fine-tuning (run_finetuning_cls.py), one ClsHeadFunction.
+  LinearOutputAdapter (:285-356) - the classification head of fine-tuning (run_finetuning_cls.py), one ClsHeadFunction;
+  ConvNeXtAdapter (:481-573)     - the semantic-segmentation head of fine-tuning (run_finetuning_semseg.py), executed as
+                                   ConvNeXtProjFunction -> ConvNeXtBlockFunction x depth -> ConvNeXtTailFunction.
 
-The dense fine-tuning heads of the reference (Segmenter / ConvNeXt / DPT adapters) are not provided."""
+SegmenterMaskTransformerAdapter and DPTOutputAdapter exist so that the fine-tuning scripts import; constructing either
+raises NotImplementedError."""
+import math
 from functools import partial
-from typing import Dict, Optional, Tuple, Union
+from typing import Dict, Iterable, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
@@ -246,3 +250,135 @@ class LinearOutputAdapter(nn.Module):
         meta = dict(self._bound, num_classes=self.num_classes, mean_pool=self.use_mean_pooling, eps=self.norm.eps,
                     save=save)
         return Fn.ClsHeadFunction.apply(encoder_tokens, meta, *params)
+
+
+class ConvNeXtBlock(nn.Module):
+    """ConvNeXt block (multimae/output_adapter_utils.py:19-57) as the adapter builds it: no layer scale (gamma None) and no
+    stochastic depth.  x + pwconv2(GELU(pwconv1(LN(dwconv(x))))); executed by functional.ConvNeXtBlockFunction."""
+
+    def __init__(self, dim):
+        super().__init__()
+        self.dwconv = nn.Conv2d(dim, dim, kernel_size=7, padding=3, groups=dim)
+        self.norm = nn.LayerNorm(dim, eps=1e-6)
+        self.pwconv1 = nn.Linear(dim, 4 * dim)
+        self.act = nn.GELU()
+        self.pwconv2 = nn.Linear(4 * dim, dim)
+        self.gamma = None
+        self.drop_path = nn.Identity()
+
+    def _params(self):
+        return (self.dwconv.weight, self.dwconv.bias, self.norm.weight, self.norm.bias, self.pwconv1.weight,
+                self.pwconv1.bias, self.pwconv2.weight, self.pwconv2.bias)
+
+
+class ConvNeXtAdapter(nn.Module):
+    """Output adapter with ConvNeXt blocks for semantic segmentation: proj_dec of the main tasks' tokens, reshaped into a
+    (nh*s) x (nw*s) map of embed_dim / preds_per_patch channels (s = sqrt(preds_per_patch)), `depth` ConvNeXt blocks, a 1x1
+    conv to num_classes and a bilinear upsample to the image size.  Extra keyword arguments (stride_level, ...) are
+    ignored, as by the reference.
+
+    The kernels keep the map as a [pixels, channels] matrix whose LayerNorm needs embed_dim / preds_per_patch to be a
+    multiple of 128 and at most 1024 (384 in every shipped semseg config); other widths raise here."""
+
+    def __init__(self, num_classes, embed_dim: int = 6144, preds_per_patch: int = 16, main_tasks: Iterable[str] = ('rgb',),
+                 patch_size: int = 16, depth: int = 4, interpolate_mode: str = 'bilinear', **kwargs):
+        super().__init__()
+        s = int(round(math.sqrt(preds_per_patch)))
+        if preds_per_patch <= 0 or s * s != preds_per_patch:
+            raise ValueError("ConvNeXtAdapter: preds_per_patch=%r must be a perfect square" % (preds_per_patch,))
+        if embed_dim % preds_per_patch != 0:
+            raise ValueError("ConvNeXtAdapter: embed_dim=%d is not divisible by preds_per_patch=%d"
+                             % (embed_dim, preds_per_patch))
+        class_dim = embed_dim // preds_per_patch
+        if class_dim % 128 != 0 or class_dim > 1024:
+            raise NotImplementedError(
+                "ConvNeXtAdapter: embed_dim / preds_per_patch = %d channels; the CUDA head needs a multiple of 128, at most "
+                "1024 (e.g. embed_dim=6144 with preds_per_patch=16)" % class_dim)
+        if interpolate_mode != 'bilinear':
+            raise NotImplementedError("ConvNeXtAdapter: interpolate_mode=%r; only 'bilinear' is implemented"
+                                      % (interpolate_mode,))
+        self.main_tasks = main_tasks
+        self.patch_size = patch_size
+        self.embed_dim = embed_dim
+        self.preds_per_patch = preds_per_patch
+        self.class_dim = class_dim
+        self.num_classes = num_classes
+        self.interpolate_mode = interpolate_mode
+        self._side = s
+        self._bound = None
+        self._own_arena = False
+
+        self.blocks = nn.Sequential(*[ConvNeXtBlock(dim=self.class_dim) for _ in range(depth)])
+        self.final_layer = nn.Conv2d(self.class_dim, self.num_classes, 1)
+        self.apply(self._init_weights)
+
+    def init(self, dim_tokens_enc: int = 768):
+        """Build proj_dec for encoder tokens of width dim_tokens_enc (called by MultiMAE.__init__)."""
+        self.in_channels = dim_tokens_enc * len(self.main_tasks)
+        self.proj_dec = nn.Linear(self.in_channels, self.embed_dim)
+        self._init_weights(self.proj_dec)
+        self._bound = None
+
+    def _init_weights(self, m):
+        if isinstance(m, nn.Linear):
+            trunc_normal_(m.weight, std=.02)
+            if m.bias is not None:
+                nn.init.constant_(m.bias, 0)
+        elif isinstance(m, nn.LayerNorm):
+            nn.init.constant_(m.bias, 0)
+            nn.init.constant_(m.weight, 1.0)
+
+    def bind(self, arena, prefix, on_grads_ready=None):
+        self._own_arena = False
+        self._bound = dict(arena=arena, prefix=prefix, on_grads_ready=on_grads_ready)
+
+    def forward(self, encoder_tokens: torch.Tensor, input_info: Dict):
+        assert hasattr(self, "proj_dec"), "Need to call init(dim_tokens_enc) function first"
+        if not torch.is_tensor(encoder_tokens):
+            raise NotImplementedError("multimae_b200: ConvNeXtAdapter takes the last layer's tokens "
+                                      "(return_all_layers=False)")
+        H, W = input_info['image_size']
+        nh, nw = H // self.patch_size, W // self.patch_size
+        for task in self.main_tasks:
+            n_t = input_info['tasks'][task]['end_idx'] - input_info['tasks'][task]['start_idx']
+            if n_t != nh * nw:
+                raise ValueError("ConvNeXtAdapter: task %r has %d tokens, the %dx%d image has %d x %d = %d patches of %d"
+                                 % (task, n_t, H, W, nh, nw, nh * nw, self.patch_size))
+        if self._bound is None or self._bound["arena"].flat.device != encoder_tokens.device:
+            # stand-alone use (outside MultiMAE / MultiViT): private gradient arena, zeroed on every training forward
+            self.bind(Fn.GradArena([(n, p) for n, p in self.named_parameters() if p.requires_grad],
+                                   encoder_tokens.device), "")
+            self._own_arena = True
+        params = [self.proj_dec.weight, self.proj_dec.bias, self.final_layer.weight, self.final_layer.bias]
+        for blk in self.blocks:
+            params += list(blk._params())
+        save = torch.is_grad_enabled() and (encoder_tokens.requires_grad or any(p.requires_grad for p in params))
+        if self._own_arena and save:
+            self._bound["arena"].zero_()
+        prefix = self._bound["prefix"]
+        base = dict(self._bound, save=save, B=encoder_tokens.shape[0], nh=nh, nw=nw, s=self._side)
+        starts = [input_info['tasks'][t]['start_idx'] for t in self.main_tasks]
+        x = Fn.ConvNeXtProjFunction.apply(encoder_tokens, dict(base, n=nh * nw, starts=starts, channels=self.class_dim),
+                                          self.proj_dec.weight, self.proj_dec.bias)
+        for i, blk in enumerate(self.blocks):
+            x = Fn.ConvNeXtBlockFunction.apply(x, dict(base, prefix="%sblocks.%d." % (prefix, i), eps=blk.norm.eps),
+                                               *blk._params())
+        return Fn.ConvNeXtTailFunction.apply(x, dict(base, num_classes=self.num_classes, H=H, W=W),
+                                             self.final_layer.weight, self.final_layer.bias)
+
+
+class SegmenterMaskTransformerAdapter(nn.Module):
+    """Placeholder so that the fine-tuning scripts import: the Segmenter head (multimae/output_adapters.py:359-478) is not
+    implemented on the CUDA path."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("multimae_b200: SegmenterMaskTransformerAdapter is not implemented; "
+                                  "use --output_adapter convnext")
+
+
+class DPTOutputAdapter(nn.Module):
+    """Placeholder so that the fine-tuning scripts import: the DPT head (multimae/output_adapters.py:576-) is not
+    implemented on the CUDA path."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("multimae_b200: DPTOutputAdapter is not implemented; use --output_adapter convnext")

@@ -4,9 +4,9 @@ so the reference's UNCHANGED run_pretraining_multimae.py drives the sm_90a path.
     python -m multimae_b200.overlay /path/to/MultiMAE/run_pretraining_multimae.py -c cfg.yaml [script args...]
 
 What is replaced (north_star "Subsystems replaced"): multimae.multimae, multimae.multimae_utils, multimae.input_adapters,
-multimae.output_adapters (SpatialOutputAdapter), multimae.criterion, utils.native_scaler.NativeScalerWithGradNormCount
-and — because the model owns its bucketed gradient all-reduce — torch.nn.parallel.DistributedDataParallel is substituted
-by an identity wrapper.  Everything else (argument parsing, data pipeline, optimizer factory, logging, checkpoints)
+multimae.output_adapters (SpatialOutputAdapter, LinearOutputAdapter, ConvNeXtAdapter), multimae.criterion,
+utils.native_scaler.NativeScalerWithGradNormCount and — because the model owns its bucketed gradient all-reduce —
+torch.nn.parallel.DistributedDataParallel is substituted by an identity wrapper.  Everything else (argument parsing, data pipeline, optimizer factory, logging, checkpoints)
 stays the reference's own code from `reference_root`."""
 import importlib
 import math
