@@ -1,15 +1,20 @@
 // wgmma / TMA GEMM for sm_90a:  C[M,N] = epilogue(alpha * A * B^T), bf16 operands, fp32 accumulate in registers.
 //
-// One CTA computes one 128 x BN output tile (BN = 64 / 128 / 192 / 256) over a K range (split-K along gridDim.z); three
+// Persistent: the grid holds at most one CTA (or two-CTA cluster) per SM, and each walks a fixed sequence of work items.
+// A work item is one 128 x BN output tile (BN = 64 / 128 / 192 / 256) over one K range (split-K).  CTA c of a grid of
+// g takes items c, c + g, c + 2g, ...; items are ordered n-tile fastest, then m-tile, then split, so the CTAs running
+// at the same time share their A rows (the large, token-sized operand) and the whole of B stays in L2.  Three
 // warpgroups:
 //   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled shared-memory ring, mbarrier
-//                    complete_tx); gives its registers to the consumers (setmaxnreg)
+//                    complete_tx); gives its registers to the consumers (setmaxnreg).  Ring slot and phase follow a
+//                    k-block count that runs across work items, so the next item's stages load during an epilogue.
 //   warpgroups 1-2 : consumers, 64 rows of the tile each: wgmma 64 x BN x 16 straight from the ring (K-major or MN-major
 //                    operands through the descriptor's transpose bit), then the fused epilogue from the accumulator
 //                    registers (bias / GELU / dGELU / residual, bf16 and fp32 outputs, red.global adds for split-K), or
-//                    for plain bf16 / fp32 outputs through shared memory and TMA tile stores / reduce-adds
+//                    for plain bf16 / fp32 outputs through a staging area of its own and TMA tile stores / reduce-adds
 // CL = 2: a cluster of two CTAs along M shares the B tile - each CTA loads half of it and multicasts it to both, so a
-// 256 x BN output tile reads B from L2 once.  A stage is refilled only after the consumers of BOTH CTAs released it.
+// 256 x BN output tile reads B from L2 once.  Both CTAs walk the same item sequence (one M-half each), so their rings
+// stay in lockstep; a stage is refilled only after the consumers of BOTH CTAs released it.
 //
 #include <algorithm>
 #include <cstdlib>
@@ -34,21 +39,43 @@ struct GemmParams {
   int M, N, K;
   int num_kb;        // total k-blocks (ceil(K / BK))
   int kb_per_split;  // k-blocks handled by one split
+  int tiles_n;       // ceil(N / BN)
+  int tiles_m;       // M units of one CTA (CL = 1) or one cluster (CL = 2): ceil(ceil(M / BM) / CL)
+  int splits;
   int tma_store;     // output through shared memory + TMA: 1 = bf16 store, 2 = fp32 store, 3 = fp32 reduce-add
   mmae_gemm_epilogue ep;
 };
 
-// ~192 KB of stages (BN = 64: 8 x 24 KB, 128: 6 x 32 KB, 192: 5 x 40 KB, 256: 4 x 48 KB).  One CTA per SM.
+// ~192 KB of stages (BN = 64: 8 x 24 KB, 128: 6 x 32 KB, 192: 4 x 40 KB, 256: 4 x 48 KB) + 32 KB of TMA-store staging
+// (per consumer warpgroup 16 KB: two 64 x 32 fp32 boxes or four bf16 boxes, used in turn).  One CTA per SM.
 template <int BN>
 struct GemmCfg {
-  static constexpr int STAGES = BN == 256 ? 4 : (BN == 192 ? 5 : (BN == 128 ? 6 : 8));
+  static constexpr int STAGES = BN == 256 ? 4 : (BN == 192 ? 4 : (BN == 128 ? 6 : 8));
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int EPI_BOX_BYTES = 64 * 32 * 4;
+  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = EPI_OFFSET + 2 * 2 * EPI_BOX_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // + barriers + alignment slack
   static_assert(TOTAL <= 232448, "GEMM exceeds the 227 KB shared-memory limit");
 };
+
+struct WorkItem {
+  int m0, n0, split, kb_begin, nkb;
+};
+
+template <int BN, int CL>
+__device__ __forceinline__ WorkItem decode_item(int item, const GemmParams& p, int rank) {
+  WorkItem w;
+  const int rest = item / p.tiles_n;
+  w.n0 = (item - rest * p.tiles_n) * BN;
+  w.split = rest / p.tiles_m;
+  w.m0 = ((rest - w.split * p.tiles_m) * CL + rank) * BM;
+  w.kb_begin = w.split * p.kb_per_split;
+  w.nkb = min(p.kb_per_split, p.num_kb - w.kb_begin);   // >= 1: the host never makes an empty split
+  return w;
+}
 
 __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
@@ -92,18 +119,20 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, int row, int n
     *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(ep.out_bf16) + int64_t(row) * ep.ld_out_bf16 + n) = pack_bf16x2(v0, v1);
 }
 
-// TMA-store staging: per consumer warpgroup, BN / 32 dense boxes of 64 rows x 32 columns
+// TMA-store staging: one dense box of 64 rows x 32 columns
 template <typename T>
-__device__ __forceinline__ void stage_pair(uint8_t* stage, int r, int c, float v0, float v1) {
-  T* box = reinterpret_cast<T*>(stage + (c >> 5) * (64 * 32 * sizeof(T)));
-  if constexpr (sizeof(T) == 4) *reinterpret_cast<float2*>(box + r * 32 + (c & 31)) = make_float2(v0, v1);
-  else *reinterpret_cast<uint32_t*>(box + r * 32 + (c & 31)) = pack_bf16x2(v0, v1);
+__device__ __forceinline__ void stage_pair(uint8_t* box, int r, int c, float v0, float v1) {
+  T* b = reinterpret_cast<T*>(box);
+  if constexpr (sizeof(T) == 4) *reinterpret_cast<float2*>(b + r * 32 + c) = make_float2(v0, v1);
+  else *reinterpret_cast<uint32_t*>(b + r * 32 + c) = pack_bf16x2(v0, v1);
 }
 
 template <int BN, int CL, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+  // the grid is never larger than what is co-resident (launch_gemm), so every item runs on a CTA that already holds its
+  // SM: a dependent kernel released here can only take SMs this grid does not use
   pdl_launch_dependents();   // the wait follows the barrier setup below
   using C = GemmCfg<BN>;
   constexpr int STAGES = C::STAGES;
@@ -118,12 +147,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
   const int wg = threadIdx.x >> 7;
   const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
-  const int n0 = blockIdx.x * BN;
-  const int m0 = blockIdx.y * BM;
-  const int kb_begin = blockIdx.z * p.kb_per_split;
-  int nkb = p.num_kb - kb_begin;
-  if (nkb > p.kb_per_split) nkb = p.kb_per_split;
-  if (nkb < 0) nkb = 0;
+  const int num_items = p.tiles_n * p.tiles_m * p.splits;
+  const int first_item = blockIdx.x / CL;
+  const int item_stride = gridDim.x / CL;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -144,35 +170,39 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % STAGES;
-        const uint32_t ph = (kb / STAGES) & 1;
-        mbar_wait(&empty_bar[s], ph ^ 1u);
-        mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
-        uint8_t* sA = smem + s * C::STAGE_BYTES;
-        uint8_t* sB = sA + C::A_BYTES;
-        const int k0 = (kb_begin + kb) * BK;
-        if constexpr (!A_MN) {
-          tma_load_2d(sA, &tmA, &full_bar[s], k0, m0);
-        } else {
-#pragma unroll
-          for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * (64 * BK * 2), &tmA, &full_bar[s], m0 + c * 64, k0);
-        }
-        if constexpr (CL == 1) {
-          if constexpr (!B_MN) {
-            tma_load_2d(sB, &tmB, &full_bar[s], k0, n0);
+      uint32_t it = 0;   // k-blocks loaded so far, over all items
+      for (int item = first_item; item < num_items; item += item_stride) {
+        const WorkItem w = decode_item<BN, CL>(item, p, rank);
+        for (int kb = 0; kb < w.nkb; ++kb, ++it) {
+          const int s = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait(&empty_bar[s], ph ^ 1u);
+          mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
+          uint8_t* sA = smem + s * C::STAGE_BYTES;
+          uint8_t* sB = sA + C::A_BYTES;
+          const int k0 = (w.kb_begin + kb) * BK;
+          if constexpr (!A_MN) {
+            tma_load_2d(sA, &tmA, &full_bar[s], k0, w.m0);
           } else {
 #pragma unroll
-            for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), &tmB, &full_bar[s], n0 + c * 64, k0);
+            for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * (64 * BK * 2), &tmA, &full_bar[s], w.m0 + c * 64, k0);
           }
-        } else {
-          if constexpr (!B_MN) {
-            tma_load_2d_multicast(sB + rank * BH * 128, &tmB, &full_bar[s], k0, n0 + rank * BH, 0x3);
-          } else {
+          if constexpr (CL == 1) {
+            if constexpr (!B_MN) {
+              tma_load_2d(sB, &tmB, &full_bar[s], k0, w.n0);
+            } else {
 #pragma unroll
-            for (int c = 0; c < BH / 64; ++c)
-              tma_load_2d_multicast(sB + (rank * (BH / 64) + c) * (64 * BK * 2), &tmB, &full_bar[s], n0 + rank * BH + c * 64,
-                                    k0, 0x3);
+              for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), &tmB, &full_bar[s], w.n0 + c * 64, k0);
+            }
+          } else {
+            if constexpr (!B_MN) {
+              tma_load_2d_multicast(sB + rank * BH * 128, &tmB, &full_bar[s], k0, w.n0 + rank * BH, 0x3);
+            } else {
+#pragma unroll
+              for (int c = 0; c < BH / 64; ++c)
+                tma_load_2d_multicast(sB + (rank * (BH / 64) + c) * (64 * BK * 2), &tmB, &full_bar[s],
+                                      w.n0 + rank * BH + c * 64, k0, 0x3);
+            }
           }
         }
       }
@@ -181,137 +211,169 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     // ------------------------------------------------------------------ consumers (warpgroups 1, 2)
     setmaxnreg_inc<232>();
     const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
-    float acc[BN / 2];   // written by the first wgmma (scale-d = 0); read only when nkb > 0
-
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % STAGES;
-      const uint32_t ph = (kb / STAGES) & 1;
-      mbar_wait(&full_bar[s], ph);
-      const uint32_t a_addr = smem_u32(smem + s * C::STAGE_BYTES) + cw * (64 * BK * 2);
-      const uint32_t b_addr = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-      wgmma_fence();
-#pragma unroll
-      for (int j = 0; j < BK / WG_K; ++j) {
-        const uint32_t sd = (kb | j) != 0 ? 1u : 0u;
-        // K-major : advance 16 elements (32 B) inside the 128 B swizzle row; this warpgroup's 64 rows start 8 KB in
-        // MN-major: advance 16 k-rows of 128 B; 64-element M/N chunks are (64 * BK * 2) bytes apart
-        const uint64_t da = A_MN ? gmma_desc_sw128(a_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
-                                 : gmma_desc_sw128(a_addr + j * (WG_K * 2), 16, 1024);
-        const uint64_t db = B_MN ? gmma_desc_sw128(b_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
-                                 : gmma_desc_sw128(b_addr + j * (WG_K * 2), 16, 1024);
-        if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-        else if constexpr (BN == 192) wgmma_m64n192k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-        else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-        else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-      }
-      wgmma_commit();
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-      wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
-      if (kb > 0 && (threadIdx.x & 127) == 0) {
-        const int rs = (kb - 1) % STAGES;
-        if constexpr (CL == 1) mbar_arrive(&empty_bar[rs]);
-        else
-          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty_bar[rs]), uint32_t(r)));
-      }
-    }
-    wgmma_wait<0>();
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-
     const int t = threadIdx.x & 127;
     const int rl = (t >> 5) * 16 + ((t & 31) >> 2);       // this thread's first row within the warpgroup's 64
-    const int row_a = m0 + cw * 64 + rl;
-    const int row_b = row_a + 8;
-    const bool first_split = blockIdx.z == 0;
-    if (nkb > 0 && p.tma_store) {
-      // ---------------------------------------------------------------- epilogue through shared memory + TMA
-      // both warpgroups have retired their last MMA before the ring is reused as the staging area
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      uint8_t* stage = smem + cw * (64 * BN * (p.tma_store == 1 ? 2 : 4));
-      const float* bias = first_split ? p.ep.bias : nullptr;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int c = j * 8 + 2 * (t & 3);
-        float v[4] = {acc[4 * j] * p.ep.alpha, acc[4 * j + 1] * p.ep.alpha, acc[4 * j + 2] * p.ep.alpha,
-                      acc[4 * j + 3] * p.ep.alpha};
-        if (bias && n0 + c < p.N) {
-          const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + n0 + c));
-          v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
-        }
-        if (p.ep.act == 1) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
-        }
-        if (p.tma_store == 1) {
-          stage_pair<bf16>(stage, rl, c, v[0], v[1]);
-          stage_pair<bf16>(stage, rl + 8, c, v[2], v[3]);
-        } else {
-          stage_pair<float>(stage, rl, c, v[0], v[1]);
-          stage_pair<float>(stage, rl + 8, c, v[2], v[3]);
-        }
-      }
-      fence_proxy_async_smem();
-      asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
+    uint8_t* epi = smem + C::EPI_OFFSET + cw * (2 * C::EPI_BOX_BYTES);
+    const bool atomic_out = p.ep.accumulate != 0 || p.splits > 1;
+    uint32_t it = 0;       // k-blocks consumed so far, over all items
+    uint32_t boxes = 0;    // TMA-store boxes issued so far by this warpgroup
+    // frees ring stage `s` in this CTA and, for a cluster, in the peer whose multicast also fills it
+    auto release = [&](int s) {
       if (t == 0) {
-        const int box_bytes = 64 * 32 * (p.tma_store == 1 ? 2 : 4);
-        for (int b = 0; b < BN / 32 && n0 + b * 32 < p.N; ++b) {
-          if (p.tma_store == 3) tma_reduce_add_2d(&tmC, stage + b * box_bytes, n0 + b * 32, m0 + cw * 64);
-          else tma_store_2d(&tmC, stage + b * box_bytes, n0 + b * 32, m0 + cw * 64);
-        }
-        bulk_commit_group();
-        bulk_wait_all();   // the stores have read the staging area before the CTA's shared memory goes away
+        if constexpr (CL == 1) mbar_arrive(&empty_bar[s]);
+        else
+          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty_bar[s]), uint32_t(r)));
       }
-    } else if (nkb > 0) {
-      // ---------------------------------------------------------------- epilogue straight from the accumulator registers
-      const bool atomic_out = p.ep.accumulate != 0 || gridDim.z > 1;
+    };
+    float acc[BN / 2];   // written by each item's first wgmma (scale-d = 0)
+
+    for (int item = first_item; item < num_items; item += item_stride) {
+      const WorkItem w = decode_item<BN, CL>(item, p, rank);
+      for (int kb = 0; kb < w.nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t a_addr = smem_u32(smem + s * C::STAGE_BYTES) + cw * (64 * BK * 2);
+        const uint32_t b_addr = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        if (n0 + j * 8 >= p.N) break;   // N % 8 == 0: a column pair is either fully inside or fully outside
-        const int n = n0 + j * 8 + 2 * (t & 3);
-        if (row_a < p.M) epilogue_pair(acc[4 * j], acc[4 * j + 1], row_a, n, p, first_split, atomic_out);
-        if (row_b < p.M) epilogue_pair(acc[4 * j + 2], acc[4 * j + 3], row_b, n, p, first_split, atomic_out);
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < BK / WG_K; ++j) {
+          const uint32_t sd = (kb | j) != 0 ? 1u : 0u;
+          // K-major : advance 16 elements (32 B) inside the 128 B swizzle row; this warpgroup's 64 rows start 8 KB in
+          // MN-major: advance 16 k-rows of 128 B; 64-element M/N chunks are (64 * BK * 2) bytes apart
+          const uint64_t da = A_MN ? gmma_desc_sw128(a_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
+                                   : gmma_desc_sw128(a_addr + j * (WG_K * 2), 16, 1024);
+          const uint64_t db = B_MN ? gmma_desc_sw128(b_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
+                                   : gmma_desc_sw128(b_addr + j * (WG_K * 2), 16, 1024);
+          if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+          else if constexpr (BN == 192) wgmma_m64n192k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+          else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+          else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+        }
+        wgmma_commit();
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+        if (kb > 0) release((it - 1) % STAGES);
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+      release((it - 1) % STAGES);   // the producer refills it with the next item's operands during the epilogue
+
+      const int row_a = w.m0 + cw * 64 + rl;
+      const int row_b = row_a + 8;
+      const bool first_split = w.split == 0;
+      if (p.tma_store) {
+        // -------------------------------------------------------------- epilogue through shared memory + TMA, one
+        // 64 x 32 box at a time through the warpgroup's staging area: 4 bf16 or 2 fp32 boxes in turn
+        const float* bias = first_split ? p.ep.bias : nullptr;
+        const bool bf16_out = p.tma_store == 1;
+#pragma unroll
+        for (int b = 0; b < BN / 32; ++b) {
+          if (w.n0 + b * 32 >= p.N) break;   // whole boxes right of N are neither staged nor stored
+          uint8_t* box = bf16_out ? epi + (boxes & 3) * (C::EPI_BOX_BYTES / 2) : epi + (boxes & 1) * C::EPI_BOX_BYTES;
+          if (t == 0) {   // the store that used this buffer last has read it
+            if (bf16_out) bulk_wait_read<3>();
+            else bulk_wait_read<1>();
+          }
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * b + jj;
+            const int c = jj * 8 + 2 * (t & 3);   // column within the box
+            float v[4] = {acc[4 * j] * p.ep.alpha, acc[4 * j + 1] * p.ep.alpha, acc[4 * j + 2] * p.ep.alpha,
+                          acc[4 * j + 3] * p.ep.alpha};
+            if (bias && w.n0 + b * 32 + c < p.N) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + w.n0 + b * 32 + c));
+              v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
+            }
+            if (p.ep.act == 1) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
+            }
+            if (bf16_out) {
+              stage_pair<bf16>(box, rl, c, v[0], v[1]);
+              stage_pair<bf16>(box, rl + 8, c, v[2], v[3]);
+            } else {
+              stage_pair<float>(box, rl, c, v[0], v[1]);
+              stage_pair<float>(box, rl + 8, c, v[2], v[3]);
+            }
+          }
+          fence_proxy_async_smem();
+          asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
+          if (t == 0) {
+            if (p.tma_store == 3) tma_reduce_add_2d(&tmC, box, w.n0 + b * 32, w.m0 + cw * 64);
+            else tma_store_2d(&tmC, box, w.n0 + b * 32, w.m0 + cw * 64);
+            bulk_commit_group();
+          }
+          ++boxes;
+        }
+      } else {
+        // -------------------------------------------------------------- epilogue straight from the accumulator registers
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (w.n0 + j * 8 >= p.N) break;   // N % 8 == 0: a column pair is either fully inside or fully outside
+          const int n = w.n0 + j * 8 + 2 * (t & 3);
+          if (row_a < p.M) epilogue_pair(acc[4 * j], acc[4 * j + 1], row_a, n, p, first_split, atomic_out);
+          if (row_b < p.M) epilogue_pair(acc[4 * j + 2], acc[4 * j + 3], row_b, n, p, first_split, atomic_out);
+        }
       }
     }
+    if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
   }
   // no CTA of a cluster may leave while its peer can still arrive on its barriers
   if constexpr (CL > 1) cluster_sync_all();
 }
 
 template <int BN, int CL, bool A_MN, bool B_MN>
-int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p, int split_k,
+int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                 cudaStream_t stream) {
   using C = GemmCfg<BN>;
   auto kern = gemm_bf16_kernel<BN, CL, A_MN, B_MN>;
-  static bool configured = false;
-  if (!configured) {
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = C::TOTAL;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = CL;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  // CTAs (CL = 1) or clusters (CL = 2) of this kernel the device can hold at once
+  static int resident = 0;
+  if (resident == 0) {
     MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::TOTAL));
-    configured = true;
+    if constexpr (CL > 1) {
+      cfg.gridDim = dim3(CL);
+      MMAE_CUDA_OK(cudaOccupancyMaxActiveClusters(&resident, kern, &cfg));
+    } else {
+      int dev = 0, sms = 0;
+      MMAE_CUDA_OK(cudaGetDevice(&dev));
+      MMAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+      resident = sms;
+    }
+    MMAE_CHECK(resident > 0, MMAE_ERR_CUDA, "mmae_gemm_bf16: the GEMM kernel does not fit on an SM");
   }
-  dim3 grid(ceil_div(p.N, BN), ceil_div(ceil_div(p.M, BM), CL) * CL, split_k);
-  const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K, (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (split_k << 8));
+  const int items = p.tiles_n * p.tiles_m * p.splits;
+  const int slots = std::min(resident, std::max(1, sm_count() / CL));
+  cfg.gridDim = dim3(std::min(items, slots) * CL);
+  const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K,
+                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (p.splits << 8));
   if constexpr (CL == 1) {
-    launch_k(kern, grid, GEMM_THREADS, C::TOTAL, stream, tmA, tmB, tmC, p);
+    cfg.attrs = attr + 1;
+    cfg.numAttrs = pdl_enabled() ? 1 : 0;
   } else {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = C::TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = CL;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    MMAE_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, p));
   }
+  MMAE_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, p));
   if (prof) gemm_profile_end(stream);
   count_launch();
   MMAE_LAUNCH_OK();
@@ -349,6 +411,15 @@ extern "C" int mmae_gemm_set_tma_store(int enable) {
 // by multicast), BN = 128 / 192 / 256
 static int variant_bn(int v) { return v == 0 ? 64 : (v == 1 || v == 6) ? 128 : (v == 3 || v == 5) ? 192 : 256; }
 
+// Fixed cost of one work item in the persistent kernel, in k-block times of its tile: its epilogue and the hand-over to
+// the next item.  scripts/gpu_time_gemm.py --fixed-cost measured 13.4, 14.0, 10.0 and 5.0 us per extra 128 x 256 fp32
+// reduce-add item at 2, 4, 8 and 12 items per SM, against 0.9 us per k-block (H100 SXM, 700 W power limit): 15 falling to
+// 5.5 k-block times as items per SM grow.  The model takes 4, near the low end, where the long-K weight gradients run;
+// 5 or more would cut fc1 / fc2's weight gradient to 5 splits of 40 k-blocks in 3 rounds, 4 keeps 9 splits of 22 in 5.
+constexpr int KB_PER_ITEM_FIXED = 4;
+// Split-K never cuts an item below this many k-blocks, which bounds the fp32 reduce-add traffic it adds
+constexpr int MIN_KB_PER_SPLIT = 16;
+
 extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb,
                               int b_mn_major, int M, int N, int K, int split_k, const mmae_gemm_epilogue* ep,
                               void* stream) {
@@ -360,31 +431,40 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
              MMAE_ERR_ARG, "mmae_gemm_bf16: operands must be 16-byte aligned");
   MMAE_CHECK(ep->out_f32 || ep->out_bf16, MMAE_ERR_ARG, "mmae_gemm_bf16: no output");
   const int num_kb = ceil_div(K, BK);
-  int variant = g_gemm_variant;
   const int sms = sm_count();
   const int tm = ceil_div(M, BM);
   if (split_k <= 0 && !(ep->out_f32 && !ep->out_bf16 && !ep->preact_bf16 && !ep->dgelu_z && ep->act == 0)) split_k = 1;
-  if (split_k <= 0) {
-    // auto split-K (weight gradients: small M x N, long K).  Joint choice of tile width and split count: one wave of
-    // ~SM-count work items; an item costs ~BN * (k-blocks + 6), the 6 standing for the fp32 reduce-add epilogue.
+
+  // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time (clusters:
+  // sm_count() / 2 items of 256 rows), so a launch lasts ceil(items / slots) rounds of one item, and an item costs
+  // ~(k-blocks + KB_PER_ITEM_FIXED) k-block times.  A k-block of a 128 x BN tile costs ~(BN + 40): the A tile's loads
+  // and MMA issue do not shrink with BN, which makes BN = 256 the better tile whenever its rounds are as full.  The
+  // automatic split (split_k
+  // <= 0) fills the last round of the long-K weight gradients instead of leaving it mostly idle.  An explicit variant
+  // fixes the tile, an explicit split_k the split.
+  int variant = g_gemm_variant;
+  {
     const int cand_var[2] = {1, 2};
+    const int nvar = variant >= 0 ? 1 : 2;
     long best_cost = -1;
     int best_split = 1, best_var = variant >= 0 ? variant : 1;
-    for (int i = 0; i < (variant >= 0 ? 1 : 2); ++i) {
+    for (int i = 0; i < nvar; ++i) {
       const int v = variant >= 0 ? variant : cand_var[i];
-      const int bn = variant_bn(v);
+      const int bn = variant_bn(v), cl = v >= 4 ? 2 : 1;
       if (variant < 0 && bn > 128 && N < bn) continue;
-      const int tiles = tm * ceil_div(N, bn);
-      int s_ = std::max(1, sms / tiles);
-      s_ = std::min(s_, std::max(1, num_kb / 4));
-      const int kbps = ceil_div(num_kb, s_);
-      s_ = ceil_div(num_kb, kbps);
-      const long rounds = (long(tiles) * s_ + sms - 1) / sms;
-      const long cost = rounds * bn * (kbps + 6);
-      if (best_cost < 0 || cost < best_cost) {
-        best_cost = cost;
-        best_split = s_;
-        best_var = v;
+      const long tiles = long(ceil_div(tm, cl)) * ceil_div(N, bn);
+      const int slots = std::max(1, sms / cl);
+      const int s_lo = split_k > 0 ? split_k : 1;
+      const int s_hi = split_k > 0 ? split_k : std::max(1, num_kb / MIN_KB_PER_SPLIT);
+      for (int s = s_lo; s <= s_hi; ++s) {
+        const int kbps = ceil_div(num_kb, std::min(s, num_kb));
+        const long rounds = (tiles * ceil_div(num_kb, kbps) + slots - 1) / slots;
+        const long cost = rounds * (bn + 40) * cl * (kbps + KB_PER_ITEM_FIXED);
+        if (best_cost < 0 || cost < best_cost) {
+          best_cost = cost;
+          best_split = s;
+          best_var = v;
+        }
       }
     }
     split_k = best_split;
@@ -405,24 +485,6 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
              MMAE_ERR_ARG, "mmae_gemm_bf16: epilogue tensors need 16-byte alignment and ld %% 8 == 0");
 #undef MMAE_LD_OK
 
-  if (variant < 0) {
-    // tile-quantisation model: ceil(tiles / SMs) waves; a wave costs ~(BN + c), c standing for the per-tile fixed work
-    // (pipeline fill, epilogue).  Pick the cheaper of BN = 128 / 256.
-    const int cand_var[2] = {1, 2};
-    long best_cost = -1;
-    variant = 1;
-    for (int i = 0; i < 2; ++i) {
-      const int bn = variant_bn(cand_var[i]);
-      if (bn > 128 && N < bn) continue;
-      const long items = long(tm) * ceil_div(N, bn) * split_k;
-      const long rounds = (items + sms - 1) / sms;
-      const long cost = rounds * (bn + 40);
-      if (best_cost < 0 || cost < best_cost) {
-        best_cost = cost;
-        variant = cand_var[i];
-      }
-    }
-  }
   if (variant == 5 && b_mn_major) variant = 4;   // an MN-major B half must be whole 64-column chunks
   const int BNsel = variant_bn(variant);
   const int CLsel = variant >= 4 ? 2 : 1;
@@ -447,6 +509,9 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   p.M = M; p.N = N; p.K = K;
   p.num_kb = num_kb;
   p.kb_per_split = kb_per_split;
+  p.tiles_n = ceil_div(N, BNsel);
+  p.tiles_m = ceil_div(tm, CLsel);
+  p.splits = split_k;
   p.ep = *ep;
   // plain bf16 / fp32 outputs (optionally with bias / GELU) leave through shared memory and TMA tile stores; fp32
   // accumulation (split-K, accumulate) through TMA reduce-add tiles
@@ -464,18 +529,18 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     }
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define MMAE_DISPATCH(BN_, CL_)                                                                               \
-  do {                                                                                                        \
-    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false>(tmA, tmB, tmC, p, split_k, st); \
-    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, CL_, false, true>(tmA, tmB, tmC, p, split_k, st);   \
-    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, true, false>(tmA, tmB, tmC, p, split_k, st);   \
-    return launch_gemm<BN_, CL_, true, true>(tmA, tmB, tmC, p, split_k, st);                                  \
+#define MMAE_DISPATCH(BN_, CL_)                                                                      \
+  do {                                                                                               \
+    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false>(tmA, tmB, tmC, p, st); \
+    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, CL_, false, true>(tmA, tmB, tmC, p, st);   \
+    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, true, false>(tmA, tmB, tmC, p, st);   \
+    return launch_gemm<BN_, CL_, true, true>(tmA, tmB, tmC, p, st);                                  \
   } while (0)
   if (variant == 4) MMAE_DISPATCH(256, 2);
   if (variant == 6) MMAE_DISPATCH(128, 2);
   if (variant == 5) {
-    if (!a_mn_major) return launch_gemm<192, 2, false, false>(tmA, tmB, tmC, p, split_k, st);
-    return launch_gemm<192, 2, true, false>(tmA, tmB, tmC, p, split_k, st);
+    if (!a_mn_major) return launch_gemm<192, 2, false, false>(tmA, tmB, tmC, p, st);
+    return launch_gemm<192, 2, true, false>(tmA, tmB, tmC, p, st);
   }
   if (variant == 0) MMAE_DISPATCH(64, 1);
   if (variant == 3) MMAE_DISPATCH(192, 1);
