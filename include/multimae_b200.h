@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 8
+#define MMAE_ABI_VERSION 9
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -240,45 +240,33 @@ typedef struct mmae_block_grads {
 
 int64_t mmae_block_saved_bytes(int B, int N, int D, int H, int hidden);
 int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hidden);
-int mmae_block_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                       const mmae_block_params* prm, void* saved, void* ws, void* stream);
-int mmae_block_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                        const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
-                        void* stream);
-/* Chained blocks (nn.Sequential of Blocks: the encoder, multimae/multimae.py:349, and each decoder_transformer,
- * multimae/output_adapters.py:271).  The residual add that ends a block, `x = x + mlp(norm2(x))`
- * (multimae/multimae_utils.py:231), is handed to the next block instead of running as a pass of its own:
- *   forward  - y_out_bf16 != NULL: the MLP branch output is written there, x_out is not written, and the block's output is
- *              x_mid + y_out, x_mid = mmae_block_saved_x_mid(saved);  x_add_bf16 != NULL: the block input is
- *              x_in + x_add_bf16, formed inside the first LayerNorm kernel and written to x_sum (fp32) - the x_in to give
- *              the backward call;
- *   backward - dx_in_bf16 != NULL: the first LayerNorm's backward also writes bf16(dx_in) there and adds colsum(dx_in) to
- *              dx_in_colsum (the PREVIOUS block's fc2 bias gradient);  dx_out_bf16 != NULL: that copy, made by the next
- *              block's backward - this block's cast + bias-gradient pass over dx_out is skipped.
- * With all optional pointers NULL the calls equal mmae_block_forward / mmae_block_backward. */
-int mmae_block_forward_chain(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
-                             int B, int N, int D, int H, int hidden, float eps, const mmae_block_params* prm, void* saved,
-                             void* ws, void* stream);
+/* One block; every pointer named below may be NULL, and with all of them NULL the calls are the plain block.  Forward
+ * computes, for the rows of sample b (row r of the [B*N, D] activation belongs to sample r / N),
+ *   x = x_in + scale_prev[b] * x_add_bf16,   x_mid = x + scale_attn[b] * attn(norm1(x)),
+ *   x_out = x_mid + scale_mlp[b] * mlp(norm2(x_mid))
+ * Hand-offs between consecutive blocks (nn.Sequential of Blocks: the encoder, multimae/multimae.py:349, and each
+ * decoder_transformer, multimae/output_adapters.py:271): the residual add that ends a block, `x = x + mlp(norm2(x))`
+ * (multimae/multimae_utils.py:231), runs inside the next block instead of as a pass of its own.
+ *   x_add_bf16   the previous block's MLP branch (its y_out_bf16); the sum x is formed inside the first LayerNorm kernel and
+ *                written to x_sum (fp32), the x_in to give the backward call.  NULL: x = x_in and x_sum is not used.
+ *   y_out_bf16   the MLP branch output is written there instead of x_out; the block's output is then x_mid + y_out_bf16,
+ *                x_mid = mmae_block_saved_x_mid(saved).  NULL: x_out is written.
+ *   dx_out_bf16  bf16(scale_mlp * dx_out), written by the next block's backward, which also added its column sums to this
+ *                block's fc2 bias gradient: this block's cast + bias-gradient pass over dx_out is skipped.  NULL: it runs.
+ *   dx_in_bf16   the first LayerNorm's backward also writes bf16(scale_prev * dx_in) there and adds its column sums to
+ *                dx_in_colsum (the PREVIOUS block's fc2 bias gradient).  NULL: neither is written.
+ * Stochastic depth (drop path, multimae/multimae_utils.py:105-132, 230-231): scale_attn, scale_mlp and scale_prev are
+ * per-sample fp32 factors, float[B]; NULL means factor 1.  scale_prev is the PREVIOUS block's scale_mlp and needs x_add_bf16
+ * (forward) and dx_in_bf16 (backward).  Backward takes the same three vectors: the gradient entering a branch is scaled,
+ * the residual-path gradient is not. */
+int mmae_block_forward(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16, int B, int N,
+                       int D, int H, int hidden, float eps, const float* scale_attn, const float* scale_mlp,
+                       const float* scale_prev, const mmae_block_params* prm, void* saved, void* ws, void* stream);
 float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H, int hidden);
-int mmae_block_backward_chain(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                              void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                              const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
-                              void* stream);
-/* Stochastic depth (drop path, multimae/multimae_utils.py:105-132, 230-231): the _chain forms with three per-sample fp32
- * factors, each float[B] or NULL (factor 1).  Forward computes
- *   x_mid = x + scale_attn[b] * attn(norm1(x)),   x_out = x_mid + scale_mlp[b] * mlp(norm2(x_mid))
- * for the rows of sample b (row r of the [B*N, D] activation belongs to sample r / N), with the block input
- * x = x_in + scale_prev[b] * x_add_bf16 when chained (scale_prev: the PREVIOUS block's scale_mlp; needs x_add_bf16).
- * Backward takes the same three vectors: the gradient entering a branch is scaled, the residual-path gradient is not;
- * dx_out_bf16 / dx_in_bf16 carry bf16(scale_mlp * dx_out) / bf16(scale_prev * dx_in) and their column sums go to the
- * fc2 bias gradients (scale_prev needs dx_in_bf16).  All three NULL: the _chain forms exactly. */
-int mmae_block_forward_dp(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16, int B,
-                          int N, int D, int H, int hidden, float eps, const float* scale_attn, const float* scale_mlp,
-                          const float* scale_prev, const mmae_block_params* prm, void* saved, void* ws, void* stream);
-int mmae_block_backward_dp(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in, void* dx_in_bf16,
-                           float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* scale_attn,
-                           const float* scale_mlp, const float* scale_prev, const mmae_block_params* prm,
-                           const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
+int mmae_block_backward(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in, void* dx_in_bf16,
+                        float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* scale_attn,
+                        const float* scale_mlp, const float* scale_prev, const mmae_block_params* prm,
+                        const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SpatialOutputAdapter, split at its decoder_transformer (multimae/output_adapters.py:236-282):
@@ -444,19 +432,13 @@ int mmae_attention_f32_backward(const float* q, int64_t ldq, const float* k, int
                                 int Nk, int head_dim, float scale, void* stream);
 int64_t mmae_block_f32_saved_bytes(int B, int N, int D, int H, int hidden);
 int64_t mmae_block_f32_workspace_bytes(int B, int N, int D, int H, int hidden);
+/* mmae_block_forward / _backward without hand-offs: scale_attn / scale_mlp as there, float[B] or NULL (factor 1) */
 int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                           const mmae_block_params* prm, void* saved, void* ws, void* stream);
+                           const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm, void* saved,
+                           void* ws, void* stream);
 int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                            const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
-                            void* stream);
-/* stochastic depth in the fp32 tier: per-sample factors of the attention / MLP branch, float[B] or NULL (see
- * mmae_block_forward_dp); both NULL: mmae_block_f32_forward / _backward */
-int mmae_block_f32_forward_dp(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                              const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm, void* saved,
-                              void* ws, void* stream);
-int mmae_block_f32_backward_dp(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                               const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm,
-                               const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
+                            const float* scale_attn, const float* scale_mlp, const mmae_block_params* prm,
+                            const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
 int64_t mmae_dechead_f32_saved_bytes(const mmae_decoder_index* ix, int D_enc, int H, int hidden);
 int64_t mmae_dechead_f32_workspace_bytes(const mmae_decoder_index* ix, int D_enc, int H, int hidden);
 int mmae_dechead_f32_forward(const float* enc, int D_enc, const mmae_decoder_index* ix, int H, int hidden, float eps,

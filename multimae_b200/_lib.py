@@ -160,23 +160,13 @@ SIGNATURES = {
                                     c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mmae_block_saved_bytes": (c_i64, [c_int] * 5),
     "mmae_block_workspace_bytes": (c_i64, [c_int] * 5),
-    "mmae_block_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float,
-                                   ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
-    "mmae_block_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                    ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
-                                    c_void_p]),
-    "mmae_block_forward_chain": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                         c_float, ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
+    "mmae_block_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                   c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams), c_void_p, c_void_p,
+                                   c_void_p]),
     "mmae_block_saved_x_mid": (c_void_p, [c_void_p, c_int, c_int, c_int, c_int, c_int]),
-    "mmae_block_backward_chain": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                          c_int, c_int, ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p,
-                                          c_void_p, c_void_p]),
-    "mmae_block_forward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                      c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams), c_void_p, c_void_p,
-                                      c_void_p]),
-    "mmae_block_backward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                       c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams),
-                                       ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
+    "mmae_block_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                    c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams),
+                                    ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
     "mmae_dechead_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -249,16 +239,11 @@ SIGNATURES = {
                                             c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mmae_block_f32_saved_bytes": (c_i64, [c_int] * 5),
     "mmae_block_f32_workspace_bytes": (c_i64, [c_int] * 5),
-    "mmae_block_f32_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float,
+    "mmae_block_f32_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                        ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
-    "mmae_block_f32_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+    "mmae_block_f32_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                         ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
                                         c_void_p]),
-    "mmae_block_f32_forward_dp": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
-                                          ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
-    "mmae_block_f32_backward_dp": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                           ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
-                                           c_void_p]),
     "mmae_dechead_f32_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_f32_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_f32_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -275,7 +260,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 def lib():

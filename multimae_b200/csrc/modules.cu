@@ -339,18 +339,19 @@ extern "C" int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hi
   return (int64_t)block_ws(nullptr, B, N, D, H, hidden).bytes;
 }
 
-// Chained form (mmae_block_forward_chain): consecutive blocks hand the last residual add over instead of running it as a
-// pass of its own.  `x_add` (bf16) != null: the block input is x_in + x_add, formed inside the first LayerNorm kernel and
-// written to `x_sum` (what backward gets as x_in).  `y_out` (bf16) != null: the MLP branch output goes there, x_out is not
-// written, and the block's output is x_mid (mmae_block_saved_x_mid) + y_out - the next block's (x_in, x_add).
-// Stochastic depth (mmae_block_forward_dp): s_attn / s_mlp [B] multiply the attention / MLP branch of each sample inside the
-// residual adds, s_prev [B] multiplies x_add (the previous block's MLP branch).  Null: factor 1, the plain block.
-static int block_forward_impl(const float* x_in, const bf16* x_add, float* x_sum, float* x_out, bf16* y_out, int B, int N,
-                              int D, int H, int hidden, float eps, const float* s_attn, const float* s_mlp,
-                              const float* s_prev, const mmae_block_params* p, void* saved, void* ws, void* st) {
+// Hand-offs between consecutive blocks: `x_add` != null: the block input is x_in + s_prev * x_add, formed inside the first
+// LayerNorm kernel and written to `x_sum` (what backward gets as x_in).  `y_out` != null: the MLP branch output goes there,
+// x_out is not written, and the block's output is x_mid (mmae_block_saved_x_mid) + y_out - the next block's (x_in, x_add).
+// Stochastic depth: s_attn / s_mlp [B] multiply the attention / MLP branch of each sample inside the residual adds, s_prev [B]
+// multiplies x_add (the previous block's MLP branch).  Null: factor 1.
+extern "C" int mmae_block_forward(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
+                                  int B, int N, int D, int H, int hidden, float eps, const float* s_attn, const float* s_mlp,
+                                  const float* s_prev, const mmae_block_params* p, void* saved, void* ws, void* st) {
+  const bf16* x_add = static_cast<const bf16*>(x_add_bf16);
+  bf16* y_out = static_cast<bf16*>(y_out_bf16);
   MMAE_CHECK(x_in && (x_out || y_out) && (!x_add || x_sum) && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0,
              MMAE_ERR_ARG, "mmae_block_forward: bad args");
-  MMAE_CHECK(!s_prev || x_add, MMAE_ERR_ARG, "mmae_block_forward_dp: the previous block's scale needs x_add");
+  MMAE_CHECK(!s_prev || x_add, MMAE_ERR_ARG, "mmae_block_forward: the previous block's scale needs x_add");
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(saved, B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, int64_t(3) * D * D, true, st));
@@ -383,43 +384,26 @@ static int block_forward_impl(const float* x_in, const bf16* x_add, float* x_sum
   return MMAE_OK;
 }
 
-extern "C" int mmae_block_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                                  const mmae_block_params* p, void* saved, void* ws, void* st) {
-  MMAE_CHECK(x_out, MMAE_ERR_ARG, "mmae_block_forward: bad args");
-  return block_forward_impl(x_in, nullptr, nullptr, x_out, nullptr, B, N, D, H, hidden, eps, nullptr, nullptr, nullptr, p,
-                            saved, ws, st);
-}
-extern "C" int mmae_block_forward_chain(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out,
-                                        void* y_out_bf16, int B, int N, int D, int H, int hidden, float eps,
-                                        const mmae_block_params* p, void* saved, void* ws, void* st) {
-  return block_forward_impl(x_in, reinterpret_cast<const bf16*>(x_add_bf16), x_sum, x_out, reinterpret_cast<bf16*>(y_out_bf16),
-                            B, N, D, H, hidden, eps, nullptr, nullptr, nullptr, p, saved, ws, st);
-}
-extern "C" int mmae_block_forward_dp(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
-                                     int B, int N, int D, int H, int hidden, float eps, const float* scale_attn,
-                                     const float* scale_mlp, const float* scale_prev, const mmae_block_params* p, void* saved,
-                                     void* ws, void* st) {
-  return block_forward_impl(x_in, reinterpret_cast<const bf16*>(x_add_bf16), x_sum, x_out, reinterpret_cast<bf16*>(y_out_bf16),
-                            B, N, D, H, hidden, eps, scale_attn, scale_mlp, scale_prev, p, saved, ws, st);
-}
 extern "C" float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H, int hidden) {
   return saved ? block_saved(saved, B, N, D, H, hidden).x_mid : nullptr;
 }
 
-// Chained form (mmae_block_backward_chain).  `dx_out_b` (bf16) != null: bf16(dx_out) made by the NEXT block's backward,
-// which also added its column sums to this block's fc2 bias gradient: the cast + column-sum pass is skipped.
-// `dx_in_b` (bf16) != null: the first LayerNorm's backward also writes bf16(dx_in) there and adds colsum(dx_in) to
-// `dx_in_colsum` - the PREVIOUS block's fc2 bias gradient - for that block's backward to start from.
+// Hand-offs: `dx_out_b` != null: bf16(dx_out) made by the NEXT block's backward, which also added its column sums to this
+// block's fc2 bias gradient: the cast + column-sum pass is skipped.  `dx_in_b` != null: the first LayerNorm's backward also
+// writes bf16(dx_in) there and adds colsum(dx_in) to `dx_in_colsum` - the PREVIOUS block's fc2 bias gradient - for that
+// block's backward to start from.
 // Stochastic depth: the gradient entering a branch is s * (gradient of the residual stream), so s_mlp scales the MLP branch's
 // bf16 operand and fc2 bias gradient, s_attn the proj operand and bias gradient that LN2's backward emits, s_prev what LN1's
 // backward hands to the previous block.  The fp32 residual-path gradients (dx_mid, dx_in) are never scaled.
-static int block_backward_impl(const float* x_in, const float* dx_out, const bf16* dx_out_b, float* dx_in, bf16* dx_in_b,
-                               float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* s_attn,
-                               const float* s_mlp, const float* s_prev, const mmae_block_params* p,
-                               const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
+                                   void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
+                                   const float* s_attn, const float* s_mlp, const float* s_prev, const mmae_block_params* p,
+                                   const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+  const bf16* dx_out_b = static_cast<const bf16*>(dx_out_bf16);
+  bf16* dx_in_b = static_cast<bf16*>(dx_in_bf16);
   MMAE_CHECK(x_in && dx_out && dx_in && (!dx_in_b || dx_in_colsum) && p && g && saved && ws, MMAE_ERR_ARG,
              "mmae_block_backward: bad args");
-  MMAE_CHECK(!s_prev || dx_in_b, MMAE_ERR_ARG, "mmae_block_backward_dp: the previous block's scale needs dx_in_bf16");
+  MMAE_CHECK(!s_prev || dx_in_b, MMAE_ERR_ARG, "mmae_block_backward: the previous block's scale needs dx_in_bf16");
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(const_cast<void*>(saved), B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, 0, false, st));
@@ -465,30 +449,6 @@ static int block_backward_impl(const float* x_in, const float* dx_out, const bf1
                                 g->norm1_b, M, D, st));
   if (side) RUN(side_join(st));   // the caller sees every gradient of this block in stream order
   return MMAE_OK;
-}
-
-extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H,
-                                   int hidden, const mmae_block_params* p, const mmae_block_grads* g, const void* saved,
-                                   void* ws, void* st) {
-  return block_backward_impl(x_in, dx_out, nullptr, dx_in, nullptr, nullptr, B, N, D, H, hidden, nullptr, nullptr, nullptr, p,
-                             g, saved, ws, st);
-}
-extern "C" int mmae_block_backward_chain(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                                         void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                                         const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
-                                         void* st) {
-  return block_backward_impl(x_in, dx_out, reinterpret_cast<const bf16*>(dx_out_bf16), dx_in,
-                             reinterpret_cast<bf16*>(dx_in_bf16), dx_in_colsum, B, N, D, H, hidden, nullptr, nullptr, nullptr,
-                             p, g, saved, ws, st);
-}
-extern "C" int mmae_block_backward_dp(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                                      void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                                      const float* scale_attn, const float* scale_mlp, const float* scale_prev,
-                                      const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
-                                      void* st) {
-  return block_backward_impl(x_in, dx_out, reinterpret_cast<const bf16*>(dx_out_bf16), dx_in,
-                             reinterpret_cast<bf16*>(dx_in_bf16), dx_in_colsum, B, N, D, H, hidden, scale_attn, scale_mlp,
-                             scale_prev, p, g, saved, ws, st);
 }
 
 extern "C" int mmae_set_wgrad_stream(int enable) {

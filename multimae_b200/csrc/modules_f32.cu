@@ -177,11 +177,11 @@ extern "C" int64_t mmae_block_f32_workspace_bytes(int B, int N, int D, int H, in
   return (int64_t)block_ws_f(nullptr, B, N, D, H, hidden).bytes;
 }
 
-// Stochastic depth (the *_dp forms): s_attn / s_mlp [B] multiply each sample's attention / MLP branch.  With a factor the
+// Stochastic depth: s_attn / s_mlp [B] (null: factor 1) multiply each sample's attention / MLP branch.  With a factor the
 // branch GEMM writes the branch alone (w.g, unused otherwise in forward) and a row-scaled add forms the residual sum.
-static int block_f32_forward_impl(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                                  const float* s_attn, const float* s_mlp, const mmae_block_params* p, void* saved, void* ws,
-                                  void* st) {
+extern "C" int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
+                                      const float* s_attn, const float* s_mlp, const mmae_block_params* p, void* saved,
+                                      void* ws, void* st) {
   MMAE_CHECK(x_in && x_out && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0, MMAE_ERR_ARG, "mmae_block_f32_forward: bad args");
   const int M = B * N, dh = D / H;
   const int64_t MD = int64_t(M) * D, ND = int64_t(N) * D;
@@ -210,21 +210,11 @@ static int block_f32_forward_impl(const float* x_in, float* x_out, int B, int N,
   return MMAE_OK;
 }
 
-extern "C" int mmae_block_f32_forward(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                                      const mmae_block_params* p, void* saved, void* ws, void* st) {
-  return block_f32_forward_impl(x_in, x_out, B, N, D, H, hidden, eps, nullptr, nullptr, p, saved, ws, st);
-}
-extern "C" int mmae_block_f32_forward_dp(const float* x_in, float* x_out, int B, int N, int D, int H, int hidden, float eps,
-                                         const float* scale_attn, const float* scale_mlp, const mmae_block_params* p,
-                                         void* saved, void* ws, void* st) {
-  return block_f32_forward_impl(x_in, x_out, B, N, D, H, hidden, eps, scale_attn, scale_mlp, p, saved, ws, st);
-}
-
 // Backward with factors: the branch's weight / input gradients are taken from a row-scaled copy of the residual-stream
 // gradient (w.g, unused otherwise in backward); the residual path itself carries the unscaled gradient.
-static int block_f32_backward_impl(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                                   const float* s_attn, const float* s_mlp, const mmae_block_params* p,
-                                   const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+extern "C" int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H,
+                                       int hidden, const float* s_attn, const float* s_mlp, const mmae_block_params* p,
+                                       const mmae_block_grads* g, const void* saved, void* ws, void* st) {
   MMAE_CHECK(x_in && dx_out && dx_in && p && g && saved && ws, MMAE_ERR_ARG, "mmae_block_f32_backward: bad args");
   const int M = B * N, dh = D / H;
   const int64_t MD = int64_t(M) * D, ND = int64_t(N) * D;
@@ -258,17 +248,6 @@ static int block_f32_backward_impl(const float* x_in, const float* dx_out, float
   RUN(mmae_layernorm_backward(w.dh, 0, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
                               g->norm1_b, M, D, st));
   return MMAE_OK;
-}
-
-extern "C" int mmae_block_f32_backward(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H, int hidden,
-                                       const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws, void* st) {
-  return block_f32_backward_impl(x_in, dx_out, dx_in, B, N, D, H, hidden, nullptr, nullptr, p, g, saved, ws, st);
-}
-extern "C" int mmae_block_f32_backward_dp(const float* x_in, const float* dx_out, float* dx_in, int B, int N, int D, int H,
-                                          int hidden, const float* scale_attn, const float* scale_mlp,
-                                          const mmae_block_params* p, const mmae_block_grads* g, const void* saved, void* ws,
-                                          void* st) {
-  return block_f32_backward_impl(x_in, dx_out, dx_in, B, N, D, H, hidden, scale_attn, scale_mlp, p, g, saved, ws, st);
 }
 
 // ================================================================================================ decoder head

@@ -37,7 +37,7 @@ class Workspace:
         return buf
 
 
-# consecutive Blocks hand their residual add / gradient cast over to each other (BlockStackFunction); 0: block by block
+# consecutive Blocks hand their residual add / gradient cast over to each other (block_stack); 0: block by block
 BLOCK_CHAIN = os.environ.get("MMAE_BLOCK_CHAIN", "1") != "0"
 
 _ARENAS = weakref.WeakSet()
@@ -166,90 +166,19 @@ BLOCK_PARAM_NAMES = ["norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.
 
 
 class BlockFunction(torch.autograd.Function):
-    """Block.forward (multimae/multimae_utils.py:229-232) as one fused sequence of kernels.
+    """n >= 1 consecutive Blocks (Block.forward, multimae/multimae_utils.py:229-232), one library call per block and
+    direction.  A stack of them (the encoder, multimae/multimae.py:349; a decoder_transformer,
+    multimae/output_adapters.py:271) hands off between consecutive blocks in the bf16 tier: the residual add that ends block
+    i runs inside block i+1's first LayerNorm kernel, and block i+1's first LayerNorm backward emits the bf16 copy of the
+    gradient and the fc2 bias gradient that block i's backward starts from.  n - 1 add passes and n - 1 cast + column-sum
+    passes less than n one-block calls; same arithmetic.
 
-    `scales`: None, or the (s_attn, s_mlp) pair of drop_path_scales - then the *_dp entry points apply stochastic depth."""
+    Stochastic depth: `scales` holds one drop_path_scales entry per block (None: factor 1).  Block i+1 also receives block
+    i's s_mlp, the factor of the MLP branch it adds in front of its first LayerNorm (forward) and of the bf16 gradient it
+    hands down (backward).
 
-    @staticmethod
-    def forward(ctx, x, meta, scales, *params):
-        _require_cuda(x, "Block")
-        B, N, D = x.shape
-        H, hidden, eps = meta["heads"], meta["hidden"], meta["eps"]
-        x = x.contiguous().float()
-        lib = L.lib()
-        # meta["fp32"]: the fp32 tier of `fp32_output_adapters` (3 x bf16 split GEMMs, fp32 attention / GELU)
-        f32 = "_f32" if meta.get("fp32") else ""
-        saved = torch.empty(getattr(lib, "mmae_block%s_saved_bytes" % f32)(B, N, D, H, hidden), dtype=torch.uint8,
-                            device=x.device)
-        ws = Workspace.get(getattr(lib, "mmae_block%s_workspace_bytes" % f32)(B, N, D, H, hidden), x.device)
-        out = torch.empty_like(x)
-        prm = L.BlockParams(*[p.data_ptr() for p in params])
-        if scales is None:
-            L.check(getattr(lib, "mmae_block%s_forward" % f32)(x.data_ptr(), out.data_ptr(), B, N, D, H, hidden, eps,
-                                                               ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                                               L.current_stream()), "mmae_block%s_forward" % f32)
-        elif f32:
-            L.check(lib.mmae_block_f32_forward_dp(x.data_ptr(), out.data_ptr(), B, N, D, H, hidden, eps, scales[0].data_ptr(),
-                                                  scales[1].data_ptr(), ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                                  L.current_stream()), "mmae_block_f32_forward_dp")
-        else:
-            L.check(lib.mmae_block_forward_dp(x.data_ptr(), None, None, out.data_ptr(), None, B, N, D, H, hidden, eps,
-                                              scales[0].data_ptr(), scales[1].data_ptr(), None, ctypes.byref(prm),
-                                              saved.data_ptr(), ws.data_ptr(), L.current_stream()), "mmae_block_forward_dp")
-        ctx.meta = meta
-        ctx.params = params
-        ctx.scales = scales
-        ctx.save_for_backward(x, saved)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        x, saved = ctx.saved_tensors
-        meta, params = ctx.meta, ctx.params
-        B, N, D = x.shape
-        H, hidden = meta["heads"], meta["hidden"]
-        arena, prefix = meta["arena"], meta["prefix"]
-        names = [prefix + n for n in BLOCK_PARAM_NAMES]
-        lib = L.lib()
-        f32 = "_f32" if meta.get("fp32") else ""
-        ws = Workspace.get(getattr(lib, "mmae_block%s_workspace_bytes" % f32)(B, N, D, H, hidden), x.device)
-        dout = dout.contiguous().float()
-        dx = torch.empty_like(x)
-        prm = L.BlockParams(*[p.data_ptr() for p in params])
-        grd = L.BlockGrads(*[_grad_ptr(arena, n) for n in names])
-        sc = ctx.scales
-        if sc is None:
-            L.check(getattr(lib, "mmae_block%s_backward" % f32)(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), B, N, D, H,
-                                                                hidden, ctypes.byref(prm), ctypes.byref(grd),
-                                                                saved.data_ptr(), ws.data_ptr(), L.current_stream()),
-                    "mmae_block%s_backward" % f32)
-        elif f32:
-            L.check(lib.mmae_block_f32_backward_dp(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), B, N, D, H, hidden,
-                                                   sc[0].data_ptr(), sc[1].data_ptr(), ctypes.byref(prm), ctypes.byref(grd),
-                                                   saved.data_ptr(), ws.data_ptr(), L.current_stream()),
-                    "mmae_block_f32_backward_dp")
-        else:
-            L.check(lib.mmae_block_backward_dp(x.data_ptr(), dout.data_ptr(), None, dx.data_ptr(), None, None, B, N, D, H,
-                                               hidden, sc[0].data_ptr(), sc[1].data_ptr(), None, ctypes.byref(prm),
-                                               ctypes.byref(grd), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
-                    "mmae_block_backward_dp")
-        if meta.get("on_grads_ready") is not None:
-            meta["on_grads_ready"](names)
-        return (dx, None, None) + tuple(_ret_grads(arena, names, params))
-
-
-class BlockStackFunction(torch.autograd.Function):
-    """nn.Sequential of n >= 2 Blocks (the encoder, multimae/multimae.py:349; a decoder_transformer,
-    multimae/output_adapters.py:271) with the hand-offs between consecutive blocks fused (mmae_block_*_chain): the residual
-    add that ends block i runs inside block i+1's first LayerNorm kernel, and block i+1's first LayerNorm backward emits the
-    bf16 copy of the gradient and the fc2 bias gradient that block i's backward starts from.  n - 1 add passes and n - 1
-    cast + column-sum passes less than n BlockFunctions; same arithmetic.
-
-    Stochastic depth: `scales` holds one drop_path_scales entry per block.  When any is set, every block runs through
-    mmae_block_*_dp, block i+1 also receiving block i's s_mlp - the factor of the MLP branch it adds in front of its first
-    LayerNorm (forward) and of the bf16 gradient it hands down (backward); otherwise the calls are the plain _chain ones.
-
-    args: x, metas (one dict per block, as for BlockFunction), scales, then the 12 BLOCK_PARAM_NAMES tensors of every
+    args: x, metas (one dict per block, all of one shape; metas[0]["fp32"]: the fp32 tier of `fp32_output_adapters` - 3 x
+    bf16 split GEMMs, fp32 attention / GELU - for one block), scales, then the 12 BLOCK_PARAM_NAMES tensors of every
     block."""
 
     @staticmethod
@@ -257,38 +186,38 @@ class BlockStackFunction(torch.autograd.Function):
         _require_cuda(x, "Block")
         lib = L.lib()
         n, P = len(metas), len(BLOCK_PARAM_NAMES)
+        tier = "_f32" if metas[0].get("fp32") else ""
         B, N, D = x.shape
         H, hidden, eps = metas[0]["heads"], metas[0]["hidden"], metas[0]["eps"]
         x = x.contiguous().float()
         dev = x.device
-        ws = Workspace.get(lib.mmae_block_workspace_bytes(B, N, D, H, hidden), dev)
-        nbytes = lib.mmae_block_saved_bytes(B, N, D, H, hidden)
-        y = torch.empty((B, N, D), dtype=torch.bfloat16, device=dev)      # MLP branch output on its way to the next block
+        ws = Workspace.get(getattr(lib, "mmae_block%s_workspace_bytes" % tier)(B, N, D, H, hidden), dev)
+        nbytes = getattr(lib, "mmae_block%s_saved_bytes" % tier)(B, N, D, H, hidden)
+        # MLP branch output on its way to the next block
+        y = torch.empty((B, N, D), dtype=torch.bfloat16, device=dev) if n > 1 else None
         out = torch.empty_like(x)
         xs, saveds = [], []
         x_ptr, add_ptr = x.data_ptr(), None
-        dp = any(sc is not None for sc in scales)
         for i in range(n):
             last = i == n - 1
             saved = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             x_sum = torch.empty_like(x) if add_ptr is not None else None
             prm = L.BlockParams(*[p.data_ptr() for p in params[i * P:(i + 1) * P]])
-            if dp:
-                s_attn, s_mlp, s_prev = _stack_scale_ptrs(scales, i)
-                L.check(lib.mmae_block_forward_dp(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
-                                                  None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
-                                                  s_prev, ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                                  L.current_stream()), "mmae_block_forward_dp")
+            s_attn, s_mlp, s_prev = _stack_scale_ptrs(scales, i)
+            if tier:
+                L.check(lib.mmae_block_f32_forward(x_ptr, out.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
+                                                   ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                        "mmae_block_f32_forward")
             else:
-                L.check(lib.mmae_block_forward_chain(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
-                                                     None if last else y.data_ptr(), B, N, D, H, hidden, eps,
-                                                     ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                                     L.current_stream()), "mmae_block_forward_chain")
+                L.check(lib.mmae_block_forward(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
+                                               None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
+                                               s_prev, ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
+                                               L.current_stream()), "mmae_block_forward")
             xs.append(x if x_sum is None else x_sum)
             saveds.append(saved)
             if not last:       # the next block's input: this block's x_mid (inside `saved`) + y
                 x_ptr, add_ptr = lib.mmae_block_saved_x_mid(saved.data_ptr(), B, N, D, H, hidden), y.data_ptr()
-        ctx.metas, ctx.params, ctx.dims, ctx.scales = metas, params, (B, N, D, H, hidden), (scales if dp else None)
+        ctx.metas, ctx.params, ctx.dims, ctx.scales = metas, params, (B, N, D, H, hidden), scales
         ctx.save_for_backward(*xs, *saveds)
         return out
 
@@ -298,9 +227,10 @@ class BlockStackFunction(torch.autograd.Function):
         metas, params = ctx.metas, ctx.params
         B, N, D, H, hidden = ctx.dims
         n, P = len(metas), len(BLOCK_PARAM_NAMES)
+        tier = "_f32" if metas[0].get("fp32") else ""
         xs, saveds = ctx.saved_tensors[:n], ctx.saved_tensors[n:]
         dev = dout.device
-        ws = Workspace.get(lib.mmae_block_workspace_bytes(B, N, D, H, hidden), dev)
+        ws = Workspace.get(getattr(lib, "mmae_block%s_workspace_bytes" % tier)(B, N, D, H, hidden), dev)
         d = dout.contiguous().float()
         g_in = None                                                        # bf16(d) handed down by the block above
         g_bufs = [torch.empty((B, N, D), dtype=torch.bfloat16, device=dev) for _ in range(min(2, n - 1))]
@@ -316,17 +246,17 @@ class BlockStackFunction(torch.autograd.Function):
             if i > 0:      # bf16(dx) + the fc2 bias gradient of the block below, from this block's first-LayerNorm backward
                 g_out = g_bufs[i % len(g_bufs)]
                 below_bias = _grad_ptr(metas[i - 1]["arena"], metas[i - 1]["prefix"] + "mlp.fc2.bias")
-            if ctx.scales is not None:
-                s_attn, s_mlp, s_prev = _stack_scale_ptrs(ctx.scales, i)
-                L.check(lib.mmae_block_backward_dp(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
-                                                   below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev, ctypes.byref(prm),
-                                                   ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
-                                                   L.current_stream()), "mmae_block_backward_dp")
+            s_attn, s_mlp, s_prev = _stack_scale_ptrs(ctx.scales, i)
+            if tier:
+                L.check(lib.mmae_block_f32_backward(xs[i].data_ptr(), d.data_ptr(), dx.data_ptr(), B, N, D, H, hidden,
+                                                    s_attn, s_mlp, ctypes.byref(prm), ctypes.byref(grd),
+                                                    saveds[i].data_ptr(), ws.data_ptr(), L.current_stream()),
+                        "mmae_block_f32_backward")
             else:
-                L.check(lib.mmae_block_backward_chain(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(),
-                                                      L.ptr(g_out), below_bias, B, N, D, H, hidden, ctypes.byref(prm),
-                                                      ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
-                                                      L.current_stream()), "mmae_block_backward_chain")
+                L.check(lib.mmae_block_backward(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
+                                                below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev, ctypes.byref(prm),
+                                                ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
+                                                L.current_stream()), "mmae_block_backward")
             if metas[i].get("on_grads_ready") is not None:
                 metas[i]["on_grads_ready"](names)       # fc2.bias of block i is complete: its column sums came from block i+1
             grads[i * P:(i + 1) * P] = _ret_grads(arena, names, blk)
@@ -343,9 +273,9 @@ def _stack_scale_ptrs(scales, i):
 
 
 def block_stack(blocks, x, fp32=False):
-    """Run an nn.Sequential of multimae_utils.Block through BlockStackFunction when it applies (CUDA path, >= 2 blocks of
-    one shape bound to an arena, BLOCK_CHAIN on), else block by block (`fp32`: in the fp32 tier, always block by block).
-    The stochastic-depth factors of all blocks are drawn once, up front (drop_path_scales)."""
+    """Run an nn.Sequential of multimae_utils.Block as one BlockFunction with hand-offs when it applies (CUDA path, >= 2
+    blocks of one shape bound to an arena, BLOCK_CHAIN on), else block by block (`fp32`: in the fp32 tier, always block by
+    block).  The stochastic-depth factors of all blocks are drawn once, up front (drop_path_scales)."""
     blocks = list(blocks)
     scales = drop_path_scales(blocks, x.shape[0], x.device)
     metas = [getattr(b, "_meta", None) for b in blocks]
@@ -360,7 +290,7 @@ def block_stack(blocks, x, fp32=False):
     flat = []
     for b in blocks:
         flat += list(b._params())
-    return BlockStackFunction.apply(x, metas, scales, *flat)
+    return BlockFunction.apply(x, metas, scales, *flat)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

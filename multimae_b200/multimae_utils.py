@@ -137,4 +137,4 @@ class Block(nn.Module):
         if getattr(self, "_own_arena", False) and torch.is_grad_enabled():
             self._meta["arena"].zero_()
         meta = dict(self._meta, fp32=True) if fp32 else self._meta
-        return Fn.BlockFunction.apply(x, meta, scales, *self._params())
+        return Fn.BlockFunction.apply(x, [meta], [scales], *self._params())

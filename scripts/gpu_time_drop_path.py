@@ -3,7 +3,7 @@ against 0.1 (encoder and decoders), the two settings alternating in one process 
 
     python scripts/gpu_time_drop_path.py [--rounds 5] [--steps 20]
 
-Both graphs are captured from one model (the rate only changes which block entry points are recorded).  Each timed
+Both graphs are captured from one model (the rate only changes the scale arguments of the recorded block calls).  Each timed
 window is bracketed by device synchronisations; prints ms/step per setting (median over rounds), GPU name and power limit."""
 import argparse
 import os

@@ -1,4 +1,4 @@
-"""GPU: stochastic depth (drop path) inside the fused block kernels (mmae_block_*_dp).
+"""GPU: stochastic depth (drop path) inside the fused block kernels (the scale arguments of mmae_block_*).
 
 The per-sample factors are pinned by substituting functional.drop_path_scales (as other tests substitute
 generate_random_masks); the oracle runs with the same factors (tests/drop_path_oracle.py).  Nothing here reads the reference checkout."""

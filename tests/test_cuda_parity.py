@@ -229,8 +229,8 @@ def test_shared_context_projection_matches_per_adapter(golden_dir, dev, monkeypa
 
 
 def test_block_chain_matches_single_blocks(golden_dir, dev, monkeypatch):
-    """Consecutive Blocks with the hand-offs fused (BlockStackFunction / mmae_block_*_chain, the default) against one
-    BlockFunction per block (MMAE_BLOCK_CHAIN=0): the residual add moves into the next block's first LayerNorm kernel and the
+    """Consecutive Blocks with the hand-offs fused (one BlockFunction per stack, the default) against one BlockFunction
+    per block (MMAE_BLOCK_CHAIN=0): the residual add moves into the next block's first LayerNorm kernel and the
     gradient cast + fc2 bias gradient into its backward - the same fp32 operations on the same values, so predictions and
     gradients must agree to fp32 summation order (split-K reduce-adds, the fc2 bias column sums).  4 encoder blocks and
     2-block decoder transformers: both alternating hand-off buffers are in use."""

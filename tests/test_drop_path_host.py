@@ -115,9 +115,10 @@ def _pinned(monkeypatch, B):
 
 
 @pytest.mark.parametrize("chain", [True, False])
-def test_drop_path_entry_points_and_scale_pointers(rec, monkeypatch, chain):
-    """p > 0 in training: every block of the call runs through mmae_block_*_dp; block i gets its own (s_attn, s_mlp) and
-    - chained - block i-1's s_mlp as the previous block's scale, forward and backward.  Block 0 (p = 0) has no own scales."""
+def test_drop_path_scale_arguments(rec, monkeypatch, chain):
+    """p > 0 in training: every block of the call carries its factors; block i gets its own (s_attn, s_mlp) and - chained -
+    block i-1's s_mlp as the previous block's scale, forward and backward.  Block 0 (p = 0) has no own scales: unchained,
+    all its scale arguments are None."""
     monkeypatch.setattr(Fn, "BLOCK_CHAIN", chain)
     B = 3
     blocks = _stack().train()
@@ -125,20 +126,10 @@ def test_drop_path_entry_points_and_scale_pointers(rec, monkeypatch, chain):
     x = torch.randn(B, 5, 128, requires_grad=True)
     out = Fn.block_stack(blocks, x)
     out.sum().backward()
-    names = rec.names()
-    assert "mmae_block_forward_chain" not in names and "mmae_block_backward_chain" not in names
-    fwd = [a for n, a in rec.calls if n == "mmae_block_forward_dp"]
-    bwd = [a for n, a in rec.calls if n == "mmae_block_backward_dp"][::-1]      # issued for blocks 3..0
-    assert len(made) == 3
-    if chain:      # the stack as a whole has factors: all four blocks run through the _dp entry points
-        assert len(fwd) == len(bwd) == 4 and "mmae_block_forward" not in names
-    else:          # block by block: block 0 (p = 0) issues the plain calls
-        assert len(fwd) == len(bwd) == 3
-        assert names.count("mmae_block_forward") == names.count("mmae_block_backward") == 1
-        fwd, bwd = [None] + fwd, [None] + bwd
+    fwd = [a for n, a in rec.calls if n == "mmae_block_forward"]
+    bwd = [a for n, a in rec.calls if n == "mmae_block_backward"][::-1]      # issued for blocks 3..0
+    assert len(made) == 3 and len(fwd) == len(bwd) == 4
     for i, b in enumerate(blocks):
-        if fwd[i] is None:
-            continue
         own = made.get(id(b))
         prev = made.get(id(blocks[i - 1])) if (chain and i > 0) else None
         want = (None, None) if own is None else (own[0].data_ptr(), own[1].data_ptr())
@@ -154,37 +145,41 @@ def test_drop_path_entry_points_and_scale_pointers(rec, monkeypatch, chain):
         assert all(f[1] is None and f[4] is None for f in fwd[1:])              # each block adds its own MLP branch
 
 
-def test_eval_and_zero_rate_issue_todays_calls(rec, monkeypatch):
+def test_eval_and_zero_rate_pass_no_scales(rec, monkeypatch):
     """eval() or drop_path = 0: the same call sequence as a stack without DropPath modules; nothing is drawn."""
     monkeypatch.setattr(Fn, "BLOCK_CHAIN", True)
     x = torch.randn(2, 5, 128)
     stacks = (_stack(rate=0.0).train(), _stack(rate=0.3).eval())
     state = torch.get_rng_state()
-    seqs = []
+    seqs, chained, scale_args = [], [], []
+    block_calls = ("mmae_block_forward", "mmae_block_backward")
     for blocks in stacks:
         rec.calls.clear()
         xi = x.clone().requires_grad_(True)
         Fn.block_stack(blocks, xi).sum().backward()
         seqs.append(rec.names())
-    assert seqs[0] == seqs[1] and "mmae_block_forward_chain" in seqs[0]
-    assert not any(n.endswith("_dp") for n in seqs[0] + seqs[1])
+        chained.append(any(a[1] is not None for n, a in rec.calls if n == "mmae_block_forward"))     # x_add handed over
+        scale_args += [a[11:14] for n, a in rec.calls if n in block_calls]
+    assert seqs[0] == seqs[1] and all(chained)
     assert torch.equal(torch.get_rng_state(), state)
     from multimae_b200.multimae_utils import Block
     rec.calls.clear()
     b = Block(128, 2, qkv_bias=True, drop_path=0.2).eval()
     b(x.clone().requires_grad_(True)).sum().backward()
     assert rec.names().count("mmae_block_forward") == 1 and rec.names().count("mmae_block_backward") == 1
+    scale_args += [a[11:14] for n, a in rec.calls if n in block_calls]
+    assert len(scale_args) == 2 * 2 * 4 + 2 and all(s == (None, None, None) for s in scale_args)
 
 
-def test_block_with_drop_path_trains(rec):
+def test_stand_alone_block_with_drop_path_trains(rec):
     """A stand-alone Block with drop_path > 0 in training no longer raises; it draws its two [B] factors itself."""
     from multimae_b200.multimae_utils import Block, DropPath
     b = Block(128, 2, qkv_bias=True, drop_path=0.25).train()
     assert repr(b.drop_path) == "DropPath(p=0.25)" and not list(b.drop_path.state_dict())
     x = torch.randn(4, 5, 128, requires_grad=True)
     b(x).sum().backward()
-    (f,) = [a for n, a in rec.calls if n == "mmae_block_forward_dp"]
-    (g,) = [a for n, a in rec.calls if n == "mmae_block_backward_dp"]
+    (f,) = [a for n, a in rec.calls if n == "mmae_block_forward"]
+    (g,) = [a for n, a in rec.calls if n == "mmae_block_backward"]
     assert f[11] is not None and f[12] is not None and f[13] is None and f[11:14] == g[11:14]
     with pytest.raises(NotImplementedError, match="inside Block"):
         DropPath(0.25).train()(x)
@@ -210,9 +205,9 @@ def test_drop_path_scales_values():
     assert all(s is None for s in Fn.drop_path_scales(list(blocks.eval()), 4, torch.device("cpu")))
 
 
-def test_model_paths_reach_drop_path_entry_points(rec, monkeypatch):
+def test_model_paths_pass_drop_path_scales(rec, monkeypatch):
     """MultiMAE (encoder + every decoder_transformer, one adapter in the fp32 tier) and MultiViT with return_all_layers run
-    stochastic depth through the *_dp entry points when drop_path > 0 in training."""
+    stochastic depth through the block calls' scale arguments when drop_path > 0 in training."""
     from multimae_b200.multimae_utils import DropPath
     from test_host_api import _build
     model = _build(depth=3, dec_depth=2).train()
@@ -224,8 +219,15 @@ def test_model_paths_reach_drop_path_entry_points(rec, monkeypatch):
          "semseg": torch.randint(0, 133, (2, 16, 16))}
     preds, masks = model(x, num_encoded_tokens=12, fp32_output_adapters=["depth"])
     sum(v.float().sum() for v in preds.values()).backward()
-    names = rec.names()
-    assert names.count("mmae_block_forward_dp") == 3 + 3 * 2 and names.count("mmae_block_backward_dp") == 3 + 3 * 2
-    # the fp32 tier runs block by block: block 0 (p = 0) with the plain call, block 1 with factors
-    assert names.count("mmae_block_f32_forward_dp") == 1 and names.count("mmae_block_f32_backward_dp") == 1
-    assert names.count("mmae_block_f32_forward") == 1 and names.count("mmae_block_f32_backward") == 1
+    # bf16 tier: the 3 encoder blocks and the 3 two-block decoder transformers; every block with p > 0 (2 + 3 * 1) carries
+    # its own factors, and the encoder's block 2 also block 1's
+    for name in ("mmae_block_forward", "mmae_block_backward"):
+        scales = [a[11:14] for n, a in rec.calls if n == name]
+        assert len(scales) == 3 + 3 * 2, name
+        assert sum(s[0] is not None and s[1] is not None for s in scales) == 2 + 3 * 1, name
+        assert sum(s[0] is None and s[1] is None for s in scales) == 1 + 3 * 1, name
+        assert sum(s[2] is not None for s in scales) == 1, name
+    # the fp32 tier runs block by block: block 0 (p = 0) without factors, block 1 with them
+    for name in ("mmae_block_f32_forward", "mmae_block_f32_backward"):
+        scales = sorted((a[8:10] for n, a in rec.calls if n == name), key=lambda s: s[0] is None)
+        assert len(scales) == 2 and None not in scales[0] and scales[1] == (None, None), name

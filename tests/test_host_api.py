@@ -163,7 +163,7 @@ def test_ctypes_structs_match_the_c_header(tmp_path):
     assert L.ABI_VERSION == int(re.search(r"#define MMAE_ABI_VERSION (\d+)", open(header).read()).group(1))
 
 
-def test_c_abi_rejects_bad_arguments_before_any_launch():
+def test_c_abi_rejects_bad_arguments_with_messages():
     """Error behaviour of the C ABI (no GPU needed: every check fires before the first CUDA call): a non-zero code,
     the message behind mmae_last_error(), and the Python stub's exception (MmaeError, a RuntimeError like the reference's
     assertion failures, e.g. multimae/input_adapters.py:105-106)."""
@@ -173,39 +173,50 @@ def test_c_abi_rejects_bad_arguments_before_any_launch():
     ep = L.GemmEpilogue()
     ARG, UNSUPPORTED = 1, 3
     cases = [
-        (lib.mmae_gemm_bf16(None, 0, 0, None, 0, 0, 128, 128, 64, 1, ctypes.byref(ep), None), ARG, b"null operand"),
-        (lib.mmae_gemm_bf16(16, 64, 0, 16, 64, 0, 128, 100, 64, 1, ctypes.byref(ep), None), ARG, b"multiple of 8"),
-        (lib.mmae_standardize_depth(None, None, 1, 16, 1, 9, 1e-6, None, None), ARG, b"bad args"),
-        (lib.mmae_standardize_depth(16, 16, 1, 16, 9, 9, 1e-6, None, None), ARG, b"lo < hi"),
-        (lib.mmae_standardize_depth_set_variant(3), ARG, b"1 or 2"),
-        (lib.mmae_layernorm_forward(16, 100, 16, 16, 16, 100, None, 0, 16, 16, 4, 100, 1e-6, None), UNSUPPORTED, b"multiple of 128"),
-        (lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, None, 1, 1, 8, 8, 48, 0.1, None), UNSUPPORTED, b"head_dim 48"),
-        (lib.mmae_masked_loss_forward(5, 0, 0.0, 16, 16, None, 1, 3, 32, 32, 16, 16, 16, None), UNSUPPORTED, b"kind"),
+        (lambda: lib.mmae_gemm_bf16(None, 0, 0, None, 0, 0, 128, 128, 64, 1, ctypes.byref(ep), None), ARG, b"null operand"),
+        (lambda: lib.mmae_gemm_bf16(16, 64, 0, 16, 64, 0, 128, 100, 64, 1, ctypes.byref(ep), None), ARG, b"multiple of 8"),
+        (lambda: lib.mmae_standardize_depth(None, None, 1, 16, 1, 9, 1e-6, None, None), ARG, b"bad args"),
+        (lambda: lib.mmae_standardize_depth(16, 16, 1, 16, 9, 9, 1e-6, None, None), ARG, b"lo < hi"),
+        (lambda: lib.mmae_standardize_depth_set_variant(3), ARG, b"1 or 2"),
+        (lambda: lib.mmae_layernorm_forward(16, 100, 16, 16, 16, 100, None, 0, 16, 16, 4, 100, 1e-6, None), UNSUPPORTED,
+         b"multiple of 128"),
+        (lambda: lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, None, 1, 1, 8, 8, 48, 0.1, None), UNSUPPORTED,
+         b"head_dim 48"),
+        (lambda: lib.mmae_masked_loss_forward(5, 0, 0.0, 16, 16, None, 1, 3, 32, 32, 16, 16, 16, None), UNSUPPORTED, b"kind"),
     ]
-    # round-2 entry points: shared context projection, *_ctx heads, chained blocks
+    # round-2 entry points: shared context projection, *_ctx heads, blocks with hand-offs and stochastic depth
     cp = L.CtxProjParams()
     cp.num = 2
     cp.dim[0], cp.dim[1] = 256, 100                                      # 100 is not a multiple of 8
     cp.weight[0] = cp.weight[1] = cp.bias[0] = cp.bias[1] = 16
     bp, bg = L.BlockParams(), L.BlockGrads()
     cases += [
-        (lib.mmae_ctxproj_forward(16, 128, 768, ctypes.byref(cp), 16, 16, None), ARG, b"mmae_ctxproj_forward"),
-        (lib.mmae_ctxproj_forward(None, 128, 768, ctypes.byref(cp), 16, 16, None), ARG, b"mmae_ctxproj_forward"),
-        (lib.mmae_ctxproj_backward(128, 768, ctypes.byref(cp), ctypes.byref(L.CtxProjGrads()), None, 16, 16, None), ARG,
-         b"mmae_ctxproj_backward"),
-        (lib.mmae_dechead_forward_ctx(None, 1024, None, 8, 1024, 1e-6, None, None, None, None, None), ARG, b"bad args"),
-        (lib.mmae_dechead_backward_ctx(None, 8, 1024, None, None, None, None, 1024, None, None, None), ARG, b"bad args"),
+        (lambda: lib.mmae_ctxproj_forward(16, 128, 768, ctypes.byref(cp), 16, 16, None), ARG, b"mmae_ctxproj_forward"),
+        (lambda: lib.mmae_ctxproj_forward(None, 128, 768, ctypes.byref(cp), 16, 16, None), ARG, b"mmae_ctxproj_forward"),
+        (lambda: lib.mmae_ctxproj_backward(128, 768, ctypes.byref(cp), ctypes.byref(L.CtxProjGrads()), None, 16, 16, None),
+         ARG, b"mmae_ctxproj_backward"),
+        (lambda: lib.mmae_dechead_forward_ctx(None, 1024, None, 8, 1024, 1e-6, None, None, None, None, None), ARG, b"bad args"),
+        (lambda: lib.mmae_dechead_backward_ctx(None, 8, 1024, None, None, None, None, 1024, None, None, None), ARG, b"bad args"),
         # x_add without a buffer for the sum; neither x_out nor y_out; a bf16 gradient copy without its column-sum target
-        (lib.mmae_block_forward_chain(16, 16, None, 16, None, 2, 8, 128, 2, 512, 1e-6, ctypes.byref(bp), 16, 16, None), ARG,
-         b"mmae_block_forward"),
-        (lib.mmae_block_forward_chain(16, None, None, None, None, 2, 8, 128, 2, 512, 1e-6, ctypes.byref(bp), 16, 16, None), ARG,
-         b"mmae_block_forward"),
-        (lib.mmae_block_backward_chain(16, 16, None, 16, 16, None, 2, 8, 128, 2, 512, ctypes.byref(bp), ctypes.byref(bg), 16,
-                                       16, None), ARG, b"mmae_block_backward"),
+        (lambda: lib.mmae_block_forward(16, 16, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None, ctypes.byref(bp),
+                                        16, 16, None), ARG, b"mmae_block_forward"),
+        (lambda: lib.mmae_block_forward(16, None, None, None, None, 2, 8, 128, 2, 512, 1e-6, None, None, None,
+                                        ctypes.byref(bp), 16, 16, None), ARG, b"mmae_block_forward"),
+        (lambda: lib.mmae_block_backward(16, 16, None, 16, 16, None, 2, 8, 128, 2, 512, None, None, None, ctypes.byref(bp),
+                                         ctypes.byref(bg), 16, 16, None), ARG, b"mmae_block_backward"),
+        # the previous block's scale without the hand-off it scales
+        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, 16, ctypes.byref(bp),
+                                        16, 16, None), ARG, b"mmae_block_forward: the previous block's scale needs x_add"),
+        (lambda: lib.mmae_block_backward(16, 16, None, 16, None, None, 2, 8, 128, 2, 512, None, None, 16, ctypes.byref(bp),
+                                         ctypes.byref(bg), 16, 16, None), ARG,
+         b"mmae_block_backward: the previous block's scale needs dx_in_bf16"),
     ]
     assert lib.mmae_block_saved_x_mid(None, 2, 8, 128, 2, 512) is None
-    # mmae_last_error() holds the message of the most recent failure: re-issue each call to read its own message
-    assert [rc for rc, _, _ in cases] == [want for _, want, _ in cases]
+    # mmae_last_error() holds the message of the most recent failure: read it right after each call
+    got = [(call(), lib.mmae_last_error()) for call, _, _ in cases]
+    assert [rc for rc, _ in got] == [want for _, want, _ in cases]
+    for (_, err), (_, _, msg) in zip(got, cases):
+        assert msg in err, (msg, err)
     assert lib.mmae_gemm_bf16(16, 64, 0, 16, 64, 0, 128, 100, 64, 1, ctypes.byref(ep), None) == ARG
     assert b"N=100 must be a multiple of 8" in lib.mmae_last_error()
     with pytest.raises(L.MmaeError, match="multiple of 8"):

@@ -14,7 +14,11 @@ from test_host_api import _build
 
 class _StubLib:
     def __init__(self):
-        self.calls = []
+        self.calls = []        # names, in call order
+        self.log = []          # (name, args) of every call
+
+    def args_of(self, name):
+        return [a for n, a in self.log if n == name]
 
     def __getattr__(self, name):
         if name not in L.SIGNATURES:
@@ -28,6 +32,7 @@ class _StubLib:
                     continue
                 t.from_param(a)        # raises on a type the real ctypes call would reject
             self.calls.append(name)
+            self.log.append((name, args))
             if name.endswith("_bytes"):
                 return 4096
             if name == "mmae_abi_version":
@@ -53,7 +58,7 @@ def _inputs(B=2, size=64):
 
 
 @pytest.mark.parametrize("shared_ctx", [True, False])
-def test_forward_backward_plumbing(stub, monkeypatch, shared_ctx):
+def test_model_forward_backward_plumbing(stub, monkeypatch, shared_ctx):
     """shared_ctx: the four adapters' proj_context Linears as one GEMM (the default) or one per adapter (MMAE_SHARED_CTX=0)."""
     from multimae_b200 import multimae as MM
     from multimae_b200.criterion import MaskedCrossEntropyLoss, MaskedL1Loss, MaskedMSELoss
@@ -83,10 +88,13 @@ def test_forward_backward_plumbing(stub, monkeypatch, shared_ctx):
                  "mmae_block_backward", head_f, head_b, "mmae_dectail_forward",
                  "mmae_dectail_backward", "mmae_masked_loss_forward", "mmae_masked_loss_backward"):
         assert name in stub.calls, name
-    # the 2 encoder blocks run chained (one hand-off); the 4 one-block decoder transformers stay single blocks
+    # the 2 encoder blocks run chained (one hand-off: x_add / y_out forward, dx_out_bf16 / dx_in_bf16 backward); the 4
+    # one-block decoder transformers stay single blocks
     chained = 2 if shared_ctx else 0
-    assert stub.calls.count("mmae_block_forward") == 2 + 4 * 1 - chained and stub.calls.count(head_b) == 4
-    assert stub.calls.count("mmae_block_forward_chain") == stub.calls.count("mmae_block_backward_chain") == chained
+    fwd, bwd = stub.args_of("mmae_block_forward"), stub.args_of("mmae_block_backward")
+    assert len(fwd) == len(bwd) == 2 + 4 * 1 and stub.calls.count(head_b) == 4
+    assert sum(a[1] is not None or a[4] is not None for a in fwd) == chained
+    assert sum(a[2] is not None or a[4] is not None for a in bwd) == chained
     assert stub.calls.count("mmae_block_saved_x_mid") == chained // 2
     assert stub.calls.count("mmae_ctxproj_forward") == stub.calls.count("mmae_ctxproj_backward") == (1 if shared_ctx else 0)
     if shared_ctx:      # the shared projection's backward runs after the last head's, before the encoder's
@@ -211,8 +219,8 @@ def test_train_step_eager_and_sampling_options(stub):
     assert a.shape == (64, 3) and bool(((a > 0.5).sum(1) >= 1).all())      # never the all-zero task subset (:150)
 
 
-def test_block_stack_hand_off_pointers(monkeypatch):
-    """BlockStackFunction wires consecutive blocks through raw pointers: block i+1 must receive block i's x_mid (inside
+def test_block_stack_hand_off_arguments(monkeypatch):
+    """BlockFunction wires consecutive blocks through raw pointers: block i+1 must receive block i's x_mid (inside
     block i's `saved` buffer) as x_in and the shared MLP-output buffer as x_add; only the last block writes x_out; in backward
     block i+1 writes bf16(dx) into the buffer block i then reads, and its column sums into block i's fc2 bias gradient."""
     from multimae_b200.multimae_utils import Block
@@ -245,20 +253,20 @@ def test_block_stack_hand_off_pointers(monkeypatch):
         b.bind(arena, "%d." % i, lambda names: ready.append(list(names)))
     x = torch.randn(2, 5, 128, requires_grad=True)
     out = Fn.block_stack(blocks, x)
-    fwd = [a for n, a in calls if n == "mmae_block_forward_chain"]
+    fwd = [a for n, a in calls if n == "mmae_block_forward"]
     mids = [a for n, a in calls if n == "mmae_block_saved_x_mid"]
-    assert len(fwd) == 4 and len(mids) == 3 and not [n for n, _ in calls if n == "mmae_block_forward"]
-    # args: x_in, x_add, x_sum, x_out, y_out, ..., saved (index 12)
+    assert len(fwd) == 4 and len(mids) == 3
+    # args: x_in, x_add, x_sum, x_out, y_out, ..., saved (index 15)
     assert fwd[0][0] == x.data_ptr() and fwd[0][1] is None and fwd[0][2] is None        # first block: plain input
     y_buf = fwd[0][4]
     assert y_buf is not None and fwd[0][3] is None                                       # not the last: y_out, no x_out
     for i in (1, 2, 3):
-        assert fwd[i][0] == fwd[i - 1][12] + 64                  # x_in = x_mid of the block before (inside ITS saved buffer)
+        assert fwd[i][0] == fwd[i - 1][15] + 64                  # x_in = x_mid of the block before (inside ITS saved buffer)
         assert fwd[i][1] == y_buf and fwd[i][2] is not None      # x_add = the MLP branch output; the sum is materialised
     assert fwd[3][3] == out.data_ptr() and fwd[3][4] is None    # the last block adds by itself
-    assert len({a[12] for a in fwd}) == 4 and len({a[2] for a in fwd[1:]}) == 3          # own saved / x_sum buffers
+    assert len({a[15] for a in fwd}) == 4 and len({a[2] for a in fwd[1:]}) == 3          # own saved / x_sum buffers
     out.sum().backward()
-    bwd = [a for n, a in calls if n == "mmae_block_backward_chain"]
+    bwd = [a for n, a in calls if n == "mmae_block_backward"]
     assert len(bwd) == 4
     # args: x_in, dx_out, dx_out_bf16, dx_in, dx_in_bf16, dx_in_colsum, ...; issued for blocks 3, 2, 1, 0
     assert bwd[0][2] is None and bwd[3][4] is None and bwd[3][5] is None
