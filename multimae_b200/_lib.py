@@ -76,6 +76,11 @@ class BlockGrads(ctypes.Structure):
     _fields_ = [(n, c_void_p) for n in BLOCK_FIELDS]
 
 
+class BlockDropout(ctypes.Structure):
+    _fields_ = [("attn_p", c_float), ("proj_p", c_float), ("mlp_p", c_float), ("seed", c_void_p), ("prev_mlp_p", c_float),
+                ("prev_seed", c_void_p)]
+
+
 class DecoderIndex(ctypes.Structure):
     _fields_ = [("batch", c_int), ("dim", c_int), ("num_visible", c_int), ("num_global", c_int),
                 ("num_queries", c_int), ("total_tokens", c_int), ("num_tasks", c_int), ("own_task", c_int),
@@ -149,6 +154,12 @@ SIGNATURES = {
     "mmae_attention_backward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
                                         c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
                                         c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+    "mmae_attention_forward_drop": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
+                                            c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "mmae_attention_backward_drop": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
+                                             c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
+                                             c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+    "mmae_dropout_keep_mask": (c_int, [c_void_p, c_int, c_i64, c_int, c_float, c_void_p, c_void_p]),
     "mmae_sample_masks": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(c_int), c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),
     "mmae_embed_saved_bytes": (c_i64, [ctypes.POINTER(EmbedLayout), c_int, c_int, c_int]),
@@ -167,6 +178,13 @@ SIGNATURES = {
     "mmae_block_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                     c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams),
                                     ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
+    "mmae_block_forward_drop": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                        c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
+                                        ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
+    "mmae_block_backward_drop": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                         c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
+                                         ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
+                                         c_void_p]),
     "mmae_dechead_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -260,7 +278,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 def lib():

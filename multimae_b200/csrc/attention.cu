@@ -108,13 +108,24 @@ __device__ __forceinline__ void load_chunk_async(bf16* s, const bf16* gbase, int
 // =====================================================================================================================
 // forward
 // =====================================================================================================================
-template <int DH>
+// Attention dropout (Attention.attn_drop, multimae/multimae_utils.py:177) acts on the softmax probabilities P before P V.
+// Its site matrix is [B*H*Nq, Nk]: row (b*H + h)*Nq + i, column j.  With DROP the forward keeps lse undropped and multiplies
+// P by the mask before P V (the 1/(1-p) joins the final 1/l); the backward uses dV = (P*M/(1-p))^T dO and
+// dP = (dO V^T)*M/(1-p), and dS = P*(dP - delta) with delta = rowsum(dO * O) of the dropped O, unchanged.
+// factors of columns col, col + 1 (col even) of `row`
+__device__ __forceinline__ float2 dropout_factor2(const DropSite& d, uint64_t seed, uint64_t row, int col) {
+  const uint4 w = dropout_words(seed, d.site, row, col);
+  const bool hi = col & 2;
+  return make_float2((hi ? w.z : w.x) < d.thresh ? d.scale : 0.f, (hi ? w.w : w.y) < d.thresh ? d.scale : 0.f);
+}
+
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __restrict__ Q, int64_t ldq,
                                                                const bf16* __restrict__ K, int64_t ldk,
                                                                const bf16* __restrict__ V, int64_t ldv,
                                                                bf16* __restrict__ O, int64_t ldo,
                                                                float* __restrict__ lse, int Nq, int Nk, int H,
-                                                               float scale) {
+                                                               float scale, DropSite drop) {
   pdl_prologue();
   constexpr int LDS = DH + 8, LDT = ATT_CHUNK + 8;
   __shared__ __align__(16) bf16 sQ[ATT_ROWS * LDS];
@@ -142,6 +153,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __res
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const float sl2 = scale * LOG2E;
   const bool live = q0 + warp * 16 < Nq;
+  uint64_t dseed = 0, drow_a = 0;
+  if constexpr (DROP) {
+    dseed = *drop.seed;
+    drow_a = (uint64_t(b) * H + h) * Nq + q0 + warp * 16 + g;
+  }
 
   for (int k0 = 0, it = 0; k0 < Nk; k0 += ATT_CHUNK, ++it) {
     const bf16* sK = sKb[it & 1];
@@ -205,6 +221,17 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __res
         acc[j][0] *= alpha0; acc[j][1] *= alpha0;
         acc[j][2] *= alpha1; acc[j][3] *= alpha1;
       }
+      if constexpr (DROP) {   // the row sums above stay undropped; 0 / 1 here, 1/(1-p) at the end
+#pragma unroll
+        for (int j = 0; j < ATT_CHUNK / 8; ++j) {
+          const int key = k0 + j * 8 + 2 * t;
+          const float2 fa = dropout_factor2(drop, dseed, drow_a, key), fb = dropout_factor2(drop, dseed, drow_a + 8, key);
+          if (fa.x == 0.f) s[j][0] = 0.f;
+          if (fa.y == 0.f) s[j][1] = 0.f;
+          if (fb.x == 0.f) s[j][2] = 0.f;
+          if (fb.y == 0.f) s[j][3] = 0.f;
+        }
+      }
       // O += P V
 #pragma unroll
       for (int ks = 0; ks < ATT_CHUNK / 16; ++ks) {
@@ -230,7 +257,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_fwd_kernel(const bf16* __res
     l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
   }
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;
-  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+  float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+  if constexpr (DROP) {
+    inv0 *= drop.scale;
+    inv1 *= drop.scale;
+  }
   bf16* Ob = O + int64_t(b) * Nq * ldo + h * DH;
 #pragma unroll
   for (int jd = 0; jd < DH / 8; ++jd) {
@@ -288,7 +319,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict_
 // =====================================================================================================================
 // backward, part 1: dQ (query-stationary)
 // =====================================================================================================================
-template <int DH>
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const bf16* __restrict__ Q, int64_t ldq,
                                                                   const bf16* __restrict__ K, int64_t ldk,
                                                                   const bf16* __restrict__ V, int64_t ldv,
@@ -296,7 +327,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const bf16* __
                                                                   const float* __restrict__ lse,
                                                                   const float* __restrict__ delta,
                                                                   bf16* __restrict__ dQ, int64_t lddq, int Nq, int Nk,
-                                                                  int H, float scale) {
+                                                                  int H, float scale, DropSite drop) {
   pdl_prologue();
   constexpr int LDS = DH + 8, LDT = ATT_CHUNK + 8;
   __shared__ __align__(16) bf16 sA[ATT_ROWS * LDS];   // Q tile, then dO tile (staging for the A fragments)
@@ -330,6 +361,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const bf16* __
   const float lse_a = row_a < Nq ? Lp[row_a] * LOG2E : INFINITY, lse_b = row_b < Nq ? Lp[row_b] * LOG2E : INFINITY;
   const float del_a = row_a < Nq ? Dp[row_a] : 0.f, del_b = row_b < Nq ? Dp[row_b] : 0.f;
   const float sl2 = scale * LOG2E;
+  uint64_t dseed = 0;
+  const uint64_t drow_a = (uint64_t(b) * H + h) * Nq + row_a;
+  if constexpr (DROP) dseed = *drop.seed;
 
   float acc[DH / 8][4];
 #pragma unroll
@@ -363,6 +397,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const bf16* __
           mma_bf16_16816(dp, doa[kk], bv);
         }
         const int key = k0 + n0 + 2 * t;
+        if constexpr (DROP) {   // dP = (dO V^T) * M / (1-p)
+          const float2 fa = dropout_factor2(drop, dseed, drow_a, key), fb = dropout_factor2(drop, dseed, drow_a + 8, key);
+          dp[0] *= fa.x; dp[1] *= fa.y; dp[2] *= fb.x; dp[3] *= fb.y;
+        }
         const bool v0 = key < Nk, v1 = key + 1 < Nk;
         const float p0 = v0 ? fast_exp2(s[0] * sl2 - lse_a) : 0.f, p1 = v1 ? fast_exp2(s[1] * sl2 - lse_a) : 0.f;
         const float p2 = v0 ? fast_exp2(s[2] * sl2 - lse_b) : 0.f, p3 = v1 ? fast_exp2(s[3] * sl2 - lse_b) : 0.f;
@@ -390,7 +428,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dq_kernel(const bf16* __
 // =====================================================================================================================
 // backward, part 2: dK, dV (key-stationary; works on transposed score tiles S^T = K Q^T)
 // =====================================================================================================================
-template <int DH>
+// factors of the transposed tile elements a thread holds: keys key_a, key_a + 8 (rows of S^T) x queries q, q + 1 (columns)
+// -> {(key_a, q), (key_a, q+1), (key_a + 8, q), (key_a + 8, q+1)}, the order of an mma accumulator fragment
+__device__ __forceinline__ float4 dropout_factor_t(const DropSite& d, uint64_t seed, uint64_t qrow, int key_a) {
+  return make_float4(dropout_factor(d, seed, qrow, key_a), dropout_factor(d, seed, qrow + 1, key_a),
+                     dropout_factor(d, seed, qrow, key_a + 8), dropout_factor(d, seed, qrow + 1, key_a + 8));
+}
+
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const bf16* __restrict__ Q, int64_t ldq,
                                                                    const bf16* __restrict__ K, int64_t ldk,
                                                                    const bf16* __restrict__ V, int64_t ldv,
@@ -399,7 +444,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const bf16* _
                                                                    const float* __restrict__ delta,
                                                                    bf16* __restrict__ dK, int64_t lddk,
                                                                    bf16* __restrict__ dV, int64_t lddv, int Nq, int Nk,
-                                                                   int H, float scale) {
+                                                                   int H, float scale, DropSite drop) {
   pdl_prologue();
   constexpr int LDS = DH + 8, LDT = ATT_CHUNK + 8;
   __shared__ __align__(16) bf16 sQb[2][ATT_CHUNK * LDS];
@@ -435,6 +480,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const bf16* _
     dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f;
   }
   const float sl2 = scale * LOG2E;
+  uint64_t dseed = 0;
+  const uint64_t dbase = (uint64_t(b) * H + h) * Nq;
+  if constexpr (DROP) dseed = *drop.seed;
 
   // query chunks stream through two buffers: Q, dO rows and their lse / delta arrive by cp.async while the previous chunk
   // is consumed.  Rows past Nq are zero-filled: Q = dO = 0 and delta = 0 make their P and dS contributions vanish.
@@ -482,8 +530,15 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_bwd_dkv_kernel(const bf16* _
         const float l0 = sLse[qc] * LOG2E, l1 = sLse[qc + 1] * LOG2E, d0 = sDel[qc], d1 = sDel[qc + 1];
         const float p0 = fast_exp2(s[0] * sl2 - l0), p1 = fast_exp2(s[1] * sl2 - l1);
         const float p2 = fast_exp2(s[2] * sl2 - l0), p3 = fast_exp2(s[3] * sl2 - l1);
-        pa[half * 2 + 0] = pack_bf16x2(p0, p1);
-        pa[half * 2 + 1] = pack_bf16x2(p2, p3);
+        if constexpr (DROP) {
+          const float4 f = dropout_factor_t(drop, dseed, dbase + q0 + qc, k0 + warp * 16 + g);
+          pa[half * 2 + 0] = pack_bf16x2(p0 * f.x, p1 * f.y);
+          pa[half * 2 + 1] = pack_bf16x2(p2 * f.z, p3 * f.w);
+          dp[0] *= f.x; dp[1] *= f.y; dp[2] *= f.z; dp[3] *= f.w;
+        } else {
+          pa[half * 2 + 0] = pack_bf16x2(p0, p1);
+          pa[half * 2 + 1] = pack_bf16x2(p2, p3);
+        }
         dsa[half * 2 + 0] = pack_bf16x2(p0 * (dp[0] - d0), p1 * (dp[1] - d1));
         dsa[half * 2 + 1] = pack_bf16x2(p2 * (dp[2] - d0), p3 * (dp[3] - d1));
       }
@@ -563,12 +618,12 @@ __device__ __forceinline__ void load_a_frag_t(uint32_t (&a)[4], const bf16* s, i
                : "r"(smem_u32(p)));
 }
 
-template <int DH>
+template <int DH, bool DROP>
 __global__ void __launch_bounds__(FB_MAX_KEYS / 16 * 32) attn_bwd_fused_kernel(
     const bf16* __restrict__ Q, int64_t ldq, const bf16* __restrict__ K, int64_t ldk, const bf16* __restrict__ V,
     int64_t ldv, const bf16* __restrict__ O, int64_t ldo, const bf16* __restrict__ dO, int64_t lddo,
     const float* __restrict__ lse, bf16* __restrict__ dQ, int64_t lddq, bf16* __restrict__ dK, int64_t lddk,
-    bf16* __restrict__ dV, int64_t lddv, int Nq, int Nk, int H, float scale) {
+    bf16* __restrict__ dV, int64_t lddv, int Nq, int Nk, int H, float scale, DropSite drop) {
   pdl_prologue();
   constexpr int LDS = DH + 8, SE = fb_stream_elems<DH>();
   static_assert(LDS <= FB_LDD, "V is staged in the dS^T tile");
@@ -616,6 +671,9 @@ __global__ void __launch_bounds__(FB_MAX_KEYS / 16 * 32) attn_bwd_fused_kernel(
   }
   const float sl2 = scale * LOG2E;
   const bool key_a = warp * 16 + g < Nk, key_b = warp * 16 + g + 8 < Nk;
+  uint64_t dseed = 0;
+  const uint64_t dbase = (uint64_t(b) * H + h) * Nq;
+  if constexpr (DROP) dseed = *drop.seed;
 
   for (int q0 = 0, it = 0; q0 < Nq; q0 += ATT_CHUNK, ++it) {
     const int buf = it & 1;
@@ -674,8 +732,15 @@ __global__ void __launch_bounds__(FB_MAX_KEYS / 16 * 32) attn_bwd_fused_kernel(
         const float l0 = sL[qc] * LOG2E, l1 = sL[qc + 1] * LOG2E, d0 = sDel[qc], d1 = sDel[qc + 1];
         const float p0 = key_a ? fast_exp2(s[half][0] * sl2 - l0) : 0.f, p1 = key_a ? fast_exp2(s[half][1] * sl2 - l1) : 0.f;
         const float p2 = key_b ? fast_exp2(s[half][2] * sl2 - l0) : 0.f, p3 = key_b ? fast_exp2(s[half][3] * sl2 - l1) : 0.f;
-        pa[half * 2 + 0] = pack_bf16x2(p0, p1);
-        pa[half * 2 + 1] = pack_bf16x2(p2, p3);
+        if constexpr (DROP) {
+          const float4 f = dropout_factor_t(drop, dseed, dbase + q0 + qc, warp * 16 + g);
+          pa[half * 2 + 0] = pack_bf16x2(p0 * f.x, p1 * f.y);
+          pa[half * 2 + 1] = pack_bf16x2(p2 * f.z, p3 * f.w);
+          dp[half][0] *= f.x; dp[half][1] *= f.y; dp[half][2] *= f.z; dp[half][3] *= f.w;
+        } else {
+          pa[half * 2 + 0] = pack_bf16x2(p0, p1);
+          pa[half * 2 + 1] = pack_bf16x2(p2, p3);
+        }
         dsa[half * 2 + 0] = pack_bf16x2(p0 * (dp[half][0] - d0), p1 * (dp[half][1] - d1));
         dsa[half * 2 + 1] = pack_bf16x2(p2 * (dp[half][2] - d0), p3 * (dp[half][3] - d1));
       }
@@ -736,11 +801,12 @@ __global__ void __launch_bounds__(FB_MAX_KEYS / 16 * 32) attn_bwd_fused_kernel(
 
 bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-template <int DH>
+template <int DH, bool DROP>
 int launch_bwd_fused(const bf16* q, int64_t ldq, const bf16* k, int64_t ldk, const bf16* v, int64_t ldv, const bf16* o,
                      int64_t ldo, const bf16* d_o, int64_t lddo, const float* lse, bf16* dq, int64_t lddq, bf16* dk,
-                     int64_t lddk, bf16* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale, cudaStream_t st) {
-  auto kern = attn_bwd_fused_kernel<DH>;
+                     int64_t lddk, bf16* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale, DropSite drop,
+                     cudaStream_t st) {
+  auto kern = attn_bwd_fused_kernel<DH, DROP>;
   static bool configured = false;
   if (!configured) {
     MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(fb_smem_bytes<DH>(FB_MAX_KEYS))));
@@ -748,10 +814,58 @@ int launch_bwd_fused(const bf16* q, int64_t ldq, const bf16* k, int64_t ldk, con
   }
   const int nwarps = ceil_div(Nk, 16);
   launch_k(kern, dim3(B * H), dim3(nwarps * 32), fb_smem_bytes<DH>(nwarps * 16), st, q, ldq, k, ldk, v, ldv, o, ldo, d_o,
-           lddo, lse, dq, lddq, dk, lddk, dv, lddv, Nq, Nk, H, scale);
+           lddo, lse, dq, lddq, dk, lddk, dv, lddv, Nq, Nk, H, scale, drop);
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;
+}
+
+unsigned delta_grid(int B, int Nq, int H, int dh) {
+  const int64_t total = int64_t(B) * Nq * H * (dh / 8);
+  return (unsigned)std::min<int64_t>((total + 255) / 256, int64_t(sm_count()) * 16);
+}
+
+// backward above FB_MAX_KEYS keys: delta, then dQ (query-stationary) and dK / dV (key-stationary)
+template <int DH, bool DROP>
+int launch_bwd_split(const bf16* q, int64_t ldq, const bf16* k, int64_t ldk, const bf16* v, int64_t ldv, const bf16* o,
+                     int64_t ldo, const bf16* d_o, int64_t lddo, const float* lse, float* delta_ws, bf16* dq, int64_t lddq,
+                     bf16* dk, int64_t lddk, bf16* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale,
+                     DropSite drop, cudaStream_t st) {
+  dim3 gq(ceil_div(Nq, ATT_ROWS), H, B), gk(ceil_div(Nk, ATT_ROWS), H, B);
+  launch_k(attn_delta_kernel<DH>, delta_grid(B, Nq, H, DH), 256, 0, st, o, ldo, d_o, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
+  launch_k(attn_bwd_dq_kernel<DH, DROP>, gq, ATT_THREADS, 0, st, q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq,
+           Nq, Nk, H, scale, drop);
+  launch_k(attn_bwd_dkv_kernel<DH, DROP>, gk, ATT_THREADS, 0, st, q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dk, lddk,
+           dv, lddv, Nq, Nk, H, scale, drop);
+  count_launch();
+  count_launch();
+  count_launch();
+  MMAE_LAUNCH_OK();
+  return MMAE_OK;
+}
+
+template <int DH, bool DROP>
+int launch_bwd(const bf16* q, int64_t ldq, const bf16* k, int64_t ldk, const bf16* v, int64_t ldv, const bf16* o,
+               int64_t ldo, const bf16* d_o, int64_t lddo, const float* lse, float* delta_ws, bf16* dq, int64_t lddq,
+               bf16* dk, int64_t lddk, bf16* dv, int64_t lddv, int B, int H, int Nq, int Nk, float scale, DropSite drop,
+               cudaStream_t st) {
+  if (Nk <= FB_MAX_KEYS)   // one fused kernel per (b, h); delta_ws is not used
+    return launch_bwd_fused<DH, DROP>(q, ldq, k, ldk, v, ldv, o, ldo, d_o, lddo, lse, dq, lddq, dk, lddk, dv, lddv, B, H, Nq,
+                                      Nk, scale, drop, st);
+  return launch_bwd_split<DH, DROP>(q, ldq, k, ldk, v, ldv, o, ldo, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv,
+                                    B, H, Nq, Nk, scale, drop, st);
+}
+
+// keep bits of rows x cols elements of one site, 0 / 1 bytes (mmae_dropout_keep_mask)
+__global__ void __launch_bounds__(256) dropout_keep_mask_kernel(DropSite drop, int64_t rows, int cols, uint8_t* __restrict__ out) {
+  pdl_prologue();
+  const uint64_t seed = *drop.seed;
+  const int64_t n = rows * cols;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += int64_t(gridDim.x) * blockDim.x) {
+    const int64_t r = i / cols;
+    const int c = int(i - r * cols);
+    out[i] = uint8_t(word_at(dropout_words(seed, drop.site, uint64_t(r), c), c & 3) < drop.thresh);
+  }
 }
 
 }  // namespace
@@ -764,6 +878,7 @@ using namespace mmae;
 // 4 | 64 = wgmma backward (any length); the forward above 256 keys and the backward without those bits use the warp-level
 // mma.sync kernels of this file (bit 16 selected a persistent variant that has no Hopper kernel and is ignored).
 // 0 = mma.sync kernels everywhere; their backward is the fused kernel up to 256 keys, delta + dQ + dK/dV above.
+// Attention dropout (p > 0) runs the mma.sync kernels whatever the mask selects: the wgmma kernels have no dropout.
 // Default 0 (env MMAE_ATTN_TC), from scripts/gpu_time_attention.py on one H100 80GB HBM3 at a 700 W power limit,
 // MultiMAE-B bs 128, us per call (forward mma.sync / wgmma, backward mma.sync fused / wgmma; in brackets, from the same
 // run, the forward before idle warps skipped their work and the delta + dQ + dK/dV backward the fused kernel replaced):
@@ -785,38 +900,46 @@ extern "C" int mmae_attention_set_tc(int enable) {
   return MMAE_OK;
 }
 
-extern "C" int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                      void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
-                                      float scale, void* stream) {
+// Dropout (the _drop entry points with p > 0) always runs the mma.sync kernels of this file, whatever MMAE_ATTN_TC selects:
+// the wgmma kernels have no dropout.  At p = 0 the _drop entry points are the plain ones.
+extern "C" int mmae_attention_forward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                           int64_t ldv, void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk,
+                                           int head_dim, float scale, float dropout_p, const uint64_t* seed, void* stream) {
   MMAE_CHECK(q && k && v && o && B > 0 && H > 0 && Nq > 0 && Nk > 0, MMAE_ERR_ARG, "mmae_attention_forward: bad args");
   MMAE_CHECK(head_dim == 32 || head_dim == 64, MMAE_ERR_UNSUPPORTED, "mmae_attention_forward: head_dim %d (32|64)", head_dim);
   MMAE_CHECK(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && aligned16(q) && aligned16(k) &&
                  aligned16(v) && aligned16(o),
              MMAE_ERR_ARG, "mmae_attention_forward: 16-byte alignment / ld %% 8 required");
+  MMAE_CHECK(dropout_p >= 0.f && dropout_p <= 1.f && (dropout_p == 0.f || seed), MMAE_ERR_ARG,
+             "mmae_attention_forward_drop: dropout p in [0, 1] and, when p > 0, a seed are required");
+  const DropSite drop = make_drop_site(seed, MMAE_DROP_SITE_ATTN, dropout_p);
   dim3 grid(ceil_div(Nq, ATT_ROWS), H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (attn_wg_fwd_supported(Nk, head_dim) && ((Nk <= 128 && (g_attn_tc & 1)) || (Nk > 128 && (g_attn_tc & (2 | 8 | 32 | 128)))))
+  if (!drop.seed && attn_wg_fwd_supported(Nk, head_dim) &&
+      ((Nk <= 128 && (g_attn_tc & 1)) || (Nk > 128 && (g_attn_tc & (2 | 8 | 32 | 128)))))
     return attn_wg_forward(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, st);
   const bf16 *qp = (const bf16*)q, *kp = (const bf16*)k, *vp = (const bf16*)v;
-  if (head_dim == 64)
-    launch_k(attn_fwd_kernel<64>, grid, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, (bf16*)o, ldo, lse, Nq, Nk, H, scale);
-  else
-    launch_k(attn_fwd_kernel<32>, grid, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, (bf16*)o, ldo, lse, Nq, Nk, H, scale);
+  auto kern = head_dim == 64 ? (drop.seed ? attn_fwd_kernel<64, true> : attn_fwd_kernel<64, false>)
+                             : (drop.seed ? attn_fwd_kernel<32, true> : attn_fwd_kernel<32, false>);
+  launch_k(kern, grid, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, (bf16*)o, ldo, lse, Nq, Nk, H, scale, drop);
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;
 }
 
-static unsigned delta_grid(int B, int Nq, int H, int dh) {
-  const int64_t total = int64_t(B) * Nq * H * (dh / 8);
-  return (unsigned)std::min<int64_t>((total + 255) / 256, int64_t(sm_count()) * 16);
+extern "C" int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                      void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
+                                      float scale, void* stream) {
+  return mmae_attention_forward_drop(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, 0.f, nullptr,
+                                     stream);
 }
 
-extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                                       int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
-                                       const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
-                                       int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
-                                       int head_dim, float scale, void* stream) {
+extern "C" int mmae_attention_backward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                            int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
+                                            const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
+                                            int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
+                                            int head_dim, float scale, float dropout_p, const uint64_t* seed,
+                                            void* stream) {
   MMAE_CHECK(q && k && v && o && d_o && lse && delta_ws && dq && dk && dv && B > 0 && H > 0 && Nq > 0 && Nk > 0,
              MMAE_ERR_ARG, "mmae_attention_backward: bad args");
   MMAE_CHECK(head_dim == 32 || head_dim == 64, MMAE_ERR_UNSUPPORTED, "mmae_attention_backward: head_dim %d (32|64)", head_dim);
@@ -824,11 +947,13 @@ extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k
                  lddk % 8 == 0 && lddv % 8 == 0 && aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) &&
                  aligned16(d_o) && aligned16(dq) && aligned16(dk) && aligned16(dv),
              MMAE_ERR_ARG, "mmae_attention_backward: 16-byte alignment / ld %% 8 required");
+  MMAE_CHECK(dropout_p >= 0.f && dropout_p <= 1.f && (dropout_p == 0.f || seed), MMAE_ERR_ARG,
+             "mmae_attention_backward_drop: dropout p in [0, 1] and, when p > 0, a seed are required");
+  const DropSite drop = make_drop_site(seed, MMAE_DROP_SITE_ATTN, dropout_p);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bf16 *qp = (const bf16*)q, *kp = (const bf16*)k, *vp = (const bf16*)v, *op = (const bf16*)o,
              *dop = (const bf16*)d_o;
-  dim3 gq(ceil_div(Nq, ATT_ROWS), H, B), gk(ceil_div(Nk, ATT_ROWS), H, B);
-  if (g_attn_tc & (4 | 64)) {   // wgmma backward (attention_wgmma.cu) behind the delta kernel
+  if (!drop.seed && (g_attn_tc & (4 | 64))) {   // wgmma backward (attention_wgmma.cu) behind the delta kernel
     if (head_dim == 64)
       launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
     else
@@ -838,28 +963,32 @@ extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k
     return attn_wg_backward(q, ldq, k, ldk, v, ldv, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv, B, H, Nq, Nk,
                             head_dim, scale, st);
   }
-  if (Nk <= FB_MAX_KEYS) {   // one fused kernel per (b, h); delta_ws is not used
-    if (head_dim == 64)
-      return launch_bwd_fused<64>(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, (bf16*)dq, lddq, (bf16*)dk, lddk,
-                                  (bf16*)dv, lddv, B, H, Nq, Nk, scale, st);
-    return launch_bwd_fused<32>(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, (bf16*)dq, lddq, (bf16*)dk, lddk,
-                                (bf16*)dv, lddv, B, H, Nq, Nk, scale, st);
+  auto run = head_dim == 64 ? (drop.seed ? launch_bwd<64, true> : launch_bwd<64, false>)
+                            : (drop.seed ? launch_bwd<32, true> : launch_bwd<32, false>);
+  return run(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, delta_ws, (bf16*)dq, lddq, (bf16*)dk, lddk, (bf16*)dv, lddv,
+             B, H, Nq, Nk, scale, drop, st);
+}
+
+extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                       int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
+                                       const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
+                                       int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
+                                       int head_dim, float scale, void* stream) {
+  return mmae_attention_backward_drop(q, ldq, k, ldk, v, ldv, o, ldo, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv,
+                                      B, H, Nq, Nk, head_dim, scale, 0.f, nullptr, stream);
+}
+
+extern "C" int mmae_dropout_keep_mask(const uint64_t* seed, int site, int64_t rows, int cols, float p, void* out,
+                                      void* stream) {
+  MMAE_CHECK(seed && out && rows > 0 && cols > 0 && p >= 0.f && p <= 1.f, MMAE_ERR_ARG, "mmae_dropout_keep_mask: bad args");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (p == 0.f) {   // a site at p = 0 drops nothing
+    MMAE_CUDA_OK(cudaMemsetAsync(out, 1, size_t(rows) * cols, st));
+    return MMAE_OK;
   }
-  if (head_dim == 64) {
-    launch_k(attn_delta_kernel<64>, delta_grid(B, Nq, H, 64), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
-    launch_k(attn_bwd_dq_kernel<64>, gq, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, dop, lddo, lse, delta_ws, (bf16*)dq,
-                                                       lddq, Nq, Nk, H, scale);
-    launch_k(attn_bwd_dkv_kernel<64>, gk, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, dop, lddo, lse, delta_ws, (bf16*)dk,
-                                                        lddk, (bf16*)dv, lddv, Nq, Nk, H, scale);
-  } else {
-    launch_k(attn_delta_kernel<32>, delta_grid(B, Nq, H, 32), 256, 0, st, op, ldo, dop, lddo, delta_ws, Nq, H, int64_t(B) * Nq);
-    launch_k(attn_bwd_dq_kernel<32>, gq, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, dop, lddo, lse, delta_ws, (bf16*)dq,
-                                                       lddq, Nq, Nk, H, scale);
-    launch_k(attn_bwd_dkv_kernel<32>, gk, ATT_THREADS, 0, st, qp, ldq, kp, ldk, vp, ldv, dop, lddo, lse, delta_ws, (bf16*)dk,
-                                                        lddk, (bf16*)dv, lddv, Nq, Nk, H, scale);
-  }
-  count_launch();
-  count_launch();
+  const int64_t n = rows * cols;
+  launch_k(dropout_keep_mask_kernel, (unsigned)std::min<int64_t>((n + 255) / 256, int64_t(sm_count()) * 16), 256, 0, st,
+           make_drop_site(seed, site, p), rows, cols, static_cast<uint8_t*>(out));
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;

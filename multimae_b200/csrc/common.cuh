@@ -74,7 +74,59 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Dropout (nn.Dropout in training, multimae/multimae_utils.py:154,177,181).  The keep bit of element (row, col) of a
+// site's [rows, cols] matrix is word (col & 3) of Philox4x32-10 at counter {col >> 2, row lo, row hi, site} under the key
+// *seed, compared with `thresh` = (1 - p) * 2^32.  Forward and backward regenerate the same bits, so no mask is stored.
+// seed == nullptr: the site drops nothing (and the kernels skip the generator entirely).
+// ---------------------------------------------------------------------------------------------
+struct DropSite {
+  const uint64_t* seed;   // device pointer: a captured graph reads the value of each replay
+  uint32_t site;
+  uint32_t thresh;        // keep iff u32 < thresh
+  float scale;            // 1 / (1 - p) for a kept element (0 at p = 1)
+};
+inline DropSite make_drop_site(const uint64_t* seed, int site, float p) {
+  DropSite d;
+  d.seed = p > 0.f ? seed : nullptr;
+  d.site = uint32_t(site);
+  const double t = (1.0 - double(p)) * 4294967296.0;
+  d.thresh = t >= 4294967295.0 ? 0xFFFFFFFFu : (t <= 0.0 ? 0u : uint32_t(t));
+  d.scale = p < 1.f ? 1.0f / (1.0f - p) : 0.f;
+  return d;
+}
+
 #ifdef __CUDACC__
+
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+// the four random words of columns [4 (col >> 2), 4 (col >> 2) + 4) of `row`
+__device__ __forceinline__ uint4 dropout_words(uint64_t seed, uint32_t site, uint64_t row, int col) {
+  return philox4x32_10(make_uint4(uint32_t(col) >> 2, uint32_t(row), uint32_t(row >> 32), site),
+                       make_uint2(uint32_t(seed), uint32_t(seed >> 32)));
+}
+__device__ __forceinline__ uint32_t word_at(const uint4& w, int i) {
+  return i == 0 ? w.x : (i == 1 ? w.y : (i == 2 ? w.z : w.w));
+}
+// factor of element (row, col): scale when kept, 0 when dropped
+__device__ __forceinline__ float dropout_factor(const DropSite& d, uint64_t seed, uint64_t row, int col) {
+  return word_at(dropout_words(seed, d.site, row, col), col & 3) < d.thresh ? d.scale : 0.f;
+}
+// factors of the four columns 4k .. 4k+3 of `row` (col0 a multiple of 4)
+__device__ __forceinline__ float4 dropout_factor4(const DropSite& d, uint64_t seed, uint64_t row, int col0) {
+  const uint4 w = dropout_words(seed, d.site, row, col0);
+  return make_float4(w.x < d.thresh ? d.scale : 0.f, w.y < d.thresh ? d.scale : 0.f, w.z < d.thresh ? d.scale : 0.f,
+                     w.w < d.thresh ? d.scale : 0.f);
+}
 
 // ---------------------------------------------------------------------------------------------
 // small device utilities

@@ -77,14 +77,15 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, bf16* __rest
 
 // Tile: ROWS_PER_BLOCK rows x 128 columns; block (32, 8).  Each thread owns 4 consecutive columns.
 
-template <bool SRC_BF16>
+template <bool SRC_BF16, bool DROP>
 __global__ void __launch_bounds__(256) cast_colsum_kernel(const void* __restrict__ src_, int64_t ld_src,
                                                           bf16* __restrict__ dst, int64_t ld_dst,
                                                           float* __restrict__ colsum, float* __restrict__ partial,
                                                           unsigned int* __restrict__ counters, int M, int N,
                                                           int rows_per_block, const float* __restrict__ row_scale,
-                                                          int rows_per_sample) {
+                                                          int rows_per_sample, DropSite drop) {
   pdl_prologue();
+  const uint64_t dseed = DROP ? *drop.seed : 0;
   __shared__ float4 red[8][32];
   __shared__ float red2[8 * 32 * 5];
   const int col = blockIdx.x * 128 + threadIdx.x * 4;
@@ -103,6 +104,10 @@ __global__ void __launch_bounds__(256) cast_colsum_kernel(const void* __restrict
         if (row_scale != nullptr) {   // per-sample factor (stochastic depth) on the cast copy and on the column sums
           const float sc = __ldg(row_scale + r / rows_per_sample);
           v = make_float4(sc * v.x, sc * v.y, sc * v.z, sc * v.w);
+        }
+        if constexpr (DROP) {   // dropout of the branch this gradient enters: its mask and 1/(1-p)
+          const float4 f = dropout_factor4(drop, dseed, uint64_t(r), col);
+          v = make_float4(f.x * v.x, f.y * v.y, f.z * v.z, f.w * v.w);
         }
         if (dst) {
           uint2 o;
@@ -341,11 +346,13 @@ __global__ void __launch_bounds__(256) dgelu_colsum_kernel(const bf16* __restric
 // out[i] = x[i] + s * y[i]   (residual add of a branch output onto the fp32 stream; y bf16 or fp32)
 // s = row_scale[i / per_sample] (stochastic depth: 0 or 1/keep per sample), 1 without row_scale - then x + 1 * y == x + y
 // exactly, with or without FMA contraction.  x == null: out = s * y (the fp32 tier's scaled copy of a branch gradient).
-template <bool Y_BF16>
+template <bool Y_BF16, bool DROP>
 __global__ void __launch_bounds__(256) add_bf16_f32_kernel(const float* __restrict__ x, const void* __restrict__ y_,
                                                            float* __restrict__ out, int64_t n,
-                                                           const float* __restrict__ row_scale, int64_t per_sample) {
+                                                           const float* __restrict__ row_scale, int64_t per_sample,
+                                                           DropSite drop, int drop_cols) {
   pdl_prologue();
+  const uint64_t dseed = DROP ? *drop.seed : 0;
   const int64_t stride = int64_t(gridDim.x) * blockDim.x * 8;
   for (int64_t i = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) * 8; i < n; i += stride) {
     const float4 a = x != nullptr ? __ldg(reinterpret_cast<const float4*>(x + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -361,6 +368,13 @@ __global__ void __launch_bounds__(256) add_bf16_f32_kernel(const float* __restri
       y1 = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(y_) + i + 4));
     }
     const float s = row_scale != nullptr ? __ldg(row_scale + i / per_sample) : 1.0f;   // per_sample % 8 == 0
+    if constexpr (DROP) {   // dropout of the branch, element (i / drop_cols, i % drop_cols); drop_cols % 8 == 0
+      const int64_t r = i / drop_cols;
+      const int c = int(i - r * drop_cols);
+      const float4 f0 = dropout_factor4(drop, dseed, uint64_t(r), c), f1 = dropout_factor4(drop, dseed, uint64_t(r), c + 4);
+      y0 = make_float4(f0.x * y0.x, f0.y * y0.y, f0.z * y0.z, f0.w * y0.w);
+      y1 = make_float4(f1.x * y1.x, f1.y * y1.y, f1.z * y1.z, f1.w * y1.w);
+    }
     *reinterpret_cast<float4*>(out + i) = make_float4(a.x + s * y0.x, a.y + s * y0.y, a.z + s * y0.z, a.w + s * y0.w);
     *reinterpret_cast<float4*>(out + i + 4) = make_float4(b.x + s * y1.x, b.y + s * y1.y, b.z + s * y1.z, b.w + s * y1.w);
   }
@@ -529,7 +543,7 @@ extern "C" int mmae_cast_f32_to_bf16(const float* src, void* dst_bf16, int64_t n
 }
 
 int mmae::cast_colsum_f32_scaled(const float* src, int64_t ld_src, bf16* dst_bf16, int64_t ld_dst, float* colsum,
-                                 const float* row_scale, int rows_per_sample, int M, int N, void* stream) {
+                                 const float* row_scale, int rows_per_sample, int M, int N, void* stream, DropSite drop) {
   MMAE_CHECK(src && M > 0 && N > 0 && N % 4 == 0 && ld_src % 4 == 0 && (!dst_bf16 || ld_dst % 4 == 0), MMAE_ERR_ARG,
              "mmae_cast_colsum_f32: bad args (N, ld must be multiples of 4)");
   MMAE_CHECK(!row_scale || (rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
@@ -542,9 +556,9 @@ int mmae::cast_colsum_f32_scaled(const float* src, int64_t ld_src, bf16* dst_bf1
     partial = colred_scratch(size_t(grid.y) * N, cst);
     if (!partial) return MMAE_ERR_CUDA;
   }
-  launch_k(cast_colsum_kernel<false>, grid, block, 0, cst, src, ld_src, dst_bf16, ld_dst, colsum, partial,
+  launch_k(drop.seed ? cast_colsum_kernel<false, true> : cast_colsum_kernel<false, false>, grid, block, 0, cst, src, ld_src, dst_bf16, ld_dst, colsum, partial,
                                                      g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb, row_scale,
-                                                     rows_per_sample);
+                                                     rows_per_sample, drop);
   count_launch();
   MMAE_LAUNCH_OK();
   if (partial && !g_colred_fold) return colred_finalize(partial, grid.y, N, N, colsum, nullptr, nullptr, cst);
@@ -573,9 +587,9 @@ extern "C" int mmae_colsum_bf16(const void* src_bf16, int64_t ld_src, float* col
     launch_k(colsum_bf16_kernel, grid, block, 0, cst, reinterpret_cast<const bf16*>(src_bf16), ld_src, colsum, partial,
                                                 g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb);
   else
-    launch_k(cast_colsum_kernel<true>, grid, block, 0, cst, src_bf16, ld_src, nullptr, 0, colsum, partial,
+    launch_k(cast_colsum_kernel<true, false>, grid, block, 0, cst, src_bf16, ld_src, nullptr, 0, colsum, partial,
                                                       g_colred_fold ? colred_counters(partial) : nullptr, M, N, rpb,
-                                                      nullptr, 1);
+                                                      nullptr, 1, DropSite());
   count_launch();
   MMAE_LAUNCH_OK();
   if (partial && !g_colred_fold) return colred_finalize(partial, grid.y, N, N, colsum, nullptr, nullptr, cst);
@@ -611,20 +625,21 @@ extern "C" int mmae_gelu_bf16(const void* z, void* io, int64_t n, int backward, 
 }
 
 int mmae::add_scaled_f32(const float* x, const void* y, int y_is_bf16, const float* row_scale, int64_t per_sample, float* out,
-                         int64_t n, void* stream) {
+                         int64_t n, void* stream, DropSite drop, int drop_cols) {
   MMAE_CHECK(y && out && n >= 0 && n % 8 == 0, MMAE_ERR_ARG, "mmae_add_bf16_f32: bad args (n %% 8)");
   MMAE_CHECK(x || row_scale, MMAE_ERR_ARG, "mmae_add_bf16_f32: null x");
   MMAE_CHECK(!row_scale || (per_sample > 0 && per_sample % 8 == 0 && n % per_sample == 0), MMAE_ERR_ARG,
              "mmae_add_bf16_f32: a row scale needs a multiple of 8 elements per sample dividing n");
+  MMAE_CHECK(!drop.seed || (drop_cols > 0 && drop_cols % 8 == 0 && n % drop_cols == 0), MMAE_ERR_ARG,
+             "mmae_add_bf16_f32: a dropout mask needs a multiple of 8 columns dividing n");
   if (n == 0) return MMAE_OK;
   int64_t blocks = (n / 8 + 255) / 256;
   const int64_t cap = int64_t(sm_count()) * 16;
   if (blocks > cap) blocks = cap;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (y_is_bf16)
-    launch_k(add_bf16_f32_kernel<true>, (unsigned)blocks, 256, 0, st, x, y, out, n, row_scale, per_sample);
-  else
-    launch_k(add_bf16_f32_kernel<false>, (unsigned)blocks, 256, 0, st, x, y, out, n, row_scale, per_sample);
+  auto kern = y_is_bf16 ? (drop.seed ? add_bf16_f32_kernel<true, true> : add_bf16_f32_kernel<true, false>)
+                        : (drop.seed ? add_bf16_f32_kernel<false, true> : add_bf16_f32_kernel<false, false>);
+  launch_k(kern, (unsigned)blocks, 256, 0, st, x, y, out, n, row_scale, per_sample, drop, drop_cols);
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;

@@ -57,22 +57,26 @@ int launch_cast2d(const float* src, int64_t ld_src, bf16* dst, int64_t ld_dst, i
 
 // Row-scaled forms of the streaming kernels behind stochastic depth (drop path).  `row_scale` is one fp32 factor per sample,
 // row r of the [M, D] activation belonging to sample r / rows_per_sample; a null row_scale gives the plain kernel.
+// `drop` (dropout of a branch): element (r, c) of the branch is further multiplied by its keep factor at site drop (0 or
+// 1/(1-p), common.cuh); a default DropSite (null seed) drops nothing and leaves the arithmetic as without it.
 // layernorm.cu: x_sum = x + s * addend, then LayerNorm
 int add_layernorm_forward_scaled(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, const float* row_scale,
                                  int rows_per_sample, float* x_sum, int64_t ldsum, const float* gamma, const float* beta,
-                                 bf16* y_bf16, int64_t ldy, float* mean, float* rstd, int M, int D, float eps, void* stream);
+                                 bf16* y_bf16, int64_t ldy, float* mean, float* rstd, int M, int D, float eps, void* stream,
+                                 DropSite drop = DropSite());
 // layernorm.cu: mmae_layernorm_backward_ex with bf16(dx) and colsum(dx) multiplied by s (dx itself unscaled)
 int layernorm_backward_ex_scaled(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx, const float* mean,
                                  const float* rstd, const float* gamma, const float* dx_resid, int64_t ldr, float* dx,
                                  int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16, int64_t lddxb, float* dx_colsum,
-                                 const float* row_scale, int rows_per_sample, int M, int D, void* stream);
+                                 const float* row_scale, int rows_per_sample, int M, int D, void* stream,
+                                 DropSite drop = DropSite());
 // elementwise.cu: dst = bf16(s * src), colsum += column sums of s * src
 int cast_colsum_f32_scaled(const float* src, int64_t ld_src, bf16* dst, int64_t ld_dst, float* colsum, const float* row_scale,
-                           int rows_per_sample, int M, int N, void* stream);
+                           int rows_per_sample, int M, int N, void* stream, DropSite drop = DropSite());
 // elementwise.cu: out = x + s * y over n contiguous elements, `per_sample` elements per sample; y is bf16 (y_is_bf16) or
-// fp32; x may be null (out = s * y, a scaled copy)
+// fp32; x may be null (out = s * y, a scaled copy).  With `drop`, y is a [n / drop_cols, drop_cols] matrix.
 int add_scaled_f32(const float* x, const void* y, int y_is_bf16, const float* row_scale, int64_t per_sample, float* out,
-                   int64_t n, void* stream);
+                   int64_t n, void* stream, DropSite drop = DropSite(), int drop_cols = 0);
 // cls_head.cu: dst[i] += src[i] over n contiguous fp32 elements (any n)
 int add_f32(float* dst, const float* src, int64_t n, cudaStream_t st);
 

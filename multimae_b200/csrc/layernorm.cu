@@ -13,7 +13,7 @@ namespace {
 constexpr int LN_WARPS = 8;
 
 // D = NVEC * 128 (each lane owns NVEC float4, strided by 32 lanes)
-template <int NVEC>
+template <int NVEC, bool DROP>
 __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __restrict__ x, int64_t ldx,
                                                                const bf16* __restrict__ addend, int64_t ldadd,
                                                                float* __restrict__ x_sum, int64_t ldsum,
@@ -23,7 +23,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
                                                                float* __restrict__ mean_out,
                                                                float* __restrict__ rstd_out,
                                                                const float* __restrict__ add_scale, int rows_per_sample,
-                                                               int M, float eps) {
+                                                               int M, float eps, DropSite drop) {
   pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * LN_WARPS + warp;
@@ -32,6 +32,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
   const float* xr = x + int64_t(row) * ldx;
   // per-sample factor of the addend (stochastic depth: 0 or 1/keep); 1 when none is given, which leaves x + a exact
   const float sc = add_scale != nullptr ? __ldg(add_scale + row / rows_per_sample) : 1.0f;
+  const uint64_t dseed = DROP ? *drop.seed : 0;
   float4 v[NVEC];
   float s = 0.f;
 #pragma unroll
@@ -41,7 +42,12 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_kernel(const float* __re
     if (addend != nullptr) {   // residual add fused in front of the normalisation: x <- x + bf16 branch output
       const uint2 u = __ldg(reinterpret_cast<const uint2*>(addend + int64_t(row) * ldadd + c));
       const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y);
-      v[i].x += sc * a.x; v[i].y += sc * a.y; v[i].z += sc * b.x; v[i].w += sc * b.y;
+      if constexpr (DROP) {   // dropout of the branch: per-element factor 0 or 1/(1-p)
+        const float4 f = dropout_factor4(drop, dseed, uint64_t(row), c);
+        v[i].x += sc * f.x * a.x; v[i].y += sc * f.y * a.y; v[i].z += sc * f.z * b.x; v[i].w += sc * f.w * b.y;
+      } else {
+        v[i].x += sc * a.x; v[i].y += sc * a.y; v[i].z += sc * b.x; v[i].w += sc * b.y;
+      }
       if (x_sum != nullptr) *reinterpret_cast<float4*>(x_sum + int64_t(row) * ldsum + c) = v[i];
     }
     s += v[i].x + v[i].y + v[i].z + v[i].w;
@@ -121,7 +127,7 @@ __device__ __forceinline__ float4 ln_row_dy(const LnRow<NVEC, DY_BF16>& r, int i
   }
 }
 
-template <int NVEC, bool DY_BF16>
+template <int NVEC, bool DY_BF16, bool DROP>
 __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __restrict__ dy_, int64_t lddy,
                                                                const float* __restrict__ x, int64_t ldx,
                                                                const float* __restrict__ mean_in,
@@ -132,7 +138,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
                                                                float* __restrict__ partial, bool want_colsum,
                                                                bf16* __restrict__ dx_bf16, int64_t lddxb,
                                                                const float* __restrict__ out_scale, int rows_per_sample,
-                                                               int M) {
+                                                               int M, DropSite drop) {
   pdl_prologue();
   constexpr int D = NVEC * 128;
   __shared__ float4 red[LN_WARPS][32];
@@ -149,6 +155,7 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
   }
   const int row_stride = gridDim.x * LN_WARPS;
   int row = blockIdx.x * LN_WARPS + warp;
+  const uint64_t dseed = DROP ? *drop.seed : 0;
   LnRow<NVEC, DY_BF16> cur, nxt;
   float mean = 0.f, rstd = 0.f, mean_n = 0.f, rstd_n = 0.f;
   if (row < M) {
@@ -198,7 +205,11 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
       *reinterpret_cast<float4*>(dx + int64_t(row) * lddx + c) = o;
       if (dx_bf16 != nullptr) {   // bf16 copy of dx (next GEMM operand) and its column sums (next bias gradient)
         uint2 pk;
-        const float4 os = make_float4(sc * o.x, sc * o.y, sc * o.z, sc * o.w);
+        float4 os = make_float4(sc * o.x, sc * o.y, sc * o.z, sc * o.w);
+        if constexpr (DROP) {   // the gradient entering a dropout branch: the forward's mask and 1/(1-p)
+          const float4 f = dropout_factor4(drop, dseed, uint64_t(row), c);
+          os = make_float4(os.x * f.x, os.y * f.y, os.z * f.z, os.w * f.w);
+        }
         pk.x = pack_bf16x2(os.x, os.y);
         pk.y = pack_bf16x2(os.z, os.w);
         *reinterpret_cast<uint2*>(dx_bf16 + int64_t(row) * lddxb + c) = pk;
@@ -242,7 +253,7 @@ using namespace mmae;
 static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, float* x_sum, int64_t ldsum,
                            const float* gamma, const float* beta, void* y_bf16, int64_t ldy, float* y_f32, int64_t ldyf,
                            float* mean, float* rstd, const float* add_scale, int rows_per_sample, int M, int D, float eps,
-                           void* stream) {
+                           void* stream, DropSite drop = DropSite()) {
   MMAE_CHECK(x && gamma && beta && (y_bf16 || y_f32) && M > 0, MMAE_ERR_ARG, "mmae_layernorm_forward: bad args");
   MMAE_CHECK(!add_scale || (addend && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
              "mmae_add_layernorm_forward: a row scale needs an addend and rows-per-sample dividing M=%d", M);
@@ -251,10 +262,10 @@ static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int6
   dim3 grid(ceil_div(M, LN_WARPS)), block(LN_WARPS * 32);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   bf16* yb = reinterpret_cast<bf16*>(y_bf16);
-#define LN_CASE(NV)                                                                                            \
-  case NV:                                                                                                     \
-    launch_k(ln_fwd_kernel<NV>, grid, block, 0, st, x, ldx, addend, ldadd, x_sum, ldsum, gamma, beta, yb, ldy, y_f32, ldyf, \
-                                              mean, rstd, add_scale, rows_per_sample, M, eps);                                          \
+#define LN_CASE(NV)                                                                                                         \
+  case NV:                                                                                                                  \
+    launch_k(drop.seed ? ln_fwd_kernel<NV, true> : ln_fwd_kernel<NV, false>, grid, block, 0, st, x, ldx, addend, ldadd, x_sum, \
+             ldsum, gamma, beta, yb, ldy, y_f32, ldyf, mean, rstd, add_scale, rows_per_sample, M, eps, drop);                  \
     break;
   switch (D / 128) {
     LN_CASE(1) LN_CASE(2) LN_CASE(3) LN_CASE(4) LN_CASE(5) LN_CASE(6) LN_CASE(7) LN_CASE(8)
@@ -279,10 +290,10 @@ extern "C" int mmae_layernorm_forward(const float* x, int64_t ldx, const float* 
 int mmae::add_layernorm_forward_scaled(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, const float* row_scale,
                                        int rows_per_sample, float* x_sum, int64_t ldsum, const float* gamma, const float* beta,
                                        bf16* y_bf16, int64_t ldy, float* mean, float* rstd, int M, int D, float eps,
-                                       void* stream) {
+                                       void* stream, DropSite drop) {
   MMAE_CHECK(addend && ldadd % 4 == 0 && (!x_sum || ldsum % 4 == 0), MMAE_ERR_ARG, "mmae_add_layernorm_forward: bad args");
   return ln_forward_impl(x, ldx, addend, ldadd, x_sum, ldsum, gamma, beta, y_bf16, ldy, nullptr, 0, mean, rstd, row_scale,
-                         rows_per_sample, M, D, eps, stream);
+                         rows_per_sample, M, D, eps, stream, drop);
 }
 
 extern "C" int mmae_add_layernorm_forward(const float* x, int64_t ldx, const void* addend_bf16, int64_t ldadd, float* x_sum,
@@ -295,10 +306,12 @@ extern "C" int mmae_add_layernorm_forward(const float* x, int64_t ldx, const voi
 static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx, const float* mean,
                             const float* rstd, const float* gamma, const float* dx_resid, int64_t ldr, float* dx,
                             int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16, int64_t lddxb, float* dx_colsum,
-                            const float* out_scale, int rows_per_sample, int M, int D, void* stream) {
+                            const float* out_scale, int rows_per_sample, int M, int D, void* stream,
+                            DropSite drop = DropSite()) {
   MMAE_CHECK(dy && x && mean && rstd && gamma && dx && M > 0, MMAE_ERR_ARG, "mmae_layernorm_backward: bad args");
   MMAE_CHECK(!out_scale || (dx_bf16 && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
              "mmae_layernorm_backward_ex: a row scale needs the bf16 output and rows-per-sample dividing M=%d", M);
+  MMAE_CHECK(!drop.seed || dx_bf16, MMAE_ERR_ARG, "mmae_layernorm_backward_ex: a dropout mask needs the bf16 output");
   MMAE_CHECK(D % 128 == 0 && D <= 1024 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0 && ldr % 4 == 0,
              MMAE_ERR_UNSUPPORTED, "mmae_layernorm_backward: D=%d must be a multiple of 128 and <= 1024", D);
   // one wave: resident blocks per SM follow from the register footprint of the per-lane column accumulators
@@ -315,14 +328,10 @@ static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const 
   if (!partial) return MMAE_ERR_CUDA;
 #define LNB_CASE(NV)                                                                                              \
   case NV:                                                                                                        \
-    if (dy_is_bf16)                                                                                               \
-      launch_k(ln_bwd_kernel<NV, true>, grid, block, 0, st, dy, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx,     \
-                                                      lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb,     \
-                                                      out_scale, rows_per_sample, M);                            \
-    else                                                                                                          \
-      launch_k(ln_bwd_kernel<NV, false>, grid, block, 0, st, dy, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx,    \
-                                                       lddx, partial, dx_colsum != nullptr, dx_bf16, lddxb,     \
-                                                       out_scale, rows_per_sample, M);                           \
+    launch_k(dy_is_bf16 ? (drop.seed ? ln_bwd_kernel<NV, true, true> : ln_bwd_kernel<NV, true, false>)             \
+                        : (drop.seed ? ln_bwd_kernel<NV, false, true> : ln_bwd_kernel<NV, false, false>),          \
+             grid, block, 0, st, dy, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, partial,           \
+             dx_colsum != nullptr, dx_bf16, lddxb, out_scale, rows_per_sample, M, drop);                          \
     break;
   switch (D / 128) {
     LNB_CASE(1) LNB_CASE(2) LNB_CASE(3) LNB_CASE(4) LNB_CASE(5) LNB_CASE(6) LNB_CASE(7) LNB_CASE(8)
@@ -349,10 +358,10 @@ int mmae::layernorm_backward_ex_scaled(const void* dy, int dy_is_bf16, int64_t l
                                        const float* mean, const float* rstd, const float* gamma, const float* dx_resid,
                                        int64_t ldr, float* dx, int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16,
                                        int64_t lddxb, float* dx_colsum, const float* row_scale, int rows_per_sample, int M,
-                                       int D, void* stream) {
+                                       int D, void* stream, DropSite drop) {
   MMAE_CHECK(!dx_bf16 || lddxb % 4 == 0, MMAE_ERR_ARG, "mmae_layernorm_backward_ex: bad bf16 leading dimension");
   return ln_backward_impl(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta, dx_bf16,
-                          lddxb, dx_colsum, row_scale, rows_per_sample, M, D, stream);
+                          lddxb, dx_colsum, row_scale, rows_per_sample, M, D, stream, drop);
 }
 
 // same, additionally emitting bf16(dx) and colsum += sum_rows(dx): the operand and bias gradient of the next Linear backward

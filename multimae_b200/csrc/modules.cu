@@ -344,14 +344,51 @@ extern "C" int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hi
 // x_out is not written, and the block's output is x_mid (mmae_block_saved_x_mid) + y_out - the next block's (x_in, x_add).
 // Stochastic depth: s_attn / s_mlp [B] multiply the attention / MLP branch of each sample inside the residual adds, s_prev [B]
 // multiplies x_add (the previous block's MLP branch).  Null: factor 1.
+// Dropout: the three sites of this block from drop->seed, the previous block's MLP site from drop->prev_seed.  A null
+// `drop` or rate 0 gives a DropSite with a null seed: the kernels below then run exactly as without dropout.
+namespace {
+struct BlockDrop {
+  float attn_p;
+  const uint64_t* seed;
+  DropSite proj, mlp, prev;
+};
+int block_drop(const mmae_block_dropout* d, bool has_prev, const char* who, BlockDrop* out) {
+  const mmae_block_dropout z = {0.f, 0.f, 0.f, nullptr, 0.f, nullptr};
+  const mmae_block_dropout& r = d ? *d : z;
+  auto ok = [](float p) { return p >= 0.f && p <= 1.f; };
+  MMAE_CHECK(ok(r.attn_p) && ok(r.proj_p) && ok(r.mlp_p) && ok(r.prev_mlp_p), MMAE_ERR_ARG, "%s: dropout rates must lie in [0, 1]",
+             who);
+  MMAE_CHECK((r.attn_p == 0.f && r.proj_p == 0.f && r.mlp_p == 0.f) || r.seed, MMAE_ERR_ARG, "%s: dropout needs a seed", who);
+  MMAE_CHECK(r.prev_mlp_p == 0.f || (r.prev_seed && has_prev), MMAE_ERR_ARG,
+             "%s: the previous block's dropout needs its seed and the hand-off it applies to", who);
+  out->attn_p = r.attn_p;
+  out->seed = r.seed;
+  out->proj = make_drop_site(r.seed, MMAE_DROP_SITE_PROJ, r.proj_p);
+  out->mlp = make_drop_site(r.seed, MMAE_DROP_SITE_MLP, r.mlp_p);
+  out->prev = make_drop_site(r.prev_seed, MMAE_DROP_SITE_MLP, r.prev_mlp_p);
+  return MMAE_OK;
+}
+}  // namespace
+
 extern "C" int mmae_block_forward(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
                                   int B, int N, int D, int H, int hidden, float eps, const float* s_attn, const float* s_mlp,
                                   const float* s_prev, const mmae_block_params* p, void* saved, void* ws, void* st) {
+  return mmae_block_forward_drop(x_in, x_add_bf16, x_sum, x_out, y_out_bf16, B, N, D, H, hidden, eps, s_attn, s_mlp, s_prev,
+                                 nullptr, p, saved, ws, st);
+}
+
+extern "C" int mmae_block_forward_drop(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out,
+                                       void* y_out_bf16, int B, int N, int D, int H, int hidden, float eps,
+                                       const float* s_attn, const float* s_mlp, const float* s_prev,
+                                       const mmae_block_dropout* drop, const mmae_block_params* p, void* saved, void* ws,
+                                       void* st) {
   const bf16* x_add = static_cast<const bf16*>(x_add_bf16);
   bf16* y_out = static_cast<bf16*>(y_out_bf16);
   MMAE_CHECK(x_in && (x_out || y_out) && (!x_add || x_sum) && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0,
              MMAE_ERR_ARG, "mmae_block_forward: bad args");
   MMAE_CHECK(!s_prev || x_add, MMAE_ERR_ARG, "mmae_block_forward: the previous block's scale needs x_add");
+  BlockDrop dr;
+  RUN(block_drop(drop, x_add != nullptr, "mmae_block_forward_drop", &dr));
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(saved, B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, int64_t(3) * D * D, true, st));
@@ -365,22 +402,22 @@ extern "C" int mmae_block_forward(const float* x_in, const void* x_add_bf16, flo
   // x = x + attn(norm1(x))                                       multimae_utils.py:230
   if (x_add) {   // the previous block's `x = x + mlp(..)` (multimae_utils.py:231) fused in front of this block's norm1
     RUN(add_layernorm_forward_scaled(x_in, D, x_add, D, s_prev, N, x_sum, D, p->norm1_w, p->norm1_b, s.h1, D, s.mean1, s.rstd1,
-                                     M, D, eps, st));
+                                     M, D, eps, st, dr.prev));
     x_in = x_sum;
   } else {
     RUN(mmae_layernorm_forward(x_in, D, p->norm1_w, p->norm1_b, s.h1, D, nullptr, 0, s.mean1, s.rstd1, M, D, eps, st));
   }
   RUN(linear_bf16(s.h1, s.wqkv, p->qkv_b, s.qkv, M, 3 * D, D, st));
-  RUN(mmae_attention_forward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, s.lse, B, H, N, N, dh,
-                             1.0f / sqrtf((float)dh), st));
+  RUN(mmae_attention_forward_drop(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, s.lse, B, H, N, N, dh,
+                                  1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
   RUN(linear_bf16(s.o, s.wproj, p->proj_b, y, M, D, D, st));
   // x = x + mlp(norm2(x))                                        multimae_utils.py:231  (add fused in front of norm2)
   RUN(add_layernorm_forward_scaled(x_in, D, y, D, s_attn, N, s.x_mid, D, p->norm2_w, p->norm2_b, s.h2, D, s.mean2, s.rstd2, M,
-                                   D, eps, st));
+                                   D, eps, st, dr.proj));
   RUN(linear_gelu(s.h2, s.w1, p->fc1_b, s.z, s.a, M, hidden, D, st));
   if (y_out) return linear_bf16(s.a, s.w2, p->fc2_b, y_out, M, D, hidden, st);   // the add is the next block's first kernel
   RUN(linear_bf16(s.a, s.w2, p->fc2_b, y, M, D, hidden, st));
-  RUN(add_scaled_f32(s.x_mid, y, 1, s_mlp, int64_t(N) * D, x_out, int64_t(M) * D, st));
+  RUN(add_scaled_f32(s.x_mid, y, 1, s_mlp, int64_t(N) * D, x_out, int64_t(M) * D, st, dr.mlp, D));
   return MMAE_OK;
 }
 
@@ -399,11 +436,24 @@ extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const
                                    void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
                                    const float* s_attn, const float* s_mlp, const float* s_prev, const mmae_block_params* p,
                                    const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+  return mmae_block_backward_drop(x_in, dx_out, dx_out_bf16, dx_in, dx_in_bf16, dx_in_colsum, B, N, D, H, hidden, s_attn,
+                                  s_mlp, s_prev, nullptr, p, g, saved, ws, st);
+}
+
+// Dropout: the same factors as forward on the gradient entering each branch - fc2's operand and bias gradient (unless the
+// next block's backward made them), proj's from LN2's backward, the previous block's from LN1's - and on dP in attention.
+extern "C" int mmae_block_backward_drop(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
+                                        void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
+                                        const float* s_attn, const float* s_mlp, const float* s_prev,
+                                        const mmae_block_dropout* drop, const mmae_block_params* p,
+                                        const mmae_block_grads* g, const void* saved, void* ws, void* st) {
   const bf16* dx_out_b = static_cast<const bf16*>(dx_out_bf16);
   bf16* dx_in_b = static_cast<bf16*>(dx_in_bf16);
   MMAE_CHECK(x_in && dx_out && dx_in && (!dx_in_b || dx_in_colsum) && p && g && saved && ws, MMAE_ERR_ARG,
              "mmae_block_backward: bad args");
   MMAE_CHECK(!s_prev || dx_in_b, MMAE_ERR_ARG, "mmae_block_backward: the previous block's scale needs dx_in_bf16");
+  BlockDrop dr;
+  RUN(block_drop(drop, dx_in_b != nullptr, "mmae_block_backward_drop", &dr));
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(const_cast<void*>(saved), B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, 0, false, st));
@@ -418,7 +468,7 @@ extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const
   // ---- MLP branch
   const bf16* gout = dx_out_b;
   if (!gout) {
-    RUN(cast_colsum_f32_scaled(dx_out, D, w.g, D, g->fc2_b, s_mlp, N, M, D, st));
+    RUN(cast_colsum_f32_scaled(dx_out, D, w.g, D, g->fc2_b, s_mlp, N, M, D, st, dr.mlp));
     gout = w.g;
   }
   if (side) RUN(side_fork(st, 0));
@@ -429,21 +479,21 @@ extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const
   RUN(dgrad_bf16(w.big, hidden, s.w1, nullptr, w.dh, M, hidden, D, st));
   // LN2 backward also emits bf16(dx_mid) and its column sums = operand and bias gradient of the proj backward
   RUN(layernorm_backward_ex_scaled(w.dh, 1, D, s.x_mid, D, s.mean2, s.rstd2, p->norm2_w, dx_out, D, w.dx_mid, D, g->norm2_w,
-                                   g->norm2_b, g2, D, g->proj_b, s_attn, N, M, D, st));
+                                   g->norm2_b, g2, D, g->proj_b, s_attn, N, M, D, st, dr.proj));
   // ---- attention branch
   if (side) RUN(side_fork(st, 2));
   RUN(wgrad(g2, D, s.o, D, g->proj_w, M, D, D, ws_st));
   RUN(dgrad_bf16(g2, D, s.wproj, nullptr, w.d_o, M, D, D, st));
-  RUN(mmae_attention_backward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, w.d_o, D, s.lse, w.delta,
-                              dqkv, 3 * D, dqkv + D, 3 * D, dqkv + 2 * D, 3 * D, B, H, N, N, dh,
-                              1.0f / sqrtf((float)dh), st));
+  RUN(mmae_attention_backward_drop(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, w.d_o, D, s.lse, w.delta,
+                                   dqkv, 3 * D, dqkv + D, 3 * D, dqkv + 2 * D, 3 * D, B, H, N, N, dh,
+                                   1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
   RUN(mmae_colsum_bf16(dqkv, 3 * D, g->qkv_b, M, 3 * D, st));
   if (side) RUN(side_fork(st, 3));
   RUN(wgrad(dqkv, 3 * D, s.h1, D, g->qkv_w, M, 3 * D, D, ws_st));
   RUN(dgrad_bf16(dqkv, 3 * D, s.wqkv, nullptr, w.dh, M, 3 * D, D, st));
   if (dx_in_b)
     RUN(layernorm_backward_ex_scaled(w.dh, 1, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
-                                     g->norm1_b, dx_in_b, D, dx_in_colsum, s_prev, N, M, D, st));
+                                     g->norm1_b, dx_in_b, D, dx_in_colsum, s_prev, N, M, D, st, dr.prev));
   else
     RUN(mmae_layernorm_backward(w.dh, 1, D, x_in, D, s.mean1, s.rstd1, p->norm1_w, w.dx_mid, D, dx_in, D, g->norm1_w,
                                 g->norm1_b, M, D, st));

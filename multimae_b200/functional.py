@@ -160,6 +160,54 @@ def drop_path_scales(blocks, batch, device):
     return out
 
 
+def dropout_rates(block):
+    """(attn_p, proj_p, mlp_p) that apply to `block` in this call: the rates of its Attention.attn_drop,
+    Attention.proj_drop and Mlp.drop (multimae/multimae_utils.py:154,177,181) in training mode, else zeros."""
+    if not block.training:
+        return (0.0, 0.0, 0.0)
+    return (float(block.attn.attn_drop.p), float(block.attn.proj_drop.p), float(block.mlp.drop.p))
+
+
+def dropout_seeds(blocks, device):
+    """Dropout seeds for one run of consecutive Blocks: one entry per block, None when the block drops nothing in this call,
+    else a 0-dim int64 tensor on `device` from which the kernels derive the block's three masks (counter-based, nothing is
+    stored).  All seeds come from ONE torch.randint on `device`; no host synchronisation, so it can be captured in a CUDA
+    graph and every replay draws anew."""
+    live = [i for i, b in enumerate(blocks) if any(p > 0.0 for p in dropout_rates(b))]
+    out = [None] * len(blocks)
+    if not live:
+        return out
+    seeds = torch.randint(0, 2 ** 63 - 1, (len(live),), dtype=torch.int64, device=device)
+    for j, i in enumerate(live):
+        out[i] = seeds[j]
+    return out
+
+
+def block_dropouts(blocks, device, fp32=False):
+    """One entry per block: None when the block drops nothing in this call, else (attn_p, proj_p, mlp_p, seed) with the seed
+    from dropout_seeds.  The fp32 tier has no dropout kernels: a live rate there raises."""
+    if fp32 and any(any(p > 0.0 for p in dropout_rates(b)) for b in blocks):
+        raise NotImplementedError("multimae_b200: dropout in training is not supported in the fp32 tier "
+                                  "(fp32_output_adapters); set the adapter's drop rates to 0 or run it in eval mode")
+    seeds = dropout_seeds(blocks, device)
+    return [None if s is None else dropout_rates(b) + (s,) for b, s in zip(blocks, seeds)]
+
+
+def _block_dropout_arg(drops, i, chained):
+    """ctypes BlockDropout for block i of a stack, or None when neither its own sites nor (chained) the previous block's MLP
+    site drop anything - then the plain entry points run."""
+    own = drops[i]
+    prev = drops[i - 1] if chained and i > 0 else None
+    if own is None and (prev is None or prev[2] == 0.0):
+        return None
+    d = L.BlockDropout()
+    if own is not None:
+        d.attn_p, d.proj_p, d.mlp_p, d.seed = own[0], own[1], own[2], own[3].data_ptr()
+    if prev is not None and prev[2] > 0.0:
+        d.prev_mlp_p, d.prev_seed = prev[2], prev[3].data_ptr()
+    return d
+
+
 BLOCK_PARAM_NAMES = ["norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight",
                      "attn.proj.bias", "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias", "mlp.fc2.weight",
                      "mlp.fc2.bias"]
@@ -177,12 +225,16 @@ class BlockFunction(torch.autograd.Function):
     i's s_mlp, the factor of the MLP branch it adds in front of its first LayerNorm (forward) and of the bf16 gradient it
     hands down (backward).
 
+    Dropout: `drops` holds one block_dropouts entry per block (None: no dropout).  A block with one calls the _drop entry
+    points with its rates and seed, forward and backward; block i+1 also receives block i's mlp rate and seed, for the same
+    reason it receives s_mlp.  Blocks without any make exactly the plain calls.
+
     args: x, metas (one dict per block, all of one shape; metas[0]["fp32"]: the fp32 tier of `fp32_output_adapters` - 3 x
-    bf16 split GEMMs, fp32 attention / GELU - for one block), scales, then the 12 BLOCK_PARAM_NAMES tensors of every
+    bf16 split GEMMs, fp32 attention / GELU - for one block), scales, drops, then the 12 BLOCK_PARAM_NAMES tensors of every
     block."""
 
     @staticmethod
-    def forward(ctx, x, metas, scales, *params):
+    def forward(ctx, x, metas, scales, drops, *params):
         _require_cuda(x, "Block")
         lib = L.lib()
         n, P = len(metas), len(BLOCK_PARAM_NAMES)
@@ -208,16 +260,22 @@ class BlockFunction(torch.autograd.Function):
                 L.check(lib.mmae_block_f32_forward(x_ptr, out.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
                                                    ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
                         "mmae_block_f32_forward")
-            else:
+            elif _block_dropout_arg(drops, i, add_ptr is not None) is None:
                 L.check(lib.mmae_block_forward(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
                                                None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
                                                s_prev, ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
                                                L.current_stream()), "mmae_block_forward")
+            else:
+                L.check(lib.mmae_block_forward_drop(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
+                                                    None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
+                                                    s_prev, ctypes.byref(_block_dropout_arg(drops, i, add_ptr is not None)),
+                                                    ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                        "mmae_block_forward_drop")
             xs.append(x if x_sum is None else x_sum)
             saveds.append(saved)
             if not last:       # the next block's input: this block's x_mid (inside `saved`) + y
                 x_ptr, add_ptr = lib.mmae_block_saved_x_mid(saved.data_ptr(), B, N, D, H, hidden), y.data_ptr()
-        ctx.metas, ctx.params, ctx.dims, ctx.scales = metas, params, (B, N, D, H, hidden), scales
+        ctx.metas, ctx.params, ctx.dims, ctx.scales, ctx.drops = metas, params, (B, N, D, H, hidden), scales, drops
         ctx.save_for_backward(*xs, *saveds)
         return out
 
@@ -252,16 +310,22 @@ class BlockFunction(torch.autograd.Function):
                                                     s_attn, s_mlp, ctypes.byref(prm), ctypes.byref(grd),
                                                     saveds[i].data_ptr(), ws.data_ptr(), L.current_stream()),
                         "mmae_block_f32_backward")
-            else:
+            elif _block_dropout_arg(ctx.drops, i, i > 0) is None:
                 L.check(lib.mmae_block_backward(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
                                                 below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev, ctypes.byref(prm),
                                                 ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
                                                 L.current_stream()), "mmae_block_backward")
+            else:
+                L.check(lib.mmae_block_backward_drop(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(),
+                                                     L.ptr(g_out), below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev,
+                                                     ctypes.byref(_block_dropout_arg(ctx.drops, i, i > 0)),
+                                                     ctypes.byref(prm), ctypes.byref(grd), saveds[i].data_ptr(),
+                                                     ws.data_ptr(), L.current_stream()), "mmae_block_backward_drop")
             if metas[i].get("on_grads_ready") is not None:
                 metas[i]["on_grads_ready"](names)       # fc2.bias of block i is complete: its column sums came from block i+1
             grads[i * P:(i + 1) * P] = _ret_grads(arena, names, blk)
             d, g_in = dx, g_out
-        return (d, None, None) + tuple(grads)
+        return (d, None, None, None) + tuple(grads)
 
 
 def _stack_scale_ptrs(scales, i):
@@ -275,22 +339,24 @@ def _stack_scale_ptrs(scales, i):
 def block_stack(blocks, x, fp32=False):
     """Run an nn.Sequential of multimae_utils.Block as one BlockFunction with hand-offs when it applies (CUDA path, >= 2
     blocks of one shape bound to an arena, BLOCK_CHAIN on), else block by block (`fp32`: in the fp32 tier, always block by
-    block).  The stochastic-depth factors of all blocks are drawn once, up front (drop_path_scales)."""
+    block).  The stochastic-depth factors and the dropout seeds of all blocks are drawn once, up front (drop_path_scales,
+    block_dropouts)."""
     blocks = list(blocks)
     scales = drop_path_scales(blocks, x.shape[0], x.device)
+    drops = block_dropouts(blocks, x.device, fp32)
     metas = [getattr(b, "_meta", None) for b in blocks]
     ok = (BLOCK_CHAIN and not fp32 and len(blocks) >= 2
           and all(m is not None and m["arena"].flat.device == x.device for m in metas)
           and not any(getattr(b, "_own_arena", False) for b in blocks)
           and len({(b.dim, b.num_heads, b.hidden, b.norm1.eps) for b in blocks}) == 1)
     if not ok:
-        for b, sc in zip(blocks, scales):
-            x = b.run(x, fp32=fp32, scales=sc)
+        for b, sc, dr in zip(blocks, scales, drops):
+            x = b.run(x, fp32=fp32, scales=sc, drops=dr)
         return x
     flat = []
     for b in blocks:
         flat += list(b._params())
-    return BlockFunction.apply(x, metas, scales, *flat)
+    return BlockFunction.apply(x, metas, scales, drops, *flat)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -59,7 +59,7 @@ class Mlp(nn.Module):
         super().__init__()
         out_features = out_features or in_features
         hidden_features = hidden_features or in_features
-        assert act_layer is nn.GELU and drop == 0.0, "multimae_b200: exact-erf GELU and drop=0 only"
+        assert act_layer is nn.GELU, "multimae_b200: exact-erf GELU only"
         self.fc1 = nn.Linear(in_features, hidden_features)
         self.act = act_layer()
         self.fc2 = nn.Linear(hidden_features, out_features)
@@ -69,7 +69,7 @@ class Mlp(nn.Module):
 class Attention(nn.Module):
     def __init__(self, dim, num_heads=8, qkv_bias=False, attn_drop=0.0, proj_drop=0.0):
         super().__init__()
-        assert qkv_bias and attn_drop == 0.0 and proj_drop == 0.0, "multimae_b200: qkv_bias=True, no dropout"
+        assert qkv_bias, "multimae_b200: qkv_bias=True only"
         self.num_heads = num_heads
         self.scale = (dim // num_heads) ** -0.5
         self.qkv = nn.Linear(dim, dim * 3, bias=qkv_bias)
@@ -125,11 +125,14 @@ class Block(nn.Module):
 
     def forward(self, x, fp32=False):
         """`fp32`: run this block in the fp32 tier (a decoder block of an adapter listed in fp32_output_adapters).  In
-        training mode with drop_path > 0 each call draws the per-sample factors of both residual branches."""
-        return self.run(x, fp32=fp32, scales=Fn.drop_path_scales([self], x.shape[0], x.device)[0])
+        training mode with drop_path > 0 each call draws the per-sample factors of both residual branches, and with a
+        dropout rate > 0 the seed of its dropout masks."""
+        return self.run(x, fp32=fp32, scales=Fn.drop_path_scales([self], x.shape[0], x.device)[0],
+                        drops=Fn.block_dropouts([self], x.device, fp32)[0])
 
-    def run(self, x, fp32=False, scales=None):
-        """One BlockFunction; `scales`: this block's entry of functional.drop_path_scales (None: no stochastic depth)."""
+    def run(self, x, fp32=False, scales=None, drops=None):
+        """One BlockFunction; `scales`: this block's entry of functional.drop_path_scales (None: no stochastic depth);
+        `drops`: its entry of functional.block_dropouts (None: no dropout)."""
         if self._meta is None or self._meta["arena"].flat.device != x.device:
             # stand-alone use (outside MultiMAE): private gradient arena, zeroed on every forward
             self.bind(Fn.GradArena(list(self.named_parameters()), x.device), "")
@@ -137,4 +140,4 @@ class Block(nn.Module):
         if getattr(self, "_own_arena", False) and torch.is_grad_enabled():
             self._meta["arena"].zero_()
         meta = dict(self._meta, fp32=True) if fp32 else self._meta
-        return Fn.BlockFunction.apply(x, [meta], [scales], *self._params())
+        return Fn.BlockFunction.apply(x, [meta], [scales], [drops], *self._params())
