@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 10
+#define MMAE_ABI_VERSION 11
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -252,6 +252,30 @@ int mmae_embed_forward(const mmae_embed_layout* layout, const mmae_embed_inputs*
 int mmae_embed_backward(const mmae_embed_layout* layout, const mmae_embed_inputs* in, const mmae_embed_params* prm,
                         const mmae_embed_grads* grads, const int64_t* ids_keep, int B, int T, int G, int D,
                         const float* dx, const void* saved, void* ws, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Trainable positional tables of the input adapters (learnable_pos_emb=True, or sincos_pos_emb=False:
+ * multimae/input_adapters.py:76-82, 183-189).  Each forward resizes the parameter pos_emb [1, D, h, w] to the patch grid
+ * (nh, nw) of the call, F.interpolate(pos_emb, (nh, nw), mode, align_corners=False) (:113 bicubic with A = -0.75 and taps
+ * clamped at the border, :235 bilinear), and hands the rows [nh*nw, D] to mmae_embed_forward as prm->pos[t].  When
+ * (nh, nw) == (h, w) the resize is the identity and the rows are the transposed table.  Every result here is computed in
+ * gather form, without atomics: bitwise repeatable.
+ * ---------------------------------------------------------------------------------------------- */
+#define MMAE_POS_BICUBIC 0  /* PatchedInputAdapter */
+#define MMAE_POS_BILINEAR 1 /* SemSegInputAdapter */
+/* rows[p, d] = resized table at grid position (p / nw, p % nw), channel d; table: [D, h, w] fp32 read in place */
+int mmae_pos_resample_forward(const float* table, int D, int h, int w, int nh, int nw, int mode, float* rows, void* stream);
+/* adjoint: dtable[d, y, x] += sum over the rows p that read (y, x) of their interpolation weight times drows[p, d] */
+int mmae_pos_resample_backward(const float* drows, int D, int h, int w, int nh, int nw, int mode, float* dtable,
+                               void* stream);
+/* Gradient of the rows prm->pos[t] of mmae_embed_forward, for the tasks whose table is trainable.  drows_host: host array
+ * of layout->num_tasks device pointers, NULL for a task whose table is frozen; drows_host[t] [N_t, D] is WRITTEN:
+ *   drows_t[p, :] = sum over b of dx[b, slot, :] where slot = ids_restore[b, tok_offset[t] + p] < T
+ * (a patch that is masked in sample b contributes nothing from b; one masked in every sample gets 0).  ids_restore:
+ * [B, tok_offset[num_tasks]] (multimae/multimae.py:205; the identity permutation when nothing is masked); dx: the
+ * [B, T+G, D] gradient given to mmae_embed_backward.  D must be a multiple of 4. */
+int mmae_embed_pos_backward(const mmae_embed_layout* layout, const int64_t* ids_restore, int B, int T, int G, int D,
+                            const float* dx, float* const* drows_host, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Pre-LN transformer block (Block / Attention / Mlp, multimae/multimae_utils.py:138-182, 217-232); used by the

@@ -37,6 +37,7 @@ class GemmEpilogue(ctypes.Structure):
 
 MAX_TASKS = 8
 c_float_p = c_void_p  # device pointers travel as integers
+POS_MODES = {"bicubic": 0, "bilinear": 1}     # MMAE_POS_BICUBIC / MMAE_POS_BILINEAR
 
 
 class EmbedLayout(ctypes.Structure):
@@ -169,6 +170,10 @@ SIGNATURES = {
     "mmae_embed_backward": (c_int, [ctypes.POINTER(EmbedLayout), ctypes.POINTER(EmbedInputs),
                                     ctypes.POINTER(EmbedParams), ctypes.POINTER(EmbedGrads), c_void_p, c_int, c_int,
                                     c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_pos_resample_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "mmae_pos_resample_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "mmae_embed_pos_backward": (c_int, [ctypes.POINTER(EmbedLayout), c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                        ctypes.POINTER(c_void_p), c_void_p]),
     "mmae_block_saved_bytes": (c_i64, [c_int] * 5),
     "mmae_block_workspace_bytes": (c_i64, [c_int] * 5),
     "mmae_block_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
@@ -278,7 +283,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 def lib():

@@ -365,7 +365,11 @@ def block_stack(blocks, x, fp32=False):
 class EmbedFunction(torch.autograd.Function):
     """input adapters + token selection + global-token append (multimae/multimae.py:312-347) as one GEMM + 2 kernels.
 
-    args: meta (dict), ids_keep, then per task [data, weight, bias, class_emb-or-None], then global_tokens."""
+    args: meta (dict), ids_keep, then per task [data, weight, bias, class_emb-or-None], then global_tokens, then - only when
+    some position table is trainable - one pos_emb parameter (or None: frozen, its rows come in meta["pos"]) per task.
+    A trainable table is resized on the device in forward (mmae_pos_resample_forward, reading the parameter in place); in
+    backward its rows' gradient (mmae_embed_pos_backward, through meta["ids_restore"]) goes through the adjoint resize into
+    the table's arena slot (mmae_pos_resample_backward).  meta then also carries pos_names and pos_modes, one per task."""
 
     @staticmethod
     def forward(ctx, meta, ids_keep, *tensors):
@@ -374,11 +378,21 @@ class EmbedFunction(torch.autograd.Function):
         T_tasks = layout.num_tasks
         per_task = [tensors[4 * t:4 * t + 4] for t in range(T_tasks)]
         global_tokens = tensors[4 * T_tasks]
+        tables = tensors[4 * T_tasks + 1:] or (None,) * T_tasks
         B, T = ids_keep.shape
         G, D = global_tokens.shape[-2], global_tokens.shape[-1]
         _require_cuda(ids_keep, "embed")
         ins, prm = L.EmbedInputs(), L.EmbedParams()
         keep_alive = []
+        pos = list(meta["pos"])
+        for t, table in enumerate(tables):
+            if table is not None:          # trainable: this call's rows, resized from the parameter as it is now
+                _require_cuda(table, "embed")
+                nh, nw = layout.grid_h[t], layout.grid_w[t]
+                pos[t] = torch.empty((nh * nw, D), dtype=torch.float32, device=ids_keep.device)
+                L.check(lib.mmae_pos_resample_forward(table.data_ptr(), D, table.shape[2], table.shape[3], nh, nw,
+                                                      meta["pos_modes"][t], pos[t].data_ptr(), L.current_stream()),
+                        "mmae_pos_resample_forward")
         for t, (data, w, b, cemb) in enumerate(per_task):
             _require_cuda(data, "embed")
             data = data.contiguous()
@@ -391,7 +405,7 @@ class EmbedFunction(torch.autograd.Function):
             ins.class_emb[t] = cemb.data_ptr() if cemb is not None else None
             prm.weight[t] = w.data_ptr()
             prm.bias[t] = b.data_ptr()
-            prm.pos[t] = meta["pos"][t].data_ptr()
+            prm.pos[t] = pos[t].data_ptr()
         prm.global_tokens = global_tokens.data_ptr()
         dev = ids_keep.device
         saved = torch.empty(lib.mmae_embed_saved_bytes(ctypes.byref(layout), B, T, D), dtype=torch.uint8, device=dev)
@@ -404,6 +418,7 @@ class EmbedFunction(torch.autograd.Function):
         ctx.meta = meta
         ctx.tensors = tensors
         ctx.keep_alive = keep_alive
+        ctx.pos = pos
         ctx.dims = (B, T, G, D)
         ctx.save_for_backward(ids_keep, saved)
         return out
@@ -424,7 +439,7 @@ class EmbedFunction(torch.autograd.Function):
             ins.class_emb[t] = cemb.data_ptr() if cemb is not None else None
             prm.weight[t] = w.data_ptr()
             prm.bias[t] = b.data_ptr()
-            prm.pos[t] = meta["pos"][t].data_ptr()
+            prm.pos[t] = ctx.pos[t].data_ptr()
             wn, bn, cn = names[t]
             grd.weight[t] = _grad_ptr(arena, wn)
             grd.bias[t] = _grad_ptr(arena, bn)
@@ -441,12 +456,34 @@ class EmbedFunction(torch.autograd.Function):
         L.check(lib.mmae_embed_backward(ctypes.byref(layout), ctypes.byref(ins), ctypes.byref(prm), ctypes.byref(grd),
                                         ids_keep.data_ptr(), B, T, G, D, dx.data_ptr(), saved.data_ptr(), ws.data_ptr(),
                                         L.current_stream()), "mmae_embed_backward")
+        tables = tensors[4 * T_tasks + 1:]
+        if tables:
+            _pos_backward(meta, tables, ctx.pos, dx, B, T, G, D)
+            flat_names += meta["pos_names"]
+            flat_params += list(tables)
         real = [(n, p) for n, p in zip(flat_names, flat_params) if n is not None]
         if meta.get("on_grads_ready") is not None:
             meta["on_grads_ready"]([n for n, _ in real])
         rets = iter(_ret_grads(arena, [n for n, _ in real], [p for _, p in real]))
         out = [None if n is None else next(rets) for n in flat_names]
         return (None, None) + tuple(out)
+
+
+def _pos_backward(meta, tables, rows, dx, B, T, G, D):
+    """Gradient of the trainable position tables of one EmbedFunction call, accumulated into their arena slots: the rows'
+    gradient of every trainable task in one pass over dx, then one adjoint resize per table."""
+    lib = L.lib()
+    layout, arena, ids_restore = meta["layout"], meta["arena"], meta["ids_restore"]
+    drows = [None if tb is None else torch.empty_like(r) for tb, r in zip(tables, rows)]
+    arr = (ctypes.c_void_p * layout.num_tasks)(*[L.ptr(g) for g in drows])
+    L.check(lib.mmae_embed_pos_backward(ctypes.byref(layout), ids_restore.data_ptr(), B, T, G, D, dx.data_ptr(), arr,
+                                        L.current_stream()), "mmae_embed_pos_backward")
+    for t, (tb, g) in enumerate(zip(tables, drows)):
+        if tb is not None:
+            L.check(lib.mmae_pos_resample_backward(g.data_ptr(), D, tb.shape[2], tb.shape[3], layout.grid_h[t],
+                                                   layout.grid_w[t], meta["pos_modes"][t],
+                                                   _grad_ptr(arena, meta["pos_names"][t]), L.current_stream()),
+                    "mmae_pos_resample_backward")
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -14,7 +14,10 @@ from .multimae_utils import build_2d_sincos_posemb, pair, trunc_normal_
 
 class _PosEmbCache:
     """Resized positional table rows [nh*nw, D] for the frozen sin-cos parameter (reference re-runs F.interpolate every
-    forward: multimae/input_adapters.py:113,235; the table is constant, so it is computed once per size/device)."""
+    forward: multimae/input_adapters.py:113,235; the table is constant, so it is computed once per size/device).
+
+    A trainable table of an input adapter never comes here: the embedding resizes it on the device every call and returns
+    its gradient (functional.EmbedFunction).  The output adapters have no such path and refuse one."""
 
     def _resized_pos(self, nh, nw, mode):
         if self.pos_emb.requires_grad:

@@ -63,18 +63,30 @@ def _build_layout(adapters, x):
     return layout
 
 
-def _embed(adapters, x, ids_keep, global_tokens, arena, prefix_of, on_grads_ready=None):
-    """Gather-first embedding of the tokens listed in ids_keep (+ global tokens appended last)."""
+def _embed(adapters, x, ids_keep, ids_restore, global_tokens, arena, prefix_of, on_grads_ready=None):
+    """Gather-first embedding of the tokens listed in ids_keep (+ global tokens appended last).  A frozen position table
+    enters as its cached resized rows; a trainable one (learnable_pos_emb=True / sincos_pos_emb=False) as an autograd input
+    of EmbedFunction, resized on the device every call (ids_restore then locates each patch's token for its gradient)."""
     layout = _build_layout(adapters, x)
-    names, tensors, pos = [], [], []
+    names, tensors, pos, tables, pos_names = [], [], [], [], []
     for t, (name, ad) in enumerate(adapters):
         pre = prefix_of(name)
         cemb = ad.class_emb.weight if ad.is_semseg else None
         names.append((pre + "proj.weight", pre + "proj.bias", pre + "class_emb.weight" if ad.is_semseg else None))
         tensors += [x[name], ad.proj.weight, ad.proj.bias, cemb]
-        pos.append(ad._resized_pos(layout.grid_h[t], layout.grid_w[t], ad.pos_mode))
+        if ad.pos_emb.requires_grad:
+            pos.append(None)
+            tables.append(ad.pos_emb)
+            pos_names.append(pre + "pos_emb")
+        else:
+            pos.append(ad._resized_pos(layout.grid_h[t], layout.grid_w[t], ad.pos_mode))
+            tables.append(None)
+            pos_names.append(None)
     meta = dict(layout=layout, arena=arena, names=names, pos=pos, on_grads_ready=on_grads_ready)
-    return Fn.EmbedFunction.apply(meta, ids_keep, *tensors, global_tokens)
+    if not any(n is not None for n in pos_names):
+        return Fn.EmbedFunction.apply(meta, ids_keep, *tensors, global_tokens)
+    meta.update(ids_restore=ids_restore.contiguous(), pos_names=pos_names, pos_modes=[L.POS_MODES[ad.pos_mode] for _, ad in adapters])
+    return Fn.EmbedFunction.apply(meta, ids_keep, *tensors, global_tokens, *tables)
 
 
 def embed_all_patches(adapter, x):
@@ -86,7 +98,7 @@ def embed_all_patches(adapter, x):
     named = [(n, p) for n, p in adapter.named_parameters() if p.requires_grad]
     dummy = torch.zeros(1, 0, adapter.dim_tokens, device=x.device, requires_grad=False)
     arena = Fn.GradArena(named + [("global_tokens", dummy)], x.device)
-    return _embed([("x", adapter)], {"x": x}, ids, dummy, arena, lambda name: "")
+    return _embed([("x", adapter)], {"x": x}, ids, ids, dummy, arena, lambda name: "")   # every patch kept, in order
 
 
 class MultiMAE(nn.Module):
@@ -335,7 +347,7 @@ class MultiMAE(nn.Module):
             if AUTO_OWN_GRADIENTS and not arena.owned:
                 self.own_gradients(True)
             arena.begin_step()
-        seq = _embed(adapters, x, ids_keep, self.global_tokens, arena, lambda d: "input_adapters.%s." % d,
+        seq = _embed(adapters, x, ids_keep, ids_restore, self.global_tokens, arena, lambda d: "input_adapters.%s." % d,
                      self._grad_callback)
         encoder_tokens = Fn.block_stack(self.encoder, seq)
         if self.output_adapters is None:
@@ -444,7 +456,8 @@ class MultiViT(MultiMAE):
             if AUTO_OWN_GRADIENTS and not arena.owned:
                 self.own_gradients(True)
             arena.begin_step()
-        seq = _embed(adapters, x, ids, self.global_tokens, arena, lambda d: "input_adapters.%s." % d, self._grad_callback)
+        seq = _embed(adapters, x, ids, ids, self.global_tokens, arena, lambda d: "input_adapters.%s." % d,
+                     self._grad_callback)                      # nothing masked: ids_restore is the identity, like ids
         return seq, input_info
 
     def forward(self, x, return_all_layers=False, **kwargs):
