@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 11
+#define MMAE_ABI_VERSION 12
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -482,6 +482,46 @@ int mmae_convnext_tail_forward(const float* x, int B, int nh, int nw, int s, int
                                const float* b, float* out, void* saved, void* ws, void* stream);
 int mmae_convnext_tail_backward(const float* dout, int B, int nh, int nw, int s, int C, int K, int H, int W, const float* w,
                                 float* d_w, float* d_b, float* dx, const void* saved, void* ws, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Segmenter head of semantic-segmentation fine-tuning: SegmenterMaskTransformerAdapter (multimae/output_adapters.py:359-478):
+ * proj -> transformer blocks (mmae_block_*) over n + K tokens -> tail.  n = nh*nw patch tokens are followed by one token per
+ * class.  E (the decoder width) must be a multiple of 128, at most 1024; 8 <= K <= 256.  GEMMs take bf16 operands and
+ * accumulate in fp32.  Backward WRITES the activation gradient and ACCUMULATES (+=) the parameter gradients; the activation
+ * gradient, d_cls and the mask_norm gradients are computed without atomics (bitwise repeatable).
+ * ---------------------------------------------------------------------------------------------- */
+/* proj: seq[b, :n] = cat_t(enc[b, start_t : start_t + n]) W^T + bias, seq[b, n:] = cls_emb  (seq [B, n + K, E] fp32,
+ * W [E, D*num_tasks], cls_emb [K, E]).  Backward writes denc [B, N, D] in full and adds sum_b dseq[b, n + k] to d_cls[k]. */
+int64_t mmae_segmenter_proj_saved_bytes(int B, int n, int D_in, int E);
+int64_t mmae_segmenter_proj_workspace_bytes(int B, int n, int D_in, int E);
+int mmae_segmenter_proj_forward(const float* enc, int B, int N, int D, int n, int num_tasks, const int* start_host, int E, int K,
+                                const float* w, const float* b, const float* cls_emb, float* seq, void* saved, void* ws,
+                                void* stream);
+int mmae_segmenter_proj_backward(const float* dseq, int B, int N, int D, int n, int num_tasks, const int* start_host, int E,
+                                 int K, const float* w, float* d_w, float* d_b, float* d_cls, float* denc, const void* saved,
+                                 void* ws, void* stream);
+/* The fused cosine mask + class LayerNorm on its own.  P [B*n, E], C [B*K, E] bf16; rp [B*n], rc [B*K] = 1 / max(norm, 1e-12) of
+ * their rows.  forward: cmap[b*n + i, j] = LN_j(P_b[i] . C_b[j] rp rc) gamma_j + beta_j, fp32 [B*n, Kp], Kp = round_up(K, 8),
+ * pad columns zero; mean / rstd [B*n] are saved for backward.  backward: dcmap [B*n, Kp] -> dP, dC (bf16, gradients of the
+ * UNnormalised rows: the normalise backward is included), d_gamma / d_beta += . */
+int64_t mmae_segmenter_mask_workspace_bytes(int B, int n, int K);
+int mmae_segmenter_mask_forward(const void* P, const void* C, const float* rp, const float* rc, const float* gamma,
+                                const float* beta, float eps, int B, int n, int K, int E, float* cmap, float* mean, float* rstd,
+                                void* stream);
+int mmae_segmenter_mask_backward(const void* P, const void* C, const float* rp, const float* rc, const float* gamma,
+                                 const float* mean, const float* rstd, const float* dcmap, int B, int n, int K, int E, void* dP,
+                                 void* dC, float* d_gamma, float* d_beta, void* ws, void* stream);
+/* tail: out [B, K, H, W] fp32 = bilinear(mask_norm(normalize(patch_proj(y[:, :n])) normalize(classes_proj(y[:, n:]))^T)),
+ * y = decoder_norm(x), x [B, n + K, E] fp32; H, W integer multiples of nh, nw.  params_host / grads_host: host arrays of 6
+ * device pointers: decoder_norm.weight, decoder_norm.bias [E], patch_proj.weight, classes_proj.weight [E, E],
+ * mask_norm.weight, mask_norm.bias [K]. */
+int64_t mmae_segmenter_tail_saved_bytes(int B, int nh, int nw, int E, int K);
+int64_t mmae_segmenter_tail_workspace_bytes(int B, int nh, int nw, int E, int K);
+int mmae_segmenter_tail_forward(const float* x, int B, int nh, int nw, int E, int K, int H, int W, float eps_dec, float eps_mask,
+                                const float* const* params_host, float* out, void* saved, void* ws, void* stream);
+int mmae_segmenter_tail_backward(const float* x, const float* dout, float* dx, int B, int nh, int nw, int E, int K, int H, int W,
+                                 const float* const* params_host, float* const* grads_host, const void* saved, void* ws,
+                                 void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * fp32 tier for `fp32_output_adapters` (multimae/multimae.py:367-377: the listed output adapters run outside autocast;

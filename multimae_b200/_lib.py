@@ -249,6 +249,22 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "mmae_convnext_tail_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_segmenter_proj_saved_bytes": (c_i64, [c_int] * 4),
+    "mmae_segmenter_proj_workspace_bytes": (c_i64, [c_int] * 4),
+    "mmae_segmenter_proj_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, c_int,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_segmenter_proj_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), c_int, c_int,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_segmenter_mask_workspace_bytes": (c_i64, [c_int] * 3),
+    "mmae_segmenter_mask_forward": (c_int, [c_void_p] * 6 + [c_float, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                                             c_void_p]),
+    "mmae_segmenter_mask_backward": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int] + [c_void_p] * 6),
+    "mmae_segmenter_tail_saved_bytes": (c_i64, [c_int] * 5),
+    "mmae_segmenter_tail_workspace_bytes": (c_i64, [c_int] * 5),
+    "mmae_segmenter_tail_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float,
+                                            ctypes.POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "mmae_segmenter_tail_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                             ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_void_p, c_void_p, c_void_p]),
     # ---- fp32 tier (fp32_output_adapters)
     "mmae_linear_f32_workspace_bytes": (c_i64, [c_int] * 3),
     "mmae_linear_f32_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -283,7 +299,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 
 def lib():

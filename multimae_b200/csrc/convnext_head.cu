@@ -562,8 +562,8 @@ extern "C" int64_t mmae_convnext_tail_workspace_bytes(int B, int nh, int nw, int
   return (int64_t)tl_ws(nullptr, int64_t(B) * nh * nw * s * s, C, K).bytes;
 }
 
-namespace {
-int check_up(const char* what, int nh, int nw, int s, int K, int H, int W) {
+namespace mmae {
+int upsample_check(const char* what, int nh, int nw, int s, int K, int H, int W) {
   const int Hf = nh * s, Wf = nw * s;
   MMAE_CHECK(K > 0 && H > 0 && W > 0 && H % Hf == 0 && W % Wf == 0, MMAE_ERR_UNSUPPORTED,
              "%s: the upsample needs K > 0 and integer ratios, got (%d, %d) -> (%d, %d)", what, Hf, Wf, H, W);
@@ -571,15 +571,29 @@ int check_up(const char* what, int nh, int nw, int s, int K, int H, int W) {
              "%s: rows of %d / %d pixels are too wide for the upsample kernels", what, Wf, W);
   return MMAE_OK;
 }
-}  // namespace
+
+int launch_upsample_fwd(const float* cmap, int Kp, int K, int B, int nh, int nw, int s, int H, int W, float* out, void* stream) {
+  const Geo g{nh, nw, s, 0};
+  const int Wf = nw * s, KC = std::min(K, UP_SMEM_FLOATS / (2 * Wf) - 1);
+  return launch(upsample_fwd_kernel, dim3(H, B, ceil_div(K, KC)), dim3(UP_THREADS), size_t(2) * Wf * (KC + 1) * sizeof(float),
+                stream, cmap, Kp, K, KC, g, H, W, out);
+}
+
+int launch_upsample_bwd(const float* dout, int Kp, int K, int B, int nh, int nw, int s, int H, int W, float* dcmap,
+                        void* stream) {
+  const Geo g{nh, nw, s, 0};
+  const int KC = std::min(Kp, UP_SMEM_FLOATS / (W + 1));
+  return launch(upsample_bwd_kernel, dim3(nh * s, B, ceil_div(Kp, KC)), dim3(UP_THREADS), size_t(KC) * (W + 1) * sizeof(float),
+                stream, dout, Kp, K, KC, g, H, W, dcmap);
+}
+}  // namespace mmae
 
 extern "C" int mmae_convnext_tail_forward(const float* x, int B, int nh, int nw, int s, int C, int K, int H, int W,
                                           const float* w, const float* bias, float* out, void* saved, void* ws, void* stream) {
   RUN(check_geo("mmae_convnext_tail_forward", B, nh, nw, s, C));
-  RUN(check_up("mmae_convnext_tail_forward", nh, nw, s, K, H, W));
+  RUN(upsample_check("mmae_convnext_tail_forward", nh, nw, s, K, H, W));
   MMAE_CHECK(x && w && bias && out && saved && ws && aligned16(x), MMAE_ERR_ARG, "mmae_convnext_tail_forward: bad args");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const Geo g{nh, nw, s, C};
   const int P = B * nh * nw * s * s, Kp = round8(K);
   TailSaved sv = tl_saved(saved, P, C, K);
   TailWs wk = tl_ws(ws, P, C, K);
@@ -595,27 +609,22 @@ extern "C" int mmae_convnext_tail_forward(const float* x, int B, int nh, int nw,
   MMAE_CUDA_OK(cudaMemcpyAsync(wk.bias_p, bias, K * sizeof(float), cudaMemcpyDeviceToDevice, st));
   RUN(linear_f32(sv.x_b, sv.w_b, wk.bias_p, nullptr, wk.cmap, P, Kp, C, stream));
   // F.interpolate(size=(H, W), mode="bilinear") (:573)
-  const int Wf = nw * s, KC = std::min(K, UP_SMEM_FLOATS / (2 * Wf) - 1);
-  return launch(upsample_fwd_kernel, dim3(H, B, ceil_div(K, KC)), dim3(UP_THREADS), size_t(2) * Wf * (KC + 1) * sizeof(float),
-                stream, (const float*)wk.cmap, Kp, K, KC, g, H, W, out);
+  return launch_upsample_fwd(wk.cmap, Kp, K, B, nh, nw, s, H, W, out, stream);
 }
 
 extern "C" int mmae_convnext_tail_backward(const float* dout, int B, int nh, int nw, int s, int C, int K, int H, int W,
                                            const float* w, float* d_w, float* d_b, float* dx, const void* saved, void* ws,
                                            void* stream) {
   RUN(check_geo("mmae_convnext_tail_backward", B, nh, nw, s, C));
-  RUN(check_up("mmae_convnext_tail_backward", nh, nw, s, K, H, W));
+  RUN(upsample_check("mmae_convnext_tail_backward", nh, nw, s, K, H, W));
   MMAE_CHECK(dout && w && d_w && d_b && dx && saved && ws && aligned16(dx), MMAE_ERR_ARG,
              "mmae_convnext_tail_backward: bad args");
   (void)w;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const Geo g{nh, nw, s, C};
   const int P = B * nh * nw * s * s, Kp = round8(K);
   TailSaved sv = tl_saved(const_cast<void*>(saved), P, C, K);
   TailWs wk = tl_ws(ws, P, C, K);
-  const int KC = std::min(Kp, UP_SMEM_FLOATS / (W + 1));
-  RUN(launch(upsample_bwd_kernel, dim3(nh * s, B, ceil_div(Kp, KC)), dim3(UP_THREADS), size_t(KC) * (W + 1) * sizeof(float),
-             stream, dout, Kp, K, KC, g, H, W, wk.cmap));
+  RUN(launch_upsample_bwd(dout, Kp, K, B, nh, nw, s, H, W, wk.cmap, stream));
   const bool pad = Kp != K;
   if (pad) {
     MMAE_CUDA_OK(cudaMemsetAsync(wk.db_p, 0, Kp * sizeof(float), st));

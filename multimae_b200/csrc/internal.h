@@ -80,6 +80,13 @@ int add_scaled_f32(const float* x, const void* y, int y_is_bf16, const float* ro
 // cls_head.cu: dst[i] += src[i] over n contiguous fp32 elements (any n)
 int add_f32(float* dst, const float* src, int64_t n, cudaStream_t st);
 
+// convnext_head.cu: the bilinear upsample of a [B*nh*nw*s*s, Kp] class map (pixel order of the ConvNeXt head; plain row-major
+// patches at s = 1) to [B, K, H, W], align_corners=False, and its gather-form backward (pad columns K..Kp-1 written as zeros)
+int upsample_check(const char* what, int nh, int nw, int s, int K, int H, int W);
+int launch_upsample_fwd(const float* cmap, int Kp, int K, int B, int nh, int nw, int s, int H, int W, float* out, void* stream);
+int launch_upsample_bwd(const float* dout, int Kp, int K, int B, int nh, int nw, int s, int H, int W, float* dcmap,
+                        void* stream);
+
 // GEMM helpers of the module-level entry points (modules.cu): bf16 operands, fp32 accumulation through mmae_gemm_bf16.
 // bf16 operand of a weight: the registered mirror of the fp32 parameter buffer, else the per-call slot *slot (cast now when
 // cast_now; in backward the forward already cast it there)

@@ -933,6 +933,97 @@ class ConvNeXtTailFunction(torch.autograd.Function):
         return (dx, None) + tuple(_report(meta, names, [weight, bias]))
 
 
+SEGMENTER_TAIL_PARAM_NAMES = ["decoder_norm.weight", "decoder_norm.bias", "patch_proj.weight", "classes_proj.weight",
+                              "mask_norm.weight", "mask_norm.bias"]
+
+
+class SegmenterProjFunction(torch.autograd.Function):
+    """Token gather + proj_dec + class tokens of SegmenterMaskTransformerAdapter.forward (multimae/output_adapters.py:
+    454-458): encoder tokens [B, N, D] -> the fp32 sequence [B, n + K, E], patch tokens first (mmae_segmenter_proj_*).
+
+    args: enc, meta, proj_dec.weight, proj_dec.bias, cls_emb.  meta: arena, prefix, on_grads_ready, save, n (tokens per
+    task), starts (first token of each main task)."""
+
+    @staticmethod
+    def forward(ctx, enc, meta, weight, bias, cls_emb):
+        _require_cuda(enc, "SegmenterMaskTransformerAdapter")
+        lib = L.lib()
+        enc = enc.contiguous().float()
+        B, N, D = enc.shape
+        n, starts, E, K = meta["n"], list(meta["starts"]), weight.shape[0], cls_emb.shape[1]
+        arr = (ctypes.c_int * len(starts))(*starts)
+        saved, saved_ptr, ws_ptr = _saved_and_ws(meta, lib.mmae_segmenter_proj_saved_bytes(B, n, D * len(starts), E),
+                                                 lib.mmae_segmenter_proj_workspace_bytes(B, n, D * len(starts), E), enc.device)
+        out = torch.empty((B, n + K, E), dtype=torch.float32, device=enc.device)
+        L.check(lib.mmae_segmenter_proj_forward(enc.data_ptr(), B, N, D, n, len(starts), arr, E, K, weight.data_ptr(),
+                                                bias.data_ptr(), cls_emb.data_ptr(), out.data_ptr(), saved_ptr, ws_ptr,
+                                                L.current_stream()), "mmae_segmenter_proj_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, (B, N, D), (weight, bias, cls_emb)
+            ctx.save_for_backward(saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        (saved,) = ctx.saved_tensors
+        meta, (weight, bias, cls_emb) = ctx.meta, ctx.params
+        B, N, D = ctx.dims
+        n, starts, E, K = meta["n"], list(meta["starts"]), weight.shape[0], cls_emb.shape[1]
+        arr = (ctypes.c_int * len(starts))(*starts)
+        names = [meta["prefix"] + k for k in ("proj_dec.weight", "proj_dec.bias", "cls_emb")]
+        ws = Workspace.get(lib.mmae_segmenter_proj_workspace_bytes(B, n, D * len(starts), E), dout.device)
+        dout = dout.contiguous().float()
+        denc = torch.empty((B, N, D), dtype=torch.float32, device=dout.device)
+        L.check(lib.mmae_segmenter_proj_backward(dout.data_ptr(), B, N, D, n, len(starts), arr, E, K, weight.data_ptr(),
+                                                 *[_grad_ptr(meta["arena"], k) for k in names], denc.data_ptr(),
+                                                 saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_segmenter_proj_backward")
+        return (denc, None) + tuple(_report(meta, names, [weight, bias, cls_emb]))
+
+
+class SegmenterTailFunction(torch.autograd.Function):
+    """Everything after the blocks of SegmenterMaskTransformerAdapter.forward (multimae/output_adapters.py:463-476):
+    decoder_norm, patch_proj / classes_proj, the fused cosine mask + class LayerNorm, bilinear upsample: [B, n + K, E] ->
+    [B, K, H, W] fp32 (mmae_segmenter_tail_*).  args: x, meta (plus B, nh, nw, num_classes, H, W, eps_dec, eps_mask), then
+    the 6 SEGMENTER_TAIL_PARAM_NAMES tensors - the order of the entry points' pointer arrays."""
+
+    @staticmethod
+    def forward(ctx, x, meta, *params):
+        _require_cuda(x, "SegmenterMaskTransformerAdapter")
+        lib = L.lib()
+        x = x.contiguous().float()
+        K, H, W = meta["num_classes"], meta["H"], meta["W"]
+        dims = (meta["B"], meta["nh"], meta["nw"], x.shape[2], K)
+        saved, saved_ptr, ws_ptr = _saved_and_ws(meta, lib.mmae_segmenter_tail_saved_bytes(*dims),
+                                                 lib.mmae_segmenter_tail_workspace_bytes(*dims), x.device)
+        out = torch.empty((meta["B"], K, H, W), dtype=torch.float32, device=x.device)
+        prm = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
+        L.check(lib.mmae_segmenter_tail_forward(x.data_ptr(), *dims, H, W, float(meta["eps_dec"]), float(meta["eps_mask"]), prm,
+                                                out.data_ptr(), saved_ptr, ws_ptr, L.current_stream()),
+                "mmae_segmenter_tail_forward")
+        if saved is not None:
+            ctx.meta, ctx.dims, ctx.params = meta, dims, params
+            ctx.save_for_backward(x, saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.lib()
+        x, saved = ctx.saved_tensors
+        meta, dims, params = ctx.meta, ctx.dims, ctx.params
+        names = [meta["prefix"] + k for k in SEGMENTER_TAIL_PARAM_NAMES]
+        ws = Workspace.get(lib.mmae_segmenter_tail_workspace_bytes(*dims), dout.device)
+        dout = dout.contiguous().float()
+        dx = torch.empty_like(x)
+        prm = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
+        grd = (ctypes.c_void_p * len(names))(*[_grad_ptr(meta["arena"], k) for k in names])
+        L.check(lib.mmae_segmenter_tail_backward(x.data_ptr(), dout.data_ptr(), dx.data_ptr(), *dims, meta["H"], meta["W"],
+                                                 prm, grd, saved.data_ptr(), ws.data_ptr(), L.current_stream()),
+                "mmae_segmenter_tail_backward")
+        return (dx, None) + tuple(_report(meta, names, params))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # masked losses
 # ---------------------------------------------------------------------------------------------------------------------

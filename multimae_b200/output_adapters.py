@@ -6,8 +6,10 @@
   ConvNeXtAdapter (:481-573)     - the semantic-segmentation head of fine-tuning (run_finetuning_semseg.py), executed as
                                    ConvNeXtProjFunction -> ConvNeXtBlockFunction x depth -> ConvNeXtTailFunction.
 
-SegmenterMaskTransformerAdapter and DPTOutputAdapter exist so that the fine-tuning scripts import; constructing either
-raises NotImplementedError."""
+  SegmenterMaskTransformerAdapter (:359-478) - the Segmenter head of the same script (--output_adapter segmenter),
+                                   executed as SegmenterProjFunction -> Block x depth -> SegmenterTailFunction.
+
+DPTOutputAdapter exists so that the fine-tuning scripts import; constructing it raises NotImplementedError."""
 import math
 from functools import partial
 from typing import Dict, Iterable, Optional, Tuple, Union
@@ -368,12 +370,99 @@ class ConvNeXtAdapter(nn.Module):
 
 
 class SegmenterMaskTransformerAdapter(nn.Module):
-    """Placeholder so that the fine-tuning scripts import: the Segmenter head (multimae/output_adapters.py:359-478) is not
-    implemented on the CUDA path."""
+    """Output adapter inspired by the Segmenter-Mask architecture (https://arxiv.org/abs/2105.05633): proj_dec of the main
+    tasks' tokens, one learned token per class appended, `depth` transformer Blocks over the n + K tokens, decoder_norm, and
+    the class map = LayerNorm over the classes of the cosine between every projected patch token and every projected class
+    token, upsampled bilinearly to the image size.  Extra keyword arguments (stride_level, ...) are ignored, as by the
+    reference.  Runs as SegmenterProjFunction -> functional.block_stack -> SegmenterTailFunction.
 
-    def __init__(self, *args, **kwargs):
-        raise NotImplementedError("multimae_b200: SegmenterMaskTransformerAdapter is not implemented; "
-                                  "use --output_adapter convnext")
+    The kernels need embed_dim to be a multiple of 128, at most 1024, with heads of 32 or 64 channels (768 with 12 heads in
+    the reference's default), and 8 to 256 classes; anything else raises here."""
+
+    def __init__(self, num_classes, depth: int = 2, num_heads: int = 12, embed_dim: int = 768, mlp_ratio=4,
+                 drop_path_rate=0.1, drop_rate=0.0, attn_drop_rate=0.0, qkv_bias=True, main_tasks: Iterable[str] = ('rgb',),
+                 patch_size: int = 16, norm_layer: nn.Module = partial(nn.LayerNorm, eps=1e-6), **kwargs):
+        super().__init__()
+        name = "SegmenterMaskTransformerAdapter"
+        if embed_dim % 128 != 0 or embed_dim > 1024 or embed_dim % num_heads != 0 or embed_dim // num_heads not in (32, 64):
+            raise NotImplementedError(
+                "%s: embed_dim=%d with %d heads; the CUDA head needs embed_dim to be a multiple of 128, at most 1024, and "
+                "heads of 32 or 64 channels (pass --decoder_dim 768 for the default 12 heads)" % (name, embed_dim, num_heads))
+        if not 8 <= num_classes <= 256:
+            raise NotImplementedError("%s: num_classes=%d; the mask kernel holds 8 to 256 classes" % (name, num_classes))
+        self.main_tasks = main_tasks
+        self.patch_size = patch_size
+        self.embed_dim = embed_dim
+        self.num_classes = num_classes
+        self._bound = None
+        self._own_arena = False
+
+        self.cls_emb = nn.Parameter(torch.zeros(1, num_classes, embed_dim))
+        trunc_normal_(self.cls_emb, std=0.02)
+
+        self.patch_proj = nn.Linear(embed_dim, embed_dim, bias=False)
+        self.classes_proj = nn.Linear(embed_dim, embed_dim, bias=False)
+
+        dpr = [x.item() for x in torch.linspace(0, drop_path_rate, depth)]
+        self.blocks = nn.ModuleList([
+            Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias, drop=drop_rate,
+                  attn_drop=attn_drop_rate, drop_path=dpr[i], norm_layer=norm_layer) for i in range(depth)])
+
+        self.decoder_norm = norm_layer(embed_dim)
+        self.mask_norm = norm_layer(num_classes)
+        assert isinstance(self.decoder_norm, nn.LayerNorm), "multimae_b200: norm_layer must build nn.LayerNorm"
+        self.apply(self._init_weights)
+
+    def init(self, dim_tokens_enc: int = 768):
+        """Build proj_dec for encoder tokens of width dim_tokens_enc (called by MultiMAE.__init__)."""
+        self.in_channels = dim_tokens_enc * len(self.main_tasks)
+        self.proj_dec = nn.Linear(self.in_channels, self.embed_dim)
+        self._init_weights(self.proj_dec)
+        self._bound = None
+
+    def _init_weights(self, m):
+        if isinstance(m, nn.Linear):
+            trunc_normal_(m.weight, std=.02)
+            if m.bias is not None:
+                nn.init.constant_(m.bias, 0)
+        elif isinstance(m, nn.LayerNorm):
+            nn.init.constant_(m.bias, 0)
+            nn.init.constant_(m.weight, 1.0)
+
+    def bind(self, arena, prefix, on_grads_ready=None):
+        self._own_arena = False
+        self._bound = dict(arena=arena, prefix=prefix, on_grads_ready=on_grads_ready)
+        for i, blk in enumerate(self.blocks):
+            blk.bind(arena, "%sblocks.%d." % (prefix, i), on_grads_ready)
+
+    def forward(self, encoder_tokens: torch.Tensor, input_info: Dict):
+        assert hasattr(self, "proj_dec"), "Need to call init(dim_tokens_enc) function first"
+        if not torch.is_tensor(encoder_tokens):
+            raise NotImplementedError("multimae_b200: SegmenterMaskTransformerAdapter takes the last layer's tokens "
+                                      "(return_all_layers=False)")
+        H, W = input_info['image_size']
+        nh, nw = H // self.patch_size, W // self.patch_size
+        for task in self.main_tasks:
+            n_t = input_info['tasks'][task]['end_idx'] - input_info['tasks'][task]['start_idx']
+            if n_t != nh * nw:
+                raise ValueError("SegmenterMaskTransformerAdapter: task %r has %d tokens, the %dx%d image has %d x %d = %d "
+                                 "patches of %d" % (task, n_t, H, W, nh, nw, nh * nw, self.patch_size))
+        if self._bound is None or self._bound["arena"].flat.device != encoder_tokens.device:
+            # stand-alone use (outside MultiMAE / MultiViT): private gradient arena, zeroed on every training forward
+            self.bind(Fn.GradArena([(n, p) for n, p in self.named_parameters() if p.requires_grad],
+                                   encoder_tokens.device), "")
+            self._own_arena = True
+        tail = [dict(self.named_parameters())[k] for k in Fn.SEGMENTER_TAIL_PARAM_NAMES]
+        save = torch.is_grad_enabled() and (encoder_tokens.requires_grad or any(p.requires_grad for p in self.parameters()))
+        if self._own_arena and save:
+            self._bound["arena"].zero_()
+        base = dict(self._bound, save=save, B=encoder_tokens.shape[0], nh=nh, nw=nw)
+        starts = [input_info['tasks'][t]['start_idx'] for t in self.main_tasks]
+        x = Fn.SegmenterProjFunction.apply(encoder_tokens, dict(base, n=nh * nw, starts=starts), self.proj_dec.weight,
+                                           self.proj_dec.bias, self.cls_emb)
+        x = Fn.block_stack(self.blocks, x)
+        return Fn.SegmenterTailFunction.apply(x, dict(base, num_classes=self.num_classes, H=H, W=W,
+                                                      eps_dec=self.decoder_norm.eps, eps_mask=self.mask_norm.eps), *tail)
 
 
 class DPTOutputAdapter(nn.Module):
@@ -381,4 +470,5 @@ class DPTOutputAdapter(nn.Module):
     implemented on the CUDA path."""
 
     def __init__(self, *args, **kwargs):
-        raise NotImplementedError("multimae_b200: DPTOutputAdapter is not implemented; use --output_adapter convnext")
+        raise NotImplementedError("multimae_b200: DPTOutputAdapter is not implemented; use --output_adapter convnext or "
+                                  "segmenter")
