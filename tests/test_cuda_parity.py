@@ -501,6 +501,59 @@ def test_losses_against_oracle(dev):
             else:                                             # all-zero mask: constant 0 (criterion.py:42,100,157)
                 assert float(got) == 0.0
 
+    # Label smoothing and ignored (-100) targets (float64 F.cross_entropy: the oracle has no ignore_index), the 448^2 shapes
+    # (28 patches per row, 112^2 semseg), non-square images (an nh / nw swap) and a batch past loss_finalize_kernel's 256
+    # threads.  An ignored pixel adds no loss and no gradient but still counts in its sample's denominator.
+    def ce64(smoothing, scale):
+        def f(p_, t, m):
+            nll = torch.nn.functional.cross_entropy(p_.double(), t, reduction="none", ignore_index=-100,
+                                                    label_smoothing=smoothing)
+            return O._masked_mean(nll, m, scale)
+        return f
+
+    def ignore(t, frac):
+        t = t.clone()
+        t[torch.rand(t.shape, generator=g) < frac] = -100
+        return t
+
+    def patch_mask(b, nh, nw):
+        m = (torch.rand(b, nh * nw, generator=g) > 0.4).long()
+        m[0] = 0                                              # a sample without masked patches
+        return m
+
+    extra = [
+        (MaskedCrossEntropyLoss(16, 4, label_smoothing=0.1), ce64(0.1, 4), torch.randn(B, 133, 56, 56, generator=g) * 2,
+         torch.randint(0, 133, (B, 56, 56), generator=g), mask),
+        (MaskedCrossEntropyLoss(16, 4), ce64(0.0, 4), torch.randn(B, 133, 56, 56, generator=g) * 2,
+         ignore(torch.randint(0, 133, (B, 56, 56), generator=g), 0.1), mask),
+        (MaskedCrossEntropyLoss(16, 4, label_smoothing=0.1), ce64(0.1, 4), torch.randn(B, 133, 56, 56, generator=g) * 2,
+         ignore(torch.randint(0, 133, (B, 56, 56), generator=g), 0.1), mask),
+        (MaskedMSELoss(16, 1), lambda p_, t, m: O.masked_mse(p_.double(), t.double(), m, 16, 1),
+         torch.randn(2, 3, 448, 448, generator=g), torch.randn(2, 3, 448, 448, generator=g), patch_mask(2, 28, 28)),
+        (MaskedCrossEntropyLoss(16, 4), ce64(0.0, 4), torch.randn(2, 133, 112, 112, generator=g) * 2,
+         ignore(torch.randint(0, 133, (2, 112, 112), generator=g), 0.05), patch_mask(2, 28, 28)),
+        (MaskedMSELoss(16, 1, norm_pix=True), lambda p_, t, m: O.masked_mse(p_.double(), t.double(), m, 16, 1, norm_pix=True),
+         torch.randn(3, 3, 224, 320, generator=g), torch.randn(3, 3, 224, 320, generator=g) * 2 + 1, patch_mask(3, 14, 20)),
+        (MaskedL1Loss(16, 1), lambda p_, t, m: O.masked_l1(p_.double(), t.double(), m, 16, 1),
+         torch.randn(3, 1, 224, 320, generator=g), torch.randn(3, 1, 224, 320, generator=g), patch_mask(3, 14, 20)),
+        (MaskedCrossEntropyLoss(16, 4, label_smoothing=0.1), ce64(0.1, 4), torch.randn(3, 133, 56, 80, generator=g) * 2,
+         torch.randint(0, 133, (3, 56, 80), generator=g), patch_mask(3, 14, 20)),
+        (MaskedMSELoss(16, 1), lambda p_, t, m: O.masked_mse(p_.double(), t.double(), m, 16, 1),
+         torch.randn(300, 3, 32, 48, generator=g), torch.randn(300, 3, 32, 48, generator=g), patch_mask(300, 2, 3)),
+    ]
+    for mod, rfn, pred, tgt, mk in extra:
+        name = "%s(smoothing=%s) %s" % (type(mod).__name__, mod.label_smoothing, tuple(pred.shape))
+        pr = pred.double().requires_grad_(True)
+        ref = rfn(pr, tgt, mk)
+        pc = pred.to(dev).requires_grad_(True)
+        got = mod(pc, tgt.to(dev), mask=mk.to(dev))
+        assert abs(float(got) - float(ref)) <= 2e-5 * max(1.0, abs(float(ref))), (name, float(got), float(ref))
+        ref.backward()
+        got.backward()
+        live = mk.sum(1) > 0
+        assert float(pc.grad[(~live).to(dev)].abs().sum()) == 0.0, name
+        assert rel_l2(pc.grad[live.to(dev)], pr.grad[live]) < 1e-5, (name, rel_l2(pc.grad[live.to(dev)], pr.grad[live]))
+
 
 def test_flat_adamw_matches_torch(dev):
     from multimae_b200 import functional as Fn
