@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 12
+#define MMAE_ABI_VERSION 13
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -602,6 +602,16 @@ int mmae_grad_unscale_norm(float* grads, int64_t n, const float* inv_scale_dev, 
 int mmae_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, int64_t n, float lr,
                     float beta1, float beta2, float eps, float weight_decay, int step, const float* found_inf_dev,
                     const float* dyn_lr_step_dev, void* stream);
+
+/* Model EMA (utils/model_ema.py:72-84, ModelEma.update): for each i < count, the fp32 tensors dst_host[i] (EMA copy) and
+ * src_host[i] (live model) of n_host[i] elements (the three arrays are HOST arrays of device pointers / sizes) get
+ *   dst = dst * decay + one_minus_decay * src
+ * with two rounded products and a rounded sum, which is what the reference's torch ops compute when decay =
+ * float(d) and one_minus_decay = float(1.0 - d), the subtraction done in double.  Up to 256 segments go in one launch
+ * (more are split over several); nothing is allocated or copied to the device.  Every argument is checked before the
+ * first launch: null pointers (allowed for n = 0), negative sizes and a non-finite decay are refused. */
+int mmae_ema_update(float* const* dst_host, const float* const* src_host, const int64_t* n_host, int count, float decay,
+                    float one_minus_decay, void* stream);
 
 /* image <-> token layout helpers ('b (nh nw) (c ph pw) <-> b c (nh ph) (nw pw)') */
 int mmae_unpatchify(const float* tokens, int64_t ld_tok, float* image, int B, int C, int nh, int nw, int P,

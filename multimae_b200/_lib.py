@@ -220,6 +220,8 @@ SIGNATURES = {
     "mmae_weight_mirror_register": (c_int, [c_void_p, c_void_p, c_i64]),
     "mmae_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_float, c_float, c_float, c_float,
                                 c_float, c_int, c_void_p, c_void_p, c_void_p]),
+    "mmae_ema_update": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), ctypes.POINTER(c_i64), c_int, c_float,
+                                c_float, c_void_p]),
     "mmae_unpatchify": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -299,7 +301,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 
 def lib():

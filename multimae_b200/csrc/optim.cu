@@ -4,6 +4,11 @@
 // reference launches ~344 per-tensor norm kernels + a stack + a norm; the L2 norm of per-tensor L2 norms equals the
 // L2 norm of the concatenation, so one pass over the flat gradient buffer suffices.
 // mmae_adamw_step is torch.optim.AdamW's update (utils/optim_factory.py:155-174 builds it) over flat buffers.
+// mmae_ema_update is ModelEma.update (utils/model_ema.py:72-84) over a list of separately allocated tensor pairs: one
+// launch instead of four torch kernels per state_dict entry.  ema_kernel: 256 threads, 64 registers (4 blocks per SM),
+// no spills (ptxas -v, sm_90a); its segment table travels as a by-value kernel parameter (EmaSegments, 7,176 bytes).
+#include <climits>
+
 #include "common.cuh"
 #include "../../include/multimae_b200.h"
 #include "internal.h"
@@ -122,6 +127,70 @@ __global__ void __launch_bounds__(256) adamw_kernel(float* __restrict__ p, const
 #undef MMAE_ADAM1
 }
 
+// ---- model EMA: e = e * d + omd * v over a list of (dst, src, n) segments
+constexpr int EMA_MAX_SEGMENTS = 256;
+constexpr int EMA_THREADS = 256;
+constexpr int EMA_UNROLL = 4;                                              // independent 16-byte loads per operand
+constexpr int64_t EMA_CHUNK = int64_t(EMA_THREADS) * 4 * EMA_UNROLL;      // elements of one segment per block iteration
+
+// by-value kernel argument (7,176 bytes; kernel parameters may be up to 32,764 bytes from CUDA 12.1 on sm_70+): nothing
+// to allocate or upload, so a launch is stream-ordered like any other and can be captured in a graph
+struct EmaSegments {
+  int count;
+  int chunk_off[EMA_MAX_SEGMENTS + 1];   // prefix sum of ceil(n / EMA_CHUNK) per segment
+  float* dst[EMA_MAX_SEGMENTS];
+  const float* src[EMA_MAX_SEGMENTS];
+  int64_t n[EMA_MAX_SEGMENTS];
+};
+
+// `ema_v * decay + (1. - decay) * model_v` as torch evaluates it in fp32: two rounded products, one rounded sum, no FMA
+__device__ __forceinline__ float ema1(float e, float v, float d, float omd) {
+  return __fadd_rn(__fmul_rn(e, d), __fmul_rn(omd, v));
+}
+
+__global__ void __launch_bounds__(EMA_THREADS) ema_kernel(const __grid_constant__ EmaSegments segs, float d, float omd) {
+  pdl_prologue();
+  const int total = segs.chunk_off[segs.count];
+  for (int c = blockIdx.x; c < total; c += gridDim.x) {
+    int s = 0, hi = segs.count - 1;        // the segment with chunk_off[s] <= c < chunk_off[s + 1] (block-uniform search)
+    while (s < hi) {
+      const int mid = (s + hi + 1) >> 1;
+      if (segs.chunk_off[mid] <= c) s = mid; else hi = mid - 1;
+    }
+    float* __restrict__ e = segs.dst[s];
+    const float* __restrict__ v = segs.src[s];
+    const int64_t base = int64_t(c - segs.chunk_off[s]) * EMA_CHUNK;
+    const int64_t end = min(base + EMA_CHUNK, segs.n[s]);
+    if (((reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(v)) & 15) == 0) {
+      uint4 ev[EMA_UNROLL], vv[EMA_UNROLL];
+#pragma unroll
+      for (int u = 0; u < EMA_UNROLL; ++u) {
+        const int64_t i = base + int64_t(u * EMA_THREADS + threadIdx.x) * 4;
+        if (i + 4 <= end) {
+          ev[u] = ld_stream_16_rw(e + i);
+          vv[u] = ld_stream_16(v + i);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < EMA_UNROLL; ++u) {
+        const int64_t i = base + int64_t(u * EMA_THREADS + threadIdx.x) * 4;
+        if (i + 4 <= end) {
+          float4 r;
+          r.x = ema1(__uint_as_float(ev[u].x), __uint_as_float(vv[u].x), d, omd);
+          r.y = ema1(__uint_as_float(ev[u].y), __uint_as_float(vv[u].y), d, omd);
+          r.z = ema1(__uint_as_float(ev[u].z), __uint_as_float(vv[u].z), d, omd);
+          r.w = ema1(__uint_as_float(ev[u].w), __uint_as_float(vv[u].w), d, omd);
+          *reinterpret_cast<float4*>(e + i) = r;
+        } else if (i < end) {
+          for (int64_t j = i; j < end; ++j) e[j] = ema1(e[j], v[j], d, omd);
+        }
+      }
+    } else {                               // a view whose data does not start on a 16-byte boundary
+      for (int64_t j = base + threadIdx.x; j < end; j += EMA_THREADS) e[j] = ema1(e[j], v[j], d, omd);
+    }
+  }
+}
+
 }  // namespace
 }  // namespace mmae
 
@@ -170,5 +239,45 @@ extern "C" int mmae_adamw_step(float* params, const float* grads, float* exp_avg
       const_cast<bf16*>(mirror_lookup(params)));
   count_launch();
   MMAE_LAUNCH_OK();
+  return MMAE_OK;
+}
+
+extern "C" int mmae_ema_update(float* const* dst_host, const float* const* src_host, const int64_t* n_host, int count,
+                               float decay, float one_minus_decay, void* stream) {
+  MMAE_CHECK(count >= 0 && (count == 0 || (dst_host && src_host && n_host)), MMAE_ERR_ARG,
+             "mmae_ema_update: bad args (count %d)", count);
+  MMAE_CHECK(isfinite(decay) && isfinite(one_minus_decay), MMAE_ERR_ARG, "mmae_ema_update: non-finite decay");
+  for (int i = 0; i < count; ++i) {
+    MMAE_CHECK(n_host[i] >= 0, MMAE_ERR_ARG, "mmae_ema_update: segment %d: negative size", i);
+    MMAE_CHECK(n_host[i] == 0 || (dst_host[i] && src_host[i]), MMAE_ERR_ARG, "mmae_ema_update: segment %d: null pointer",
+               i);
+    MMAE_CHECK((n_host[i] + EMA_CHUNK - 1) / EMA_CHUNK <= INT_MAX / 2, MMAE_ERR_ARG,
+               "mmae_ema_update: segment %d is too large", i);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  EmaSegments segs;
+  int i = 0;
+  while (i < count) {
+    // pack the next non-empty segments: as many as one launch holds, with a chunk count that stays within an int
+    segs.count = 0;
+    segs.chunk_off[0] = 0;
+    for (; i < count && segs.count < EMA_MAX_SEGMENTS; ++i) {
+      if (n_host[i] == 0) continue;
+      const int64_t chunks = (n_host[i] + EMA_CHUNK - 1) / EMA_CHUNK;
+      if (segs.count > 0 && segs.chunk_off[segs.count] + chunks > INT_MAX / 2) break;
+      segs.dst[segs.count] = dst_host[i];
+      segs.src[segs.count] = src_host[i];
+      segs.n[segs.count] = n_host[i];
+      segs.chunk_off[segs.count + 1] = segs.chunk_off[segs.count] + int(chunks);
+      ++segs.count;
+    }
+    if (segs.count == 0) break;
+    int64_t blocks = segs.chunk_off[segs.count];
+    const int64_t cap = int64_t(sm_count()) * 8;
+    if (blocks > cap) blocks = cap;
+    launch_k(ema_kernel, (unsigned)blocks, EMA_THREADS, 0, st, segs, decay, one_minus_decay);
+    count_launch();
+    MMAE_LAUNCH_OK();
+  }
   return MMAE_OK;
 }

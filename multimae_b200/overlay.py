@@ -5,7 +5,8 @@ so the reference's UNCHANGED run_pretraining_multimae.py drives the sm_90a path.
 
 What is replaced (north_star "Subsystems replaced"): multimae.multimae, multimae.multimae_utils, multimae.input_adapters,
 multimae.output_adapters (SpatialOutputAdapter, LinearOutputAdapter, ConvNeXtAdapter), multimae.criterion,
-utils.native_scaler.NativeScalerWithGradNormCount and — because the model owns its bucketed gradient all-reduce —
+utils.native_scaler.NativeScalerWithGradNormCount, utils.ModelEma (also as utils.model_ema.ModelEma and
+utils.model.ModelEma, the name unwrap_model tests) and — because the model owns its bucketed gradient all-reduce —
 torch.nn.parallel.DistributedDataParallel is substituted by an identity wrapper.  Everything else (argument parsing, data pipeline, optimizer factory, logging, checkpoints)
 stays the reference's own code from `reference_root`."""
 import importlib
@@ -105,6 +106,14 @@ def install(reference_root=None, replace_ddp=True, legacy_checkpoint_load=True):
         utils.NativeScalerWithGradNormCount = NativeScalerWithGradNormCount
         utils.native_scaler.NativeScalerWithGradNormCount = NativeScalerWithGradNormCount
         utils.native_scaler.get_grad_norm_ = get_grad_norm_
+    except Exception:  # noqa: BLE001
+        pass
+    try:
+        import utils  # type: ignore
+        from .model_ema import ModelEma
+        utils.ModelEma = ModelEma
+        utils.model_ema.ModelEma = ModelEma
+        utils.model.ModelEma = ModelEma            # unwrap_model's isinstance test: save_model stores the EMA's state_dict
     except Exception:  # noqa: BLE001
         pass
     from . import lazy_meters
