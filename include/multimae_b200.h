@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 13
+#define MMAE_ABI_VERSION 14
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -612,6 +612,34 @@ int mmae_adamw_step(float* params, const float* grads, float* exp_avg, float* ex
  * first launch: null pointers (allowed for n = 0), negative sizes and a non-finite decay are refused. */
 int mmae_ema_update(float* const* dst_host, const float* const* src_host, const int64_t* n_host, int count, float decay,
                     float one_minus_decay, void* stream);
+
+/* One segment of mmae_adamw_step_groups: n fp32 elements of parameters, gradients and both moments, an optional bf16
+ * twin of the parameters (NULL: none), and the index of the parameter group whose lr / weight decay apply. */
+typedef struct MmaeAdamwSegment {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  void* mirror_bf16;
+  int64_t n;
+  int group;
+  int reserved;
+} MmaeAdamwSegment;
+
+/* torch.optim.AdamW with parameter groups (utils/optim_factory.py:49-101 builds them: per-layer lr_scale, weight decay
+ * 0.05 or 0) over the HOST array segs_host[0 .. count): each segment is updated with lr_host[group] and
+ * weight_decay_host[group] (HOST arrays of num_groups doubles) and the shared beta1 / beta2 / eps, in the order of torch's
+ * _multi_tensor_adam: p *= 1 - lr*wd; m = lerp(m, g, 1 - beta1); v = v*beta2 + (1 - beta2)*g*g;
+ * p += -(lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps), the scalars evaluated in double and rounded to fp32.  A non-NULL
+ * mirror_bf16 receives bf16(p).  step_dev (device float) is the step count: the call advances it by one and derives the
+ * bias corrections bc1 = 1 - beta1^step, bc2 = 1 - beta2^step from it on the device.  When found_inf_dev is non-NULL and
+ * found_inf_dev[0] != 0, nothing is written: parameters, moments, twins and the step count keep their values.  Up to 448
+ * segments go in one launch (more are split over several); nothing is allocated or copied to the device.  Every argument
+ * is checked before the first launch: null pointers (allowed for n = 0), negative sizes, group indices outside
+ * [0, num_groups), non-finite lr / weight decay / betas / eps, and pointers that are not 16-byte aligned are refused. */
+int mmae_adamw_step_groups(const MmaeAdamwSegment* segs_host, int count, const double* lr_host,
+                           const double* weight_decay_host, int num_groups, double beta1, double beta2, double eps,
+                           const float* found_inf_dev, float* step_dev, void* stream);
 
 /* image <-> token layout helpers ('b (nh nw) (c ph pw) <-> b c (nh ph) (nw pw)') */
 int mmae_unpatchify(const float* tokens, int64_t ld_tok, float* image, int B, int C, int nh, int nw, int P,

@@ -110,6 +110,11 @@ class CtxProjGrads(ctypes.Structure):
     _fields_ = [("weight", c_void_p * MAX_TASKS)]
 
 
+class AdamwSegment(ctypes.Structure):
+    _fields_ = [("param", c_void_p), ("grad", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
+                ("mirror_bf16", c_void_p), ("n", c_i64), ("group", c_int), ("reserved", c_int)]
+
+
 class MmaeError(RuntimeError):
     pass
 
@@ -222,6 +227,9 @@ SIGNATURES = {
                                 c_float, c_int, c_void_p, c_void_p, c_void_p]),
     "mmae_ema_update": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), ctypes.POINTER(c_i64), c_int, c_float,
                                 c_float, c_void_p]),
+    "mmae_adamw_step_groups": (c_int, [ctypes.POINTER(AdamwSegment), c_int, ctypes.POINTER(ctypes.c_double),
+                                       ctypes.POINTER(ctypes.c_double), c_int, ctypes.c_double, ctypes.c_double,
+                                       ctypes.c_double, c_void_p, c_void_p, c_void_p]),
     "mmae_unpatchify": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -301,7 +309,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 
 def lib():

@@ -7,6 +7,10 @@
 // mmae_ema_update is ModelEma.update (utils/model_ema.py:72-84) over a list of separately allocated tensor pairs: one
 // launch instead of four torch kernels per state_dict entry.  ema_kernel: 256 threads, 64 registers (4 blocks per SM),
 // no spills (ptxas -v, sm_90a); its segment table travels as a by-value kernel parameter (EmaSegments, 7,176 bytes).
+// mmae_adamw_step_groups is torch.optim.AdamW with parameter groups (the fine-tuning scripts' layer-decay groups) over a
+// list of segments, each with its group's lr / weight decay: one launch for the whole model.  adamw_groups_kernel: 256
+// threads, 86 registers (2 blocks per SM), no spills (ptxas -v, sm_90a); segment table by value (AdamwSegments, 28,680
+// bytes).  step_advance_kernel: 8 registers, no spills.
 #include <climits>
 
 #include "common.cuh"
@@ -191,6 +195,117 @@ __global__ void __launch_bounds__(EMA_THREADS) ema_kernel(const __grid_constant_
   }
 }
 
+// ---- grouped AdamW: torch.optim.AdamW over a list of (param, grad, exp_avg, exp_avg_sq, bf16 twin, n) segments, each
+// with its parameter group's learning rate and weight decay (layer-decay groups of the fine-tuning scripts)
+constexpr int ADAMW_MAX_SEGMENTS = 448;
+constexpr int ADAMW_THREADS = 256;
+constexpr int ADAMW_UNROLL = 2;                                            // independent 16-byte loads per operand
+constexpr int64_t ADAMW_CHUNK = int64_t(ADAMW_THREADS) * 4 * ADAMW_UNROLL;
+
+// by-value kernel argument, like EmaSegments: the launch allocates and uploads nothing
+struct AdamwSegments {
+  int count;
+  int chunk_off[ADAMW_MAX_SEGMENTS + 1];   // prefix sum of ceil(n / ADAMW_CHUNK) per segment
+  float* p[ADAMW_MAX_SEGMENTS];
+  const float* g[ADAMW_MAX_SEGMENTS];
+  float* m[ADAMW_MAX_SEGMENTS];
+  float* v[ADAMW_MAX_SEGMENTS];
+  bf16* mirror[ADAMW_MAX_SEGMENTS];       // NULL: no twin
+  int64_t n[ADAMW_MAX_SEGMENTS];
+  double lr[ADAMW_MAX_SEGMENTS];          // the segment's group learning rate
+  float decay[ADAMW_MAX_SEGMENTS];        // float(1 - lr * weight_decay), evaluated in double
+};
+// the struct plus the eight scalar / pointer arguments of adamw_groups_kernel stay within the 32,764-byte limit
+static_assert(sizeof(AdamwSegments) + 64 <= 32764, "AdamwSegments exceeds the kernel parameter limit");
+
+__global__ void step_advance_kernel(float* __restrict__ step, const float* __restrict__ found_inf) {
+  pdl_prologue();
+  if (found_inf == nullptr || found_inf[0] == 0.f) step[0] += 1.0f;
+}
+
+// torch's _multi_tensor_adam (decoupled weight decay) order of operations, in fp32 with the scalars rounded from double:
+//   p *= 1 - lr*wd;  m = lerp(m, g, 1 - b1);  v = v*b2 + (1 - b2)*g*g;  p += -(lr/bc1) * m / (sqrt(v)/sqrt(bc2) + eps)
+__device__ __forceinline__ void adamw1(float& p, float g, float& m, float& v, float decay, float omb1, float b2, float omb2,
+                                       float bc2s, float eps, float step_size) {
+  p = __fmul_rn(p, decay);
+  m = __fmaf_rn(omb1, __fsub_rn(g, m), m);
+  v = __fmaf_rn(omb2, __fmul_rn(g, g), __fmul_rn(v, b2));
+  const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2s), eps);
+  p = __fmaf_rn(step_size, __fdiv_rn(m, denom), p);
+}
+
+__global__ void __launch_bounds__(ADAMW_THREADS) adamw_groups_kernel(const __grid_constant__ AdamwSegments segs, double beta1,
+                                                                     double beta2, float omb1, float b2, float omb2,
+                                                                     float eps, const float* __restrict__ found_inf,
+                                                                     const float* __restrict__ step_dev) {
+  pdl_prologue();
+  if (found_inf != nullptr && found_inf[0] != 0.f) return;
+  // bias corrections in double from the device step count (already advanced for this step), as torch computes them
+  const double step = double(step_dev[0]);
+  const double bc1 = 1.0 - pow(beta1, step);
+  const float bc2s = float(sqrt(1.0 - pow(beta2, step)));
+  const int total = segs.chunk_off[segs.count];
+  for (int c = blockIdx.x; c < total; c += gridDim.x) {
+    int s = 0, hi = segs.count - 1;        // the segment with chunk_off[s] <= c < chunk_off[s + 1] (block-uniform search)
+    while (s < hi) {
+      const int mid = (s + hi + 1) >> 1;
+      if (segs.chunk_off[mid] <= c) s = mid; else hi = mid - 1;
+    }
+    float* __restrict__ p = segs.p[s];
+    const float* __restrict__ g = segs.g[s];
+    float* __restrict__ m = segs.m[s];
+    float* __restrict__ v = segs.v[s];
+    bf16* __restrict__ tw = segs.mirror[s];
+    const float decay = segs.decay[s];
+    const float step_size = float(-(segs.lr[s] / bc1));
+    const int64_t base = int64_t(c - segs.chunk_off[s]) * ADAMW_CHUNK;
+    const int64_t end = min(base + ADAMW_CHUNK, segs.n[s]);
+    uint4 pv[ADAMW_UNROLL], gv[ADAMW_UNROLL], mv[ADAMW_UNROLL], vv[ADAMW_UNROLL];
+#pragma unroll
+    for (int u = 0; u < ADAMW_UNROLL; ++u) {
+      const int64_t i = base + int64_t(u * ADAMW_THREADS + threadIdx.x) * 4;
+      if (i + 4 <= end) {
+        pv[u] = ld_stream_16_rw(p + i);
+        gv[u] = ld_stream_16(g + i);
+        mv[u] = ld_stream_16_rw(m + i);
+        vv[u] = ld_stream_16_rw(v + i);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < ADAMW_UNROLL; ++u) {
+      const int64_t i = base + int64_t(u * ADAMW_THREADS + threadIdx.x) * 4;
+      if (i + 4 <= end) {
+        float4 P = make_float4(__uint_as_float(pv[u].x), __uint_as_float(pv[u].y), __uint_as_float(pv[u].z),
+                               __uint_as_float(pv[u].w));
+        float4 M = make_float4(__uint_as_float(mv[u].x), __uint_as_float(mv[u].y), __uint_as_float(mv[u].z),
+                               __uint_as_float(mv[u].w));
+        float4 V = make_float4(__uint_as_float(vv[u].x), __uint_as_float(vv[u].y), __uint_as_float(vv[u].z),
+                               __uint_as_float(vv[u].w));
+        adamw1(P.x, __uint_as_float(gv[u].x), M.x, V.x, decay, omb1, b2, omb2, bc2s, eps, step_size);
+        adamw1(P.y, __uint_as_float(gv[u].y), M.y, V.y, decay, omb1, b2, omb2, bc2s, eps, step_size);
+        adamw1(P.z, __uint_as_float(gv[u].z), M.z, V.z, decay, omb1, b2, omb2, bc2s, eps, step_size);
+        adamw1(P.w, __uint_as_float(gv[u].w), M.w, V.w, decay, omb1, b2, omb2, bc2s, eps, step_size);
+        *reinterpret_cast<float4*>(p + i) = P;
+        *reinterpret_cast<float4*>(m + i) = M;
+        *reinterpret_cast<float4*>(v + i) = V;
+        if (tw != nullptr) {
+          uint2 pk;
+          pk.x = pack_bf16x2(P.x, P.y);
+          pk.y = pack_bf16x2(P.z, P.w);
+          *reinterpret_cast<uint2*>(tw + i) = pk;
+        }
+      } else if (i < end) {                // the last 1-3 elements of a segment whose size is not a multiple of 4
+        for (int64_t j = i; j < end; ++j) {
+          float P = p[j], M = m[j], V = v[j];
+          adamw1(P, g[j], M, V, decay, omb1, b2, omb2, bc2s, eps, step_size);
+          p[j] = P; m[j] = M; v[j] = V;
+          if (tw != nullptr) tw[j] = __float2bfloat16_rn(P);
+        }
+      }
+    }
+  }
+}
+
 }  // namespace
 }  // namespace mmae
 
@@ -276,6 +391,74 @@ extern "C" int mmae_ema_update(float* const* dst_host, const float* const* src_h
     const int64_t cap = int64_t(sm_count()) * 8;
     if (blocks > cap) blocks = cap;
     launch_k(ema_kernel, (unsigned)blocks, EMA_THREADS, 0, st, segs, decay, one_minus_decay);
+    count_launch();
+    MMAE_LAUNCH_OK();
+  }
+  return MMAE_OK;
+}
+
+extern "C" int mmae_adamw_step_groups(const MmaeAdamwSegment* segs_host, int count, const double* lr_host,
+                                      const double* weight_decay_host, int num_groups, double beta1, double beta2,
+                                      double eps, const float* found_inf_dev, float* step_dev, void* stream) {
+  MMAE_CHECK(count >= 0 && num_groups >= 0 && (count == 0 || (segs_host && num_groups > 0)), MMAE_ERR_ARG,
+             "mmae_adamw_step_groups: bad args (count %d, num_groups %d)", count, num_groups);
+  MMAE_CHECK(num_groups == 0 || (lr_host && weight_decay_host), MMAE_ERR_ARG,
+             "mmae_adamw_step_groups: null group arrays");
+  MMAE_CHECK(step_dev != nullptr, MMAE_ERR_ARG, "mmae_adamw_step_groups: null step counter");
+  MMAE_CHECK(isfinite(beta1) && isfinite(beta2) && isfinite(eps) && beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 &&
+                 beta2 < 1.0 && eps >= 0.0,
+             MMAE_ERR_ARG, "mmae_adamw_step_groups: bad betas / eps (%g, %g, %g)", beta1, beta2, eps);
+  for (int k = 0; k < num_groups; ++k)
+    MMAE_CHECK(isfinite(lr_host[k]) && isfinite(weight_decay_host[k]), MMAE_ERR_ARG,
+               "mmae_adamw_step_groups: group %d: non-finite lr / weight_decay", k);
+  for (int i = 0; i < count; ++i) {
+    const MmaeAdamwSegment& sg = segs_host[i];
+    MMAE_CHECK(sg.n >= 0, MMAE_ERR_ARG, "mmae_adamw_step_groups: segment %d: negative size", i);
+    MMAE_CHECK(sg.group >= 0 && sg.group < num_groups, MMAE_ERR_ARG,
+               "mmae_adamw_step_groups: segment %d: group %d out of range", i, sg.group);
+    if (sg.n == 0) continue;
+    MMAE_CHECK(sg.param && sg.grad && sg.exp_avg && sg.exp_avg_sq, MMAE_ERR_ARG,
+               "mmae_adamw_step_groups: segment %d: null pointer", i);
+    MMAE_CHECK(((reinterpret_cast<uintptr_t>(sg.param) | reinterpret_cast<uintptr_t>(sg.grad) |
+                 reinterpret_cast<uintptr_t>(sg.exp_avg) | reinterpret_cast<uintptr_t>(sg.exp_avg_sq) |
+                 reinterpret_cast<uintptr_t>(sg.mirror_bf16)) & 15) == 0,
+               MMAE_ERR_ARG, "mmae_adamw_step_groups: segment %d: pointers must be 16-byte aligned", i);
+    MMAE_CHECK((sg.n + ADAMW_CHUNK - 1) / ADAMW_CHUNK <= INT_MAX / 2, MMAE_ERR_ARG,
+               "mmae_adamw_step_groups: segment %d is too large", i);
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // the step count advances (on the device, only for a step that is taken) before the update reads it
+  launch_k(step_advance_kernel, 1, 1, 0, st, step_dev, found_inf_dev);
+  count_launch();
+  MMAE_LAUNCH_OK();
+  AdamwSegments segs;
+  int i = 0;
+  while (i < count) {
+    segs.count = 0;
+    segs.chunk_off[0] = 0;
+    for (; i < count && segs.count < ADAMW_MAX_SEGMENTS; ++i) {
+      const MmaeAdamwSegment& sg = segs_host[i];
+      if (sg.n == 0) continue;
+      const int64_t chunks = (sg.n + ADAMW_CHUNK - 1) / ADAMW_CHUNK;
+      if (segs.count > 0 && segs.chunk_off[segs.count] + chunks > INT_MAX / 2) break;
+      const int k = segs.count;
+      segs.p[k] = sg.param;
+      segs.g[k] = sg.grad;
+      segs.m[k] = sg.exp_avg;
+      segs.v[k] = sg.exp_avg_sq;
+      segs.mirror[k] = reinterpret_cast<bf16*>(sg.mirror_bf16);
+      segs.n[k] = sg.n;
+      segs.lr[k] = lr_host[sg.group];
+      segs.decay[k] = float(1.0 - lr_host[sg.group] * weight_decay_host[sg.group]);
+      segs.chunk_off[k + 1] = segs.chunk_off[k] + int(chunks);
+      ++segs.count;
+    }
+    if (segs.count == 0) break;
+    int64_t blocks = segs.chunk_off[segs.count];
+    const int64_t cap = int64_t(sm_count()) * 8;
+    if (blocks > cap) blocks = cap;
+    launch_k(adamw_groups_kernel, (unsigned)blocks, ADAMW_THREADS, 0, st, segs, beta1, beta2, float(1.0 - beta1),
+             float(beta2), float(1.0 - beta2), float(eps), found_inf_dev, static_cast<const float*>(step_dev));
     count_launch();
     MMAE_LAUNCH_OK();
   }

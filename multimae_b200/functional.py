@@ -1126,3 +1126,11 @@ def adamw_step(params, grads, exp_avg, exp_avg_sq, lr, betas, eps, weight_decay,
                                     float(weight_decay), max(int(step), 1), L.ptr(found_inf), L.ptr(dyn),
                                     L.current_stream()), "mmae_adamw_step")
 
+
+def adamw_step_groups(segments, count, lrs, weight_decays, betas, eps, step, found_inf=None):
+    """One grouped AdamW step: `segments` a ctypes array of L.AdamwSegment (its first `count` entries are used), `lrs` /
+    `weight_decays` ctypes double arrays with one entry per parameter group, `step` the device step counter (float32 [1])."""
+    L.check(L.lib().mmae_adamw_step_groups(segments, count, lrs, weight_decays, len(lrs), float(betas[0]), float(betas[1]),
+                                           float(eps), L.ptr(found_inf), step.data_ptr(), L.current_stream()),
+            "mmae_adamw_step_groups")
+

@@ -8,6 +8,7 @@ fused transformer blocks, fused decoder head/tail, gradients accumulated into on
 import itertools
 import os
 import math
+import weakref
 from collections import OrderedDict
 from functools import partial
 from typing import Dict, List, Optional, Union
@@ -36,6 +37,14 @@ __all__ = ["pretrain_multimae_base", "pretrain_multimae_large", "multivit_base",
 # gradient arena on its first training forward, so that the script's scaler (which only sees model.parameters()) takes the
 # one-pass unscale / norm path instead of ~344 per-tensor launches, and autograd does not clone 98 M gradients per step.
 AUTO_OWN_GRADIENTS = False
+# every MultiMAE / MultiViT alive: GroupedFlatAdamW finds the model that owns the parameters it is given here
+_LIVE_MODELS = weakref.WeakSet()
+
+
+def live_models():
+    return list(_LIVE_MODELS)
+
+
 # one GEMM for the proj_context Linears of all half-precision output adapters (MultiMAE._project_contexts); 0: one per adapter
 SHARED_CONTEXT_PROJECTION = os.environ.get("MMAE_SHARED_CTX", "1") != "0"
 
@@ -137,6 +146,7 @@ class MultiMAE(nn.Module):
         # task decoders on concurrent CUDA streams (MMAE_DECODER_STREAMS=0 runs them one after the other)
         self.decoder_streams = os.environ.get("MMAE_DECODER_STREAMS", "1") != "0"
         self._dec_streams = None
+        _LIVE_MODELS.add(self)
 
     def draw_task_shares(self, B, n_tasks, alphas=1.0, sample_tasks_uniformly=False):
         """Host-side Dirichlet draw of generate_random_masks (multimae/multimae.py:182-187) as a separate step."""

@@ -6,7 +6,8 @@ so the reference's UNCHANGED run_pretraining_multimae.py drives the sm_90a path.
 What is replaced (north_star "Subsystems replaced"): multimae.multimae, multimae.multimae_utils, multimae.input_adapters,
 multimae.output_adapters (SpatialOutputAdapter, LinearOutputAdapter, ConvNeXtAdapter), multimae.criterion,
 utils.native_scaler.NativeScalerWithGradNormCount, utils.ModelEma (also as utils.model_ema.ModelEma and
-utils.model.ModelEma, the name unwrap_model tests) and — because the model owns its bucketed gradient all-reduce —
+utils.model.ModelEma, the name unwrap_model tests), with MMAE_FLAT_ADAMW=1 the AdamW that utils.optim_factory builds
+(GroupedFlatAdamW) and — because the model owns its bucketed gradient all-reduce —
 torch.nn.parallel.DistributedDataParallel is substituted by an identity wrapper.  Everything else (argument parsing, data pipeline, optimizer factory, logging, checkpoints)
 stays the reference's own code from `reference_root`."""
 import importlib
@@ -51,6 +52,23 @@ class _Wrapped:
 
     def __getattr__(self, name):
         return getattr(self.__dict__["module"], name)
+
+
+class _FactoryOptim:
+    """MMAE_FLAT_ADAMW=1: what utils.optim_factory sees as `optim` (torch.optim).  `AdamW` builds the one-kernel
+    multimae_b200.optim.GroupedFlatAdamW - or torch's AdamW, with one printed line, when a trainable parameter is not on
+    CUDA or not a parameter of the MultiMAE / MultiViT; every other name (SGD, Adam) is torch's."""
+
+    def __init__(self, stock):
+        self._stock = stock
+
+    def __getattr__(self, name):
+        return getattr(self._stock, name)
+
+    @staticmethod
+    def AdamW(params, *args, **kwargs):
+        from .optim import adamw_or_stock
+        return adamw_or_stock(params, *args, **kwargs)
 
 
 def _legacy_checkpoint_load():
@@ -116,6 +134,13 @@ def install(reference_root=None, replace_ddp=True, legacy_checkpoint_load=True):
         utils.model.ModelEma = ModelEma            # unwrap_model's isinstance test: save_model stores the EMA's state_dict
     except Exception:  # noqa: BLE001
         pass
+    if os.environ.get("MMAE_FLAT_ADAMW", "0") == "1":
+        try:
+            import utils.optim_factory as factory  # type: ignore
+            if not isinstance(factory.optim, _FactoryOptim):
+                factory.optim = _FactoryOptim(factory.optim)   # create_optimizer calls optim.AdamW through this global
+        except Exception:  # noqa: BLE001
+            pass
     from . import lazy_meters
     lazy_meters.install()                          # MMAE_LAZY_METERS=1: the script's ~10 .item() per step answer one step late
     from . import data
