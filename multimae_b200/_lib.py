@@ -230,6 +230,9 @@ SIGNATURES = {
     "mmae_adamw_step_groups": (c_int, [ctypes.POINTER(AdamwSegment), c_int, ctypes.POINTER(ctypes.c_double),
                                        ctypes.POINTER(ctypes.c_double), c_int, ctypes.c_double, ctypes.c_double,
                                        ctypes.c_double, c_void_p, c_void_p, c_void_p]),
+    "mmae_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, ctypes.POINTER(c_int), c_int, c_i64, c_void_p,
+                                   c_i64, ctypes.POINTER(c_void_p), ctypes.POINTER(c_float), ctypes.POINTER(c_float),
+                                   c_void_p]),
     "mmae_unpatchify": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -309,7 +312,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 
 def lib():

@@ -127,3 +127,27 @@ def attention_bwd(q, k, v, o, do, lse, dq, dk, dv, B, H, Nq, Nk, dh, scale):
                                             lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dq.stride(0),
                                             dk.data_ptr(), dk.stride(0), dv.data_ptr(), dv.stride(0), B, H, Nq, Nk, dh,
                                             scale, L.current_stream()), "mmae_attention_backward")
+
+
+
+AUGMENT_KINDS = {"rgb": 0, "depth": 1, "semseg": 2, "semseg_coco": 2}     # task -> kind code of mmae_augment_batch
+
+
+def augment_batch(host, dev, tasks, batch, size, map4, scratch_bytes, mean, std):
+    """Resample one packed batch (multimae_b200.data.pack_batch: `host` its uint8 host buffer, `dev` the device copy) on
+    the current stream: {task: fp32 [B,3,S,S] (rgb) | fp32 [B,1,S,S] (depth) | int64 [B,S/4,S/4] (semseg)}."""
+    _need_cuda(dev)
+    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() == dev.numel()
+    kinds = [AUGMENT_KINDS[t] for t in tasks]
+    T, S = len(tasks), int(size)
+    outs = {}
+    for t, k in zip(tasks, kinds):
+        shape = (batch, S // 4, S // 4) if k == 2 else (batch, 3 if k == 0 else 1, S, S)
+        outs[t] = torch.empty(shape, dtype=torch.int64 if k == 2 else torch.float32, device=dev.device)
+    scratch = torch.empty(max(int(scratch_bytes), 16), dtype=torch.uint8, device=dev.device)
+    ptrs = (ctypes.c_void_p * T)(*[outs[t].data_ptr() for t in tasks])
+    L.check(L.lib().mmae_augment_batch(host.data_ptr(), dev.data_ptr(), host.numel(), batch, T, (ctypes.c_int * T)(*kinds),
+                                       S, int(map4), scratch.data_ptr(), int(scratch_bytes), ptrs,
+                                       (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std), L.current_stream()),
+            "mmae_augment_batch")
+    return outs
