@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 15
+#define MMAE_ABI_VERSION 16
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -665,6 +665,26 @@ int mmae_adamw_step_groups(const MmaeAdamwSegment* segs_host, int count, const d
 int mmae_augment_batch(const void* packed_host, const void* packed, int64_t packed_bytes, int batch, int num_tasks,
                        const int* kinds_host, int out_size, int64_t map4_offset, void* scratch, int64_t scratch_bytes,
                        void* const* out_host, const float* mean_host, const float* std_host, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Classification fine-tuning augmentation (MMAE_GPU_AUGMENT) — the pixel half of utils/datasets.py:build_transform:
+ * Pillow-exact Image.resize of each crop to out_size x out_size (BILINEAR or BICUBIC, 8-bit fixed point), the horizontal
+ * flip, then `num_layers` RandAugment layers on the 8-bit image, then TF.normalize(TF.to_tensor(img)).
+ *
+ * `packed` / `packed_host` hold, 16-byte aligned: int32 descriptors [batch][8] as mmae_augment_batch's with one rgb task
+ * (kind 0); at ops_offset * 16 the op records [batch][num_layers] of 72 bytes = {int32 kind, filter, iarg, pad; double
+ * factor; double m[6]} (kinds: 0 identity, 1 invert, 2 posterize iarg bits, 3 solarize threshold iarg, 4 solarize-add
+ * iarg, 5 autocontrast, 6 equalize, 7 color, 8 contrast, 9 brightness, 10 sharpness (blend factor), 11 affine transform
+ * with the inverse matrix m and filter 2 bilinear / 3 bicubic, 12 transpose by iarg = 90 / 180 / 270 degrees); the
+ * tables (type 1 BICUBIC or 3 BILINEAR, mmae_augment_batch's layout, n_in = crop extent, n_out = out_size); the crops.
+ * fill_host: the affine transforms' fill colour (3 ints in [0, 255]).  `scratch`: the horizontal pass's intermediates
+ * (descriptor field 7) from offset 0; with num_layers > 0 then, each section 256-byte aligned after the end of the last
+ * intermediate, two uint8 [batch][S][S][3] images and int32 [batch][1024].  out: fp32 [batch, 3, S, S].
+ * 2 + 2 * num_layers launches for the whole batch.  Every descriptor, table and op record is checked on the host first.
+ * ---------------------------------------------------------------------------------------------- */
+int mmae_cls_augment_batch(const void* packed_host, const void* packed, int64_t packed_bytes, int batch, int num_layers,
+                           int64_t ops_offset, int out_size, const int* fill_host, void* scratch, int64_t scratch_bytes,
+                           float* out, const float* mean_host, const float* std_host, void* stream);
 
 /* image <-> token layout helpers ('b (nh nw) (c ph pw) <-> b c (nh ph) (nw pw)') */
 int mmae_unpatchify(const float* tokens, int64_t ld_tok, float* image, int B, int C, int nh, int nw, int P,

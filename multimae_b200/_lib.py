@@ -233,6 +233,9 @@ SIGNATURES = {
     "mmae_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, ctypes.POINTER(c_int), c_int, c_i64, c_void_p,
                                    c_i64, ctypes.POINTER(c_void_p), ctypes.POINTER(c_float), ctypes.POINTER(c_float),
                                    c_void_p]),
+    "mmae_cls_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_i64, c_int, ctypes.POINTER(c_int),
+                                       c_void_p, c_i64, c_void_p, ctypes.POINTER(c_float), ctypes.POINTER(c_float),
+                                       c_void_p]),
     "mmae_unpatchify": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -312,7 +315,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 
 def lib():

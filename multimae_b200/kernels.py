@@ -151,3 +151,26 @@ def augment_batch(host, dev, tasks, batch, size, map4, scratch_bytes, mean, std)
                                        (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std), L.current_stream()),
             "mmae_augment_batch")
     return outs
+
+
+def cls_scratch_bytes(inter_bytes, batch, size, layers):
+    """Scratch of mmae_cls_augment_batch: the horizontal pass's intermediates, then (with RandAugment layers) two uint8
+    [B, S, S, 3] images and int32 [B, 1024] of per-sample tables, each 256-byte aligned."""
+    a = lambda n: (int(n) + 255) // 256 * 256  # noqa: E731
+    return a(inter_bytes) + (2 * a(batch * size * size * 3) + batch * 1024 * 4 if layers else 0)
+
+
+def cls_augment_batch(host, dev, batch, size, layers, ops_offset, inter_bytes, mean, std, fill):
+    """Resample, flip, RandAugment and normalise one packed classification batch (multimae_b200.data.pack_cls_batch) on
+    the current stream: fp32 [B, 3, S, S]."""
+    _need_cuda(dev)
+    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() == dev.numel()
+    S = int(size)
+    out = torch.empty((batch, 3, S, S), dtype=torch.float32, device=dev.device)
+    nbytes = cls_scratch_bytes(inter_bytes, batch, S, layers)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev.device)
+    L.check(L.lib().mmae_cls_augment_batch(host.data_ptr(), dev.data_ptr(), host.numel(), batch, int(layers),
+                                           int(ops_offset), S, (ctypes.c_int * 3)(*fill), scratch.data_ptr(), nbytes,
+                                           out.data_ptr(), (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std),
+                                           L.current_stream()), "mmae_cls_augment_batch")
+    return out
