@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 16
+#define MMAE_ABI_VERSION 17
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -158,13 +158,17 @@ int mmae_layernorm_backward_ex(const void* dy, int dy_is_bf16, int64_t lddy, con
  * 4 | 64 = wgmma backward; otherwise the mma.sync kernels run (16: no Hopper kernel, ignored); 0 = mma.sync everywhere.
  * Default 0, the fastest measured on H100 (attention.cu); env MMAE_ATTN_TC; a negative value restores the start-up default. */
 int mmae_attention_set_tc(int enable);
+/* dropout_p: dropout on the softmax probabilities (site MMAE_DROP_SITE_ATTN below), its mask from *seed; seed may be NULL
+ * when dropout_p is 0, which means no dropout.  With dropout_p > 0 the mma.sync kernels run whatever
+ * mmae_attention_set_tc selects (the wgmma kernels have no dropout).  lse stays the log-sum-exp of the undropped scores. */
 int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                           void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
-                           float scale, void* stream);
+                           void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim, float scale,
+                           float dropout_p, const uint64_t* seed, void* stream);
 int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                             const void* o, int64_t ldo, const void* d_o, int64_t lddo, const float* lse,
                             float* delta_ws, void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv,
-                            int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale, void* stream);
+                            int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale, float dropout_p,
+                            const uint64_t* seed, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Dropout in training (nn.Dropout, multimae/multimae_utils.py:154,177,181): inverted dropout, a kept element is scaled by
@@ -179,17 +183,6 @@ int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t l
 #define MMAE_DROP_SITE_ATTN 0
 #define MMAE_DROP_SITE_PROJ 1
 #define MMAE_DROP_SITE_MLP 2
-/* the attention entry points with dropout of rate dropout_p on the probabilities (site MMAE_DROP_SITE_ATTN); seed may be
- * NULL when dropout_p is 0, which is the plain call.  With dropout_p > 0 the mma.sync kernels run whatever
- * the attention kernel mask selects (the wgmma kernels have no dropout).  lse stays the log-sum-exp of the undropped scores. */
-int mmae_attention_forward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim, float scale,
-                                float dropout_p, const uint64_t* seed, void* stream);
-int mmae_attention_backward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                 const void* o, int64_t ldo, const void* d_o, int64_t lddo, const float* lse,
-                                 float* delta_ws, void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv,
-                                 int64_t lddv, int B, int H, int Nq, int Nk, int head_dim, float scale, float dropout_p,
-                                 const uint64_t* seed, void* stream);
 /* out[r * cols + c] = keep bit (0 / 1 byte) of element (r, c) of `site` at rate p, from the generator the kernels use;
  * all ones at p = 0.  For tests and inspection: the training path never materialises a mask. */
 int mmae_dropout_keep_mask(const uint64_t* seed, int site, int64_t rows, int cols, float p, void* out, void* stream);
@@ -289,6 +282,19 @@ typedef struct mmae_block_params {
 typedef struct mmae_block_grads {
   float *norm1_w, *norm1_b, *qkv_w, *qkv_b, *proj_w, *proj_b, *norm2_w, *norm2_b, *fc1_w, *fc1_b, *fc2_w, *fc2_b;
 } mmae_block_grads;
+/* Dropout of one block (see MMAE_DROP_SITE_ATTN): attn_p on the attention probabilities, proj_p on the attention branch
+ * and mlp_p on the MLP branch, each site's mask from `seed` (a device uint64_t; NULL is allowed where all three rates are
+ * 0).  A branch element (r, c) of sample b enters the residual stream as scale[b] * keep(r, c) / (1 - p) times the branch
+ * output, and backward applies the same factor to the gradient entering the branch (its bf16 operand and bias gradient).
+ * prev_mlp_p / prev_seed are the PREVIOUS block's mlp_p / seed, for the MLP branch it hands over through x_add_bf16
+ * (forward) and dx_in_bf16 (backward), as scale_prev is its scale_mlp. */
+typedef struct mmae_block_dropout mmae_block_dropout;
+struct mmae_block_dropout {
+  float attn_p, proj_p, mlp_p;
+  const uint64_t* seed;
+  float prev_mlp_p;
+  const uint64_t* prev_seed;
+};
 
 int64_t mmae_block_saved_bytes(int B, int N, int D, int H, int hidden);
 int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hidden);
@@ -310,38 +316,20 @@ int64_t mmae_block_workspace_bytes(int B, int N, int D, int H, int hidden);
  * Stochastic depth (drop path, multimae/multimae_utils.py:105-132, 230-231): scale_attn, scale_mlp and scale_prev are
  * per-sample fp32 factors, float[B]; NULL means factor 1.  scale_prev is the PREVIOUS block's scale_mlp and needs x_add_bf16
  * (forward) and dx_in_bf16 (backward).  Backward takes the same three vectors: the gradient entering a branch is scaled,
- * the residual-path gradient is not. */
+ * the residual-path gradient is not.
+ * Dropout: `drop` (mmae_block_dropout above), the same struct forward and backward.  NULL, or all rates 0, means no
+ * dropout: the same kernels and the same results.  With attn_p > 0 attention runs the mma.sync kernels whatever
+ * mmae_attention_set_tc selects. */
 int mmae_block_forward(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16, int B, int N,
                        int D, int H, int hidden, float eps, const float* scale_attn, const float* scale_mlp,
-                       const float* scale_prev, const mmae_block_params* prm, void* saved, void* ws, void* stream);
+                       const float* scale_prev, const mmae_block_dropout* drop, const mmae_block_params* prm, void* saved,
+                       void* ws, void* stream);
 float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H, int hidden);
 int mmae_block_backward(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in, void* dx_in_bf16,
                         float* dx_in_colsum, int B, int N, int D, int H, int hidden, const float* scale_attn,
-                        const float* scale_mlp, const float* scale_prev, const mmae_block_params* prm,
-                        const mmae_block_grads* grads, const void* saved, void* ws, void* stream);
-/* The block with dropout (see MMAE_DROP_SITE_ATTN): attn_p on the attention probabilities, proj_p on the attention branch
- * and mlp_p on the MLP branch, each site's mask from `seed` (a device uint64_t; NULL is allowed where all three rates are
- * 0).  A branch element (r, c) of sample b enters the residual stream as scale[b] * keep(r, c) / (1 - p) times the branch
- * output, and backward applies the same factor to the gradient entering the branch (its bf16 operand and bias gradient).
- * prev_mlp_p / prev_seed are the PREVIOUS block's mlp_p / seed, for the MLP branch it hands over through x_add_bf16
- * (forward) and dx_in_bf16 (backward), as scale_prev is its scale_mlp.  A NULL `drop`, or all rates 0, is the plain block:
- * the same kernels and the same results. */
-typedef struct mmae_block_dropout mmae_block_dropout;
-struct mmae_block_dropout {
-  float attn_p, proj_p, mlp_p;
-  const uint64_t* seed;
-  float prev_mlp_p;
-  const uint64_t* prev_seed;
-};
-int mmae_block_forward_drop(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16, int B,
-                            int N, int D, int H, int hidden, float eps, const float* scale_attn, const float* scale_mlp,
-                            const float* scale_prev, const mmae_block_dropout* drop, const mmae_block_params* prm,
-                            void* saved, void* ws, void* stream);
-int mmae_block_backward_drop(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                             void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                             const float* scale_attn, const float* scale_mlp, const float* scale_prev,
-                             const mmae_block_dropout* drop, const mmae_block_params* prm, const mmae_block_grads* grads,
-                             const void* saved, void* ws, void* stream);
+                        const float* scale_mlp, const float* scale_prev, const mmae_block_dropout* drop,
+                        const mmae_block_params* prm, const mmae_block_grads* grads, const void* saved, void* ws,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * SpatialOutputAdapter, split at its decoder_transformer (multimae/output_adapters.py:236-282):

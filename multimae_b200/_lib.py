@@ -156,15 +156,10 @@ SIGNATURES = {
     "mmae_set_sm_budget": (c_int, [c_int]),
     "mmae_attention_set_tc": (c_int, [c_int]),
     "mmae_attention_forward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
-                                       c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
+                                       c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "mmae_attention_backward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
                                         c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
-                                        c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
-    "mmae_attention_forward_drop": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
-                                            c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
-    "mmae_attention_backward_drop": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
-                                             c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
-                                             c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
+                                        c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
     "mmae_dropout_keep_mask": (c_int, [c_void_p, c_int, c_i64, c_int, c_float, c_void_p, c_void_p]),
     "mmae_sample_masks": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.POINTER(c_int), c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),
@@ -182,19 +177,12 @@ SIGNATURES = {
     "mmae_block_saved_bytes": (c_i64, [c_int] * 5),
     "mmae_block_workspace_bytes": (c_i64, [c_int] * 5),
     "mmae_block_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                   c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams), c_void_p, c_void_p,
-                                   c_void_p]),
+                                   c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
+                                   ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
     "mmae_block_saved_x_mid": (c_void_p, [c_void_p, c_int, c_int, c_int, c_int, c_int]),
     "mmae_block_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                    c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockParams),
-                                    ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
-    "mmae_block_forward_drop": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                        c_float, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
-                                        ctypes.POINTER(BlockParams), c_void_p, c_void_p, c_void_p]),
-    "mmae_block_backward_drop": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                         c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
-                                         ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p,
-                                         c_void_p]),
+                                    c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.POINTER(BlockDropout),
+                                    ctypes.POINTER(BlockParams), ctypes.POINTER(BlockGrads), c_void_p, c_void_p, c_void_p]),
     "mmae_dechead_saved_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_workspace_bytes": (c_i64, [ctypes.POINTER(DecoderIndex), c_int, c_int, c_int]),
     "mmae_dechead_forward": (c_int, [c_void_p, c_int, ctypes.POINTER(DecoderIndex), c_int, c_int, c_float,
@@ -315,7 +303,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 
 def lib():

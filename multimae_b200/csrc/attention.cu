@@ -878,7 +878,7 @@ using namespace mmae;
 // 4 | 64 = wgmma backward (any length); the forward above 256 keys and the backward without those bits use the warp-level
 // mma.sync kernels of this file (bit 16 selected a persistent variant that has no Hopper kernel and is ignored).
 // 0 = mma.sync kernels everywhere; their backward is the fused kernel up to 256 keys, delta + dQ + dK/dV above.
-// Attention dropout (p > 0) runs the mma.sync kernels whatever the mask selects: the wgmma kernels have no dropout.
+// Attention dropout (dropout_p > 0) runs the mma.sync kernels whatever the mask selects: the wgmma kernels have no dropout.
 // Default 0 (env MMAE_ATTN_TC), from scripts/gpu_time_attention.py on one H100 80GB HBM3 at a 700 W power limit,
 // MultiMAE-B bs 128, us per call (forward mma.sync / wgmma, backward mma.sync fused / wgmma; in brackets, from the same
 // run, the forward before idle warps skipped their work and the delta + dQ + dK/dV backward the fused kernel replaced):
@@ -900,18 +900,18 @@ extern "C" int mmae_attention_set_tc(int enable) {
   return MMAE_OK;
 }
 
-// Dropout (the _drop entry points with p > 0) always runs the mma.sync kernels of this file, whatever MMAE_ATTN_TC selects:
-// the wgmma kernels have no dropout.  At p = 0 the _drop entry points are the plain ones.
-extern "C" int mmae_attention_forward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                                           int64_t ldv, void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk,
-                                           int head_dim, float scale, float dropout_p, const uint64_t* seed, void* stream) {
+// Dropout (dropout_p > 0) always runs the mma.sync kernels of this file, whatever MMAE_ATTN_TC selects: the wgmma kernels
+// have no dropout.  At dropout_p = 0 the seed is not read and the kernels are those without dropout.
+extern "C" int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                      void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
+                                      float scale, float dropout_p, const uint64_t* seed, void* stream) {
   MMAE_CHECK(q && k && v && o && B > 0 && H > 0 && Nq > 0 && Nk > 0, MMAE_ERR_ARG, "mmae_attention_forward: bad args");
   MMAE_CHECK(head_dim == 32 || head_dim == 64, MMAE_ERR_UNSUPPORTED, "mmae_attention_forward: head_dim %d (32|64)", head_dim);
   MMAE_CHECK(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && aligned16(q) && aligned16(k) &&
                  aligned16(v) && aligned16(o),
              MMAE_ERR_ARG, "mmae_attention_forward: 16-byte alignment / ld %% 8 required");
   MMAE_CHECK(dropout_p >= 0.f && dropout_p <= 1.f && (dropout_p == 0.f || seed), MMAE_ERR_ARG,
-             "mmae_attention_forward_drop: dropout p in [0, 1] and, when p > 0, a seed are required");
+             "mmae_attention_forward: dropout p in [0, 1] and, when p > 0, a seed are required");
   const DropSite drop = make_drop_site(seed, MMAE_DROP_SITE_ATTN, dropout_p);
   dim3 grid(ceil_div(Nq, ATT_ROWS), H, B);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -927,19 +927,11 @@ extern "C" int mmae_attention_forward_drop(const void* q, int64_t ldq, const voi
   return MMAE_OK;
 }
 
-extern "C" int mmae_attention_forward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                      void* o, int64_t ldo, float* lse, int B, int H, int Nq, int Nk, int head_dim,
-                                      float scale, void* stream) {
-  return mmae_attention_forward_drop(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Nq, Nk, head_dim, scale, 0.f, nullptr,
-                                     stream);
-}
-
-extern "C" int mmae_attention_backward_drop(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                                            int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
-                                            const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
-                                            int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
-                                            int head_dim, float scale, float dropout_p, const uint64_t* seed,
-                                            void* stream) {
+extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                       int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
+                                       const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
+                                       int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
+                                       int head_dim, float scale, float dropout_p, const uint64_t* seed, void* stream) {
   MMAE_CHECK(q && k && v && o && d_o && lse && delta_ws && dq && dk && dv && B > 0 && H > 0 && Nq > 0 && Nk > 0,
              MMAE_ERR_ARG, "mmae_attention_backward: bad args");
   MMAE_CHECK(head_dim == 32 || head_dim == 64, MMAE_ERR_UNSUPPORTED, "mmae_attention_backward: head_dim %d (32|64)", head_dim);
@@ -948,7 +940,7 @@ extern "C" int mmae_attention_backward_drop(const void* q, int64_t ldq, const vo
                  aligned16(d_o) && aligned16(dq) && aligned16(dk) && aligned16(dv),
              MMAE_ERR_ARG, "mmae_attention_backward: 16-byte alignment / ld %% 8 required");
   MMAE_CHECK(dropout_p >= 0.f && dropout_p <= 1.f && (dropout_p == 0.f || seed), MMAE_ERR_ARG,
-             "mmae_attention_backward_drop: dropout p in [0, 1] and, when p > 0, a seed are required");
+             "mmae_attention_backward: dropout p in [0, 1] and, when p > 0, a seed are required");
   const DropSite drop = make_drop_site(seed, MMAE_DROP_SITE_ATTN, dropout_p);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bf16 *qp = (const bf16*)q, *kp = (const bf16*)k, *vp = (const bf16*)v, *op = (const bf16*)o,
@@ -967,15 +959,6 @@ extern "C" int mmae_attention_backward_drop(const void* q, int64_t ldq, const vo
                             : (drop.seed ? launch_bwd<32, true> : launch_bwd<32, false>);
   return run(qp, ldq, kp, ldk, vp, ldv, op, ldo, dop, lddo, lse, delta_ws, (bf16*)dq, lddq, (bf16*)dk, lddk, (bf16*)dv, lddv,
              B, H, Nq, Nk, scale, drop, st);
-}
-
-extern "C" int mmae_attention_backward(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                                       int64_t ldv, const void* o, int64_t ldo, const void* d_o, int64_t lddo,
-                                       const float* lse, float* delta_ws, void* dq, int64_t lddq, void* dk,
-                                       int64_t lddk, void* dv, int64_t lddv, int B, int H, int Nq, int Nk,
-                                       int head_dim, float scale, void* stream) {
-  return mmae_attention_backward_drop(q, ldq, k, ldk, v, ldv, o, ldo, d_o, lddo, lse, delta_ws, dq, lddq, dk, lddk, dv, lddv,
-                                      B, H, Nq, Nk, head_dim, scale, 0.f, nullptr, stream);
 }
 
 extern "C" int mmae_dropout_keep_mask(const uint64_t* seed, int site, int64_t rows, int cols, float p, void* out,

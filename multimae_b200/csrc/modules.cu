@@ -372,23 +372,15 @@ int block_drop(const mmae_block_dropout* d, bool has_prev, const char* who, Bloc
 
 extern "C" int mmae_block_forward(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out, void* y_out_bf16,
                                   int B, int N, int D, int H, int hidden, float eps, const float* s_attn, const float* s_mlp,
-                                  const float* s_prev, const mmae_block_params* p, void* saved, void* ws, void* st) {
-  return mmae_block_forward_drop(x_in, x_add_bf16, x_sum, x_out, y_out_bf16, B, N, D, H, hidden, eps, s_attn, s_mlp, s_prev,
-                                 nullptr, p, saved, ws, st);
-}
-
-extern "C" int mmae_block_forward_drop(const float* x_in, const void* x_add_bf16, float* x_sum, float* x_out,
-                                       void* y_out_bf16, int B, int N, int D, int H, int hidden, float eps,
-                                       const float* s_attn, const float* s_mlp, const float* s_prev,
-                                       const mmae_block_dropout* drop, const mmae_block_params* p, void* saved, void* ws,
-                                       void* st) {
+                                  const float* s_prev, const mmae_block_dropout* drop, const mmae_block_params* p,
+                                  void* saved, void* ws, void* st) {
   const bf16* x_add = static_cast<const bf16*>(x_add_bf16);
   bf16* y_out = static_cast<bf16*>(y_out_bf16);
   MMAE_CHECK(x_in && (x_out || y_out) && (!x_add || x_sum) && p && saved && ws && B > 0 && N > 0 && H > 0 && D % H == 0,
              MMAE_ERR_ARG, "mmae_block_forward: bad args");
   MMAE_CHECK(!s_prev || x_add, MMAE_ERR_ARG, "mmae_block_forward: the previous block's scale needs x_add");
   BlockDrop dr;
-  RUN(block_drop(drop, x_add != nullptr, "mmae_block_forward_drop", &dr));
+  RUN(block_drop(drop, x_add != nullptr, "mmae_block_forward", &dr));
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(saved, B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, int64_t(3) * D * D, true, st));
@@ -408,8 +400,8 @@ extern "C" int mmae_block_forward_drop(const float* x_in, const void* x_add_bf16
     RUN(mmae_layernorm_forward(x_in, D, p->norm1_w, p->norm1_b, s.h1, D, nullptr, 0, s.mean1, s.rstd1, M, D, eps, st));
   }
   RUN(linear_bf16(s.h1, s.wqkv, p->qkv_b, s.qkv, M, 3 * D, D, st));
-  RUN(mmae_attention_forward_drop(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, s.lse, B, H, N, N, dh,
-                                  1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
+  RUN(mmae_attention_forward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, s.lse, B, H, N, N, dh,
+                             1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
   RUN(linear_bf16(s.o, s.wproj, p->proj_b, y, M, D, D, st));
   // x = x + mlp(norm2(x))                                        multimae_utils.py:231  (add fused in front of norm2)
   RUN(add_layernorm_forward_scaled(x_in, D, y, D, s_attn, N, s.x_mid, D, p->norm2_w, p->norm2_b, s.h2, D, s.mean2, s.rstd2, M,
@@ -432,28 +424,20 @@ extern "C" float* mmae_block_saved_x_mid(void* saved, int B, int N, int D, int H
 // Stochastic depth: the gradient entering a branch is s * (gradient of the residual stream), so s_mlp scales the MLP branch's
 // bf16 operand and fc2 bias gradient, s_attn the proj operand and bias gradient that LN2's backward emits, s_prev what LN1's
 // backward hands to the previous block.  The fp32 residual-path gradients (dx_mid, dx_in) are never scaled.
-extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                                   void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                                   const float* s_attn, const float* s_mlp, const float* s_prev, const mmae_block_params* p,
-                                   const mmae_block_grads* g, const void* saved, void* ws, void* st) {
-  return mmae_block_backward_drop(x_in, dx_out, dx_out_bf16, dx_in, dx_in_bf16, dx_in_colsum, B, N, D, H, hidden, s_attn,
-                                  s_mlp, s_prev, nullptr, p, g, saved, ws, st);
-}
-
 // Dropout: the same factors as forward on the gradient entering each branch - fc2's operand and bias gradient (unless the
 // next block's backward made them), proj's from LN2's backward, the previous block's from LN1's - and on dP in attention.
-extern "C" int mmae_block_backward_drop(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
-                                        void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
-                                        const float* s_attn, const float* s_mlp, const float* s_prev,
-                                        const mmae_block_dropout* drop, const mmae_block_params* p,
-                                        const mmae_block_grads* g, const void* saved, void* ws, void* st) {
+extern "C" int mmae_block_backward(const float* x_in, const float* dx_out, const void* dx_out_bf16, float* dx_in,
+                                   void* dx_in_bf16, float* dx_in_colsum, int B, int N, int D, int H, int hidden,
+                                   const float* s_attn, const float* s_mlp, const float* s_prev,
+                                   const mmae_block_dropout* drop, const mmae_block_params* p, const mmae_block_grads* g,
+                                   const void* saved, void* ws, void* st) {
   const bf16* dx_out_b = static_cast<const bf16*>(dx_out_bf16);
   bf16* dx_in_b = static_cast<bf16*>(dx_in_bf16);
   MMAE_CHECK(x_in && dx_out && dx_in && (!dx_in_b || dx_in_colsum) && p && g && saved && ws, MMAE_ERR_ARG,
              "mmae_block_backward: bad args");
   MMAE_CHECK(!s_prev || dx_in_b, MMAE_ERR_ARG, "mmae_block_backward: the previous block's scale needs dx_in_bf16");
   BlockDrop dr;
-  RUN(block_drop(drop, dx_in_b != nullptr, "mmae_block_backward_drop", &dr));
+  RUN(block_drop(drop, dx_in_b != nullptr, "mmae_block_backward", &dr));
   const int M = B * N, dh = D / H;
   BlockSaved s = block_saved(const_cast<void*>(saved), B, N, D, H, hidden);
   RUN(weight_operand(p->qkv_w, &s.wqkv, 0, false, st));
@@ -484,9 +468,9 @@ extern "C" int mmae_block_backward_drop(const float* x_in, const float* dx_out, 
   if (side) RUN(side_fork(st, 2));
   RUN(wgrad(g2, D, s.o, D, g->proj_w, M, D, D, ws_st));
   RUN(dgrad_bf16(g2, D, s.wproj, nullptr, w.d_o, M, D, D, st));
-  RUN(mmae_attention_backward_drop(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, w.d_o, D, s.lse, w.delta,
-                                   dqkv, 3 * D, dqkv + D, 3 * D, dqkv + 2 * D, 3 * D, B, H, N, N, dh,
-                                   1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
+  RUN(mmae_attention_backward(s.qkv, 3 * D, s.qkv + D, 3 * D, s.qkv + 2 * D, 3 * D, s.o, D, w.d_o, D, s.lse, w.delta,
+                              dqkv, 3 * D, dqkv + D, 3 * D, dqkv + 2 * D, 3 * D, B, H, N, N, dh,
+                              1.0f / sqrtf((float)dh), dr.attn_p, dr.seed, st));
   RUN(mmae_colsum_bf16(dqkv, 3 * D, g->qkv_b, M, 3 * D, st));
   if (side) RUN(side_fork(st, 3));
   RUN(wgrad(dqkv, 3 * D, s.h1, D, g->qkv_w, M, 3 * D, D, ws_st));
@@ -558,7 +542,7 @@ static int dechead_forward_impl(const float* enc, const float* ctx_ext, int64_t 
   RUN(linear_bf16(s.qn, s.wq, p->q_b, s.q, Mq, Dd, Dd, st));
   RUN(linear_bf16(s.cn, s.wkv, p->kv_b, s.kv, Mc, 2 * Dd, Dd, st));
   RUN(mmae_attention_forward(s.q, Dd, s.kv, 2 * Dd, s.kv + Dd, 2 * Dd, s.o, Dd, s.lse, B, H, P, Nc, dh,
-                             1.0f / sqrtf((float)dh), st));
+                             1.0f / sqrtf((float)dh), 0.f, nullptr, st));
   RUN(linear_f32(s.o, s.wproj, p->proj_b, nullptr, s.x0, Mq, Dd, Dd, st));
   // x = x + mlp(out_norm(x))                                       output_adapters.py:266
   RUN(mmae_layernorm_forward(s.x0, Dd, p->out_norm_w, p->out_norm_b, s.h, Dd, nullptr, 0, s.omean, s.orstd, Mq, Dd, eps,
@@ -613,7 +597,8 @@ static int dechead_backward_impl(int De, const mmae_decoder_index* ixp, int H, i
   RUN(wgrad(w.g, Dd, s.o, Dd, g->proj_w, Mq, Dd, Dd, st));
   RUN(dgrad_bf16(w.g, Dd, s.wproj, nullptr, w.d_o, Mq, Dd, Dd, st));
   RUN(mmae_attention_backward(s.q, Dd, s.kv, 2 * Dd, s.kv + Dd, 2 * Dd, s.o, Dd, w.d_o, Dd, s.lse, w.delta, w.dq, Dd,
-                              w.dkv, 2 * Dd, w.dkv + Dd, 2 * Dd, B, H, P, Nc, dh, 1.0f / sqrtf((float)dh), st));
+                              w.dkv, 2 * Dd, w.dkv + Dd, 2 * Dd, B, H, P, Nc, dh, 1.0f / sqrtf((float)dh), 0.f, nullptr,
+                              st));
   RUN(mmae_colsum_bf16(w.dq, Dd, g->q_b, Mq, Dd, st));
   RUN(wgrad(w.dq, Dd, s.qn, Dd, g->q_w, Mq, Dd, Dd, st));
   RUN(dgrad_bf16(w.dq, Dd, s.wq, nullptr, w.dqn, Mq, Dd, Dd, st));

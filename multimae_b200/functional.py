@@ -194,8 +194,8 @@ def block_dropouts(blocks, device, fp32=False):
 
 
 def _block_dropout_arg(drops, i, chained):
-    """ctypes BlockDropout for block i of a stack, or None when neither its own sites nor (chained) the previous block's MLP
-    site drop anything - then the plain entry points run."""
+    """ctypes BlockDropout for block i of a stack, or None (no dropout) when neither its own sites nor (chained) the
+    previous block's MLP site drop anything."""
     own = drops[i]
     prev = drops[i - 1] if chained and i > 0 else None
     if own is None and (prev is None or prev[2] == 0.0):
@@ -225,9 +225,9 @@ class BlockFunction(torch.autograd.Function):
     i's s_mlp, the factor of the MLP branch it adds in front of its first LayerNorm (forward) and of the bf16 gradient it
     hands down (backward).
 
-    Dropout: `drops` holds one block_dropouts entry per block (None: no dropout).  A block with one calls the _drop entry
-    points with its rates and seed, forward and backward; block i+1 also receives block i's mlp rate and seed, for the same
-    reason it receives s_mlp.  Blocks without any make exactly the plain calls.
+    Dropout: `drops` holds one block_dropouts entry per block (None: no dropout).  A block with one passes its rates and
+    seed to the block calls, forward and backward; block i+1 also receives block i's mlp rate and seed, for the same
+    reason it receives s_mlp.  Blocks without any pass NULL, the calls of a stack without dropout.
 
     args: x, metas (one dict per block, all of one shape; metas[0]["fp32"]: the fp32 tier of `fp32_output_adapters` - 3 x
     bf16 split GEMMs, fp32 attention / GELU - for one block), scales, drops, then the 12 BLOCK_PARAM_NAMES tensors of every
@@ -260,17 +260,12 @@ class BlockFunction(torch.autograd.Function):
                 L.check(lib.mmae_block_f32_forward(x_ptr, out.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
                                                    ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
                         "mmae_block_f32_forward")
-            elif _block_dropout_arg(drops, i, add_ptr is not None) is None:
+            else:
+                drop = _block_dropout_arg(drops, i, add_ptr is not None)
                 L.check(lib.mmae_block_forward(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
                                                None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
-                                               s_prev, ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(),
-                                               L.current_stream()), "mmae_block_forward")
-            else:
-                L.check(lib.mmae_block_forward_drop(x_ptr, add_ptr, L.ptr(x_sum), out.data_ptr() if last else None,
-                                                    None if last else y.data_ptr(), B, N, D, H, hidden, eps, s_attn, s_mlp,
-                                                    s_prev, ctypes.byref(_block_dropout_arg(drops, i, add_ptr is not None)),
-                                                    ctypes.byref(prm), saved.data_ptr(), ws.data_ptr(), L.current_stream()),
-                        "mmae_block_forward_drop")
+                                               s_prev, ctypes.byref(drop) if drop is not None else None, ctypes.byref(prm),
+                                               saved.data_ptr(), ws.data_ptr(), L.current_stream()), "mmae_block_forward")
             xs.append(x if x_sum is None else x_sum)
             saveds.append(saved)
             if not last:       # the next block's input: this block's x_mid (inside `saved`) + y
@@ -310,17 +305,13 @@ class BlockFunction(torch.autograd.Function):
                                                     s_attn, s_mlp, ctypes.byref(prm), ctypes.byref(grd),
                                                     saveds[i].data_ptr(), ws.data_ptr(), L.current_stream()),
                         "mmae_block_f32_backward")
-            elif _block_dropout_arg(ctx.drops, i, i > 0) is None:
+            else:
+                drop = _block_dropout_arg(ctx.drops, i, i > 0)
                 L.check(lib.mmae_block_backward(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(), L.ptr(g_out),
-                                                below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev, ctypes.byref(prm),
+                                                below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev,
+                                                ctypes.byref(drop) if drop is not None else None, ctypes.byref(prm),
                                                 ctypes.byref(grd), saveds[i].data_ptr(), ws.data_ptr(),
                                                 L.current_stream()), "mmae_block_backward")
-            else:
-                L.check(lib.mmae_block_backward_drop(xs[i].data_ptr(), d.data_ptr(), L.ptr(g_in), dx.data_ptr(),
-                                                     L.ptr(g_out), below_bias, B, N, D, H, hidden, s_attn, s_mlp, s_prev,
-                                                     ctypes.byref(_block_dropout_arg(ctx.drops, i, i > 0)),
-                                                     ctypes.byref(prm), ctypes.byref(grd), saveds[i].data_ptr(),
-                                                     ws.data_ptr(), L.current_stream()), "mmae_block_backward_drop")
             if metas[i].get("on_grads_ready") is not None:
                 metas[i]["on_grads_ready"](names)       # fc2.bias of block i is complete: its column sums came from block i+1
             grads[i * P:(i + 1) * P] = _ret_grads(arena, names, blk)

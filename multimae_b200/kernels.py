@@ -116,7 +116,7 @@ def attention_fwd(q, k, v, B, H, Nq, Nk, dh, scale, out=None):
     lse = torch.empty((B, H, Nq), dtype=torch.float32, device=q.device)
     L.check(L.lib().mmae_attention_forward(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(),
                                            v.stride(0), out.data_ptr(), out.stride(0), lse.data_ptr(), B, H, Nq, Nk,
-                                           dh, scale, L.current_stream()), "mmae_attention_forward")
+                                           dh, scale, 0.0, None, L.current_stream()), "mmae_attention_forward")
     return out, lse
 
 
@@ -126,7 +126,7 @@ def attention_bwd(q, k, v, o, do, lse, dq, dk, dv, B, H, Nq, Nk, dh, scale):
                                             v.stride(0), o.data_ptr(), o.stride(0), do.data_ptr(), do.stride(0),
                                             lse.data_ptr(), delta.data_ptr(), dq.data_ptr(), dq.stride(0),
                                             dk.data_ptr(), dk.stride(0), dv.data_ptr(), dv.stride(0), B, H, Nq, Nk, dh,
-                                            scale, L.current_stream()), "mmae_attention_backward")
+                                            scale, 0.0, None, L.current_stream()), "mmae_attention_backward")
 
 
 

@@ -6,7 +6,7 @@
    drop_path_rate 0.1, autocast, loss scaling, torch.optim.AdamW.  drop = attn_drop = 0 against 0.1 (the rates are set on
    the same model's nn.Dropout modules), alternating in one process after warm-up; ms/step from CUDA events.
 2. Per call, the attention forward and backward at 197 x 197 and 577 x 577 keys, dh 64, 12 heads, batch 128, without and
-   with dropout 0.1 (mmae_attention_*_drop).
+   with dropout 0.1 (the dropout_p argument of mmae_attention_forward / _backward).
 
 Prints one JSON line per figure with the GPU name and power limit."""
 import argparse
@@ -93,11 +93,11 @@ def main():
         st = L.current_stream()
 
         def fwd(p):
-            return lambda: L.check(lib.mmae_attention_forward_drop(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, lse.data_ptr(),
-                                                                   B, H, N, N, dh, dh ** -0.5, p, seed.data_ptr(), st))
+            return lambda: L.check(lib.mmae_attention_forward(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, lse.data_ptr(),
+                                                              B, H, N, N, dh, dh ** -0.5, p, seed.data_ptr(), st))
 
         def bwd(p):
-            return lambda: L.check(lib.mmae_attention_backward_drop(
+            return lambda: L.check(lib.mmae_attention_backward(
                 q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, d_o.data_ptr(), D, lse.data_ptr(), delta.data_ptr(),
                 dqkv.data_ptr(), 3 * D, dqkv[:, D:].data_ptr(), 3 * D, dqkv[:, 2 * D:].data_ptr(), 3 * D, B, H, N, N, dh,
                 dh ** -0.5, p, seed.data_ptr(), st))

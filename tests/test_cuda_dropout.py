@@ -1,4 +1,4 @@
-"""GPU: dropout inside the fused block and attention kernels (the _drop entry points and mmae_dropout_keep_mask).
+"""GPU: dropout inside the fused block and attention kernels (their dropout arguments and mmae_dropout_keep_mask).
 
 The masks of a run are materialised from the seeds it drew (functional.dropout_seeds, spied on) by mmae_dropout_keep_mask,
 which uses the kernels' own generator, and handed to the fp32 oracle with explicit masks (tests/dropout_oracle.py).
@@ -133,20 +133,20 @@ def _attn_call(qkv, d_o, B, H, N, dh, p, seed):
     dqkv = torch.empty_like(qkv)
     sc, st = dh ** -0.5, L.current_stream()
     q, k, v = qkv.data_ptr(), qkv[:, D:].data_ptr(), qkv[:, 2 * D:].data_ptr()
-    L.check(lib.mmae_attention_forward_drop(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, lse.data_ptr(), B, H, N, N, dh, sc,
-                                            p, L.ptr(seed), st), "mmae_attention_forward_drop")
-    L.check(lib.mmae_attention_backward_drop(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, d_o.data_ptr(), D, lse.data_ptr(),
-                                             delta.data_ptr(), dqkv.data_ptr(), 3 * D, dqkv[:, D:].data_ptr(), 3 * D,
-                                             dqkv[:, 2 * D:].data_ptr(), 3 * D, B, H, N, N, dh, sc, p, L.ptr(seed), st),
-            "mmae_attention_backward_drop")
+    L.check(lib.mmae_attention_forward(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, lse.data_ptr(), B, H, N, N, dh, sc,
+                                       p, L.ptr(seed), st), "mmae_attention_forward")
+    L.check(lib.mmae_attention_backward(q, 3 * D, k, 3 * D, v, 3 * D, o.data_ptr(), D, d_o.data_ptr(), D, lse.data_ptr(),
+                                        delta.data_ptr(), dqkv.data_ptr(), 3 * D, dqkv[:, D:].data_ptr(), 3 * D,
+                                        dqkv[:, 2 * D:].data_ptr(), 3 * D, B, H, N, N, dh, sc, p, L.ptr(seed), st),
+            "mmae_attention_backward")
     torch.cuda.synchronize()
     return o, dqkv
 
 
 @pytest.mark.parametrize("N", [197, 577])
 @pytest.mark.parametrize("dh", [32, 64])
-def test_attention_entry_points_against_oracle_and_tc_switch(dev, N, dh):
-    """mmae_attention_*_drop against the fp32 attention with the keep mask; with the wgmma kernels selected
+def test_attention_dropout_against_oracle_and_tc_switch(dev, N, dh):
+    """mmae_attention_forward / _backward with dropout against the fp32 attention with the keep mask; with the wgmma kernels selected
     (MMAE_ATTN_TC bits) the results are bit for bit those of the mma.sync kernels: dropout always runs on the latter."""
     B, H, p = 2, 2, 0.3
     qkv, d_o = _attn_inputs(dev, B, H, N, dh)

@@ -2,7 +2,8 @@
 
 1. The oracle with explicit dropout masks (tests/dropout_oracle.py), given the masks recorded from the live reference
    (tests/golden/make_golden_dropout.py), reproduces the reference's encoder tokens and every parameter gradient.
-2. The host layer against a stub of the C library: which entry points run, with which rates and seed pointers."""
+2. The host layer against a stub of the C library: which dropout struct each block call gets, with which rates and seed
+   pointers."""
 import ctypes
 
 import pytest
@@ -15,8 +16,7 @@ from multimae_b200 import functional as Fn
 from oracle import multimae_oracle as O
 from test_drop_path_host import _Rec
 
-DROP_CALLS = ("mmae_block_forward_drop", "mmae_block_backward_drop")
-PLAIN_CALLS = ("mmae_block_forward", "mmae_block_backward")
+BLOCK_CALLS = ("mmae_block_forward", "mmae_block_backward")
 
 
 def _multivit_oracle(c):
@@ -97,8 +97,8 @@ def _drop_struct(args):
 
 
 @pytest.mark.parametrize("chain", [True, False])
-def test_drop_entry_points_carry_rates_and_seeds(rec, monkeypatch, chain):
-    """Rates > 0 in training: every block calls the _drop entry points with its modules' rates and its seed, forward and
+def test_block_calls_carry_dropout_rates_and_seeds(rec, monkeypatch, chain):
+    """Rates > 0 in training: every block call carries a dropout struct with its modules' rates and its seed, forward and
     backward with the same seed pointer; chained, block i+1 also gets block i's mlp rate and seed as prev_*."""
     monkeypatch.setattr(Fn, "BLOCK_CHAIN", chain)
     blocks = _stack(drop=0.25, attn_drop=0.4).train()
@@ -106,38 +106,38 @@ def test_drop_entry_points_carry_rates_and_seeds(rec, monkeypatch, chain):
     seeds = _pinned_seeds(monkeypatch)
     x = torch.randn(2, 5, 128, requires_grad=True)
     Fn.block_stack(blocks, x).sum().backward()
-    assert not [n for n in rec.names() if n in PLAIN_CALLS]
-    fwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward_drop"]
-    bwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_backward_drop"][::-1]     # issued for blocks 2..0
+    assert all(a[14] is not None for n, a in rec.calls if n in BLOCK_CALLS)
+    fwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward"]
+    bwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_backward"][::-1]     # issued for blocks 2..0
     assert len(fwd) == len(bwd) == 3 and len(seeds) == 3
     for i, b in enumerate(blocks):
         own = seeds[id(b)].data_ptr()
         prev = (0.25, seeds[id(blocks[i - 1])].data_ptr()) if chain and i > 0 else (0.0, None)
         want = (0.4, 0.125 if i == 1 else 0.25, 0.25, own) + prev
         assert fwd[i] == pytest.approx(want) and bwd[i] == fwd[i], (i, fwd[i], bwd[i], want)
-    # the scale arguments and the rest of each call are those of a plain call
+    # the scale arguments and the rest of each call are those of a call without dropout
     for n, a in rec.calls:
-        if n in DROP_CALLS:
+        if n in BLOCK_CALLS:
             assert a[11:14] == (None, None, None)
 
 
-def test_prev_only_block_uses_drop_entry_point(rec, monkeypatch):
-    """A block without dropout of its own after one with mlp dropout still calls the _drop entry points (chained): it
-    applies the previous block's MLP mask to the branch it adds in front of its first LayerNorm."""
+def test_prev_only_block_gets_dropout_struct(rec, monkeypatch):
+    """A block without dropout of its own after one with mlp dropout still gets a dropout struct (chained): it applies the
+    previous block's MLP mask to the branch it adds in front of its first LayerNorm."""
     monkeypatch.setattr(Fn, "BLOCK_CHAIN", True)
     blocks = _stack(n=2).train()
     blocks[0].mlp.drop.p = 0.5
     seeds = _pinned_seeds(monkeypatch)
     Fn.block_stack(blocks, torch.randn(2, 5, 128, requires_grad=True)).sum().backward()
-    fwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward_drop"]
+    fwd = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward"]
     assert len(fwd) == 2 and list(seeds) == [id(blocks[0])]
     assert fwd[0] == (0.0, 0.0, 0.5, seeds[id(blocks[0])].data_ptr(), 0.0, None)
     assert fwd[1] == (0.0, 0.0, 0.0, None, 0.5, seeds[id(blocks[0])].data_ptr())
 
 
 def test_eval_no_grad_and_zero_rates_make_todays_calls(rec, monkeypatch):
-    """eval() (with or without no_grad) or all rates 0: the plain entry points with the same arguments as a stack built
-    without dropout; nothing is drawn."""
+    """eval() (with or without no_grad) or all rates 0: the block calls get a NULL dropout struct and the same arguments as
+    a stack built without dropout; nothing is drawn."""
     monkeypatch.setattr(Fn, "BLOCK_CHAIN", True)
     x = torch.randn(2, 5, 128)
 
@@ -151,26 +151,27 @@ def test_eval_no_grad_and_zero_rates_make_todays_calls(rec, monkeypatch):
             with torch.no_grad():
                 Fn.block_stack(blocks, xi)
         assert torch.equal(torch.get_rng_state(), state)
+        assert all(a[14] is None for n, a in rec.calls if n in BLOCK_CALLS)
         return [(n, tuple(a[6:14])) for n, a in rec.calls]
 
     ref_grad, ref_nograd = calls(_stack().train(), True), calls(_stack().eval(), False)
     assert calls(_stack(drop=0.3, attn_drop=0.3).eval(), True) == ref_grad
     assert calls(_stack(drop=0.3, attn_drop=0.3).eval(), False) == ref_nograd
     assert calls(_stack(drop=0.0, attn_drop=0.0).train(), True) == ref_grad
-    assert not [n for n, _ in rec.calls if n in DROP_CALLS]
     from multimae_b200.multimae_utils import Block
     rec.calls.clear()
     Block(128, 2, qkv_bias=True, drop=0.2, attn_drop=0.2).eval()(x.clone().requires_grad_(True)).sum().backward()
     assert rec.names().count("mmae_block_forward") == 1 and rec.names().count("mmae_block_backward") == 1
+    assert all(a[14] is None for n, a in rec.calls if n in BLOCK_CALLS)
 
 
-def test_stand_alone_block_draws_its_seed(rec):
+def test_stand_alone_block_draws_its_dropout_seed(rec):
     """A stand-alone Block with dropout in training draws one seed and gives the same pointer to forward and backward."""
     from multimae_b200.multimae_utils import Block
     b = Block(128, 2, qkv_bias=True, drop=0.1, attn_drop=0.2).train()
     b(torch.randn(3, 5, 128, requires_grad=True)).sum().backward()
-    (f,) = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward_drop"]
-    (g,) = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_backward_drop"]
+    (f,) = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_forward"]
+    (g,) = [_drop_struct(a) for n, a in rec.calls if n == "mmae_block_backward"]
     assert f == g and f[:3] == pytest.approx((0.2, 0.1, 0.1)) and f[3] is not None and f[4:] == (0.0, None)
 
 

@@ -163,7 +163,7 @@ def test_ctypes_structs_match_the_c_header(tmp_path):
     assert L.ABI_VERSION == int(re.search(r"#define MMAE_ABI_VERSION (\d+)", open(header).read()).group(1))
 
 
-def test_c_abi_rejects_bad_arguments_with_messages():
+def test_c_abi_rejects_bad_arguments_and_dropout_with_messages():
     """Error behaviour of the C ABI (no GPU needed: every check fires before the first CUDA call): a non-zero code,
     the message behind mmae_last_error(), and the Python stub's exception (MmaeError, a RuntimeError like the reference's
     assertion failures, e.g. multimae/input_adapters.py:105-106)."""
@@ -180,8 +180,8 @@ def test_c_abi_rejects_bad_arguments_with_messages():
         (lambda: lib.mmae_standardize_depth_set_variant(3), ARG, b"1 or 2"),
         (lambda: lib.mmae_layernorm_forward(16, 100, 16, 16, 16, 100, None, 0, 16, 16, 4, 100, 1e-6, None), UNSUPPORTED,
          b"multiple of 128"),
-        (lambda: lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, None, 1, 1, 8, 8, 48, 0.1, None), UNSUPPORTED,
-         b"head_dim 48"),
+        (lambda: lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, None, 1, 1, 8, 8, 48, 0.1, 0.0, None, None),
+         UNSUPPORTED, b"head_dim 48"),
         (lambda: lib.mmae_masked_loss_forward(5, 0, 0.0, 16, 16, None, 1, 3, 32, 32, 16, 16, 16, None), UNSUPPORTED, b"kind"),
     ]
     # round-2 entry points: shared context projection, *_ctx heads, blocks with hand-offs and stochastic depth
@@ -198,18 +198,44 @@ def test_c_abi_rejects_bad_arguments_with_messages():
         (lambda: lib.mmae_dechead_forward_ctx(None, 1024, None, 8, 1024, 1e-6, None, None, None, None, None), ARG, b"bad args"),
         (lambda: lib.mmae_dechead_backward_ctx(None, 8, 1024, None, None, None, None, 1024, None, None, None), ARG, b"bad args"),
         # x_add without a buffer for the sum; neither x_out nor y_out; a bf16 gradient copy without its column-sum target
-        (lambda: lib.mmae_block_forward(16, 16, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None, ctypes.byref(bp),
-                                        16, 16, None), ARG, b"mmae_block_forward"),
-        (lambda: lib.mmae_block_forward(16, None, None, None, None, 2, 8, 128, 2, 512, 1e-6, None, None, None,
+        (lambda: lib.mmae_block_forward(16, 16, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None, None,
                                         ctypes.byref(bp), 16, 16, None), ARG, b"mmae_block_forward"),
-        (lambda: lib.mmae_block_backward(16, 16, None, 16, 16, None, 2, 8, 128, 2, 512, None, None, None, ctypes.byref(bp),
-                                         ctypes.byref(bg), 16, 16, None), ARG, b"mmae_block_backward"),
+        (lambda: lib.mmae_block_forward(16, None, None, None, None, 2, 8, 128, 2, 512, 1e-6, None, None, None, None,
+                                        ctypes.byref(bp), 16, 16, None), ARG, b"mmae_block_forward"),
+        (lambda: lib.mmae_block_backward(16, 16, None, 16, 16, None, 2, 8, 128, 2, 512, None, None, None, None,
+                                         ctypes.byref(bp), ctypes.byref(bg), 16, 16, None), ARG, b"mmae_block_backward"),
         # the previous block's scale without the hand-off it scales
-        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, 16, ctypes.byref(bp),
-                                        16, 16, None), ARG, b"mmae_block_forward: the previous block's scale needs x_add"),
-        (lambda: lib.mmae_block_backward(16, 16, None, 16, None, None, 2, 8, 128, 2, 512, None, None, 16, ctypes.byref(bp),
-                                         ctypes.byref(bg), 16, 16, None), ARG,
+        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, 16, None,
+                                        ctypes.byref(bp), 16, 16, None), ARG,
+         b"mmae_block_forward: the previous block's scale needs x_add"),
+        (lambda: lib.mmae_block_backward(16, 16, None, 16, None, None, 2, 8, 128, 2, 512, None, None, 16, None,
+                                         ctypes.byref(bp), ctypes.byref(bg), 16, 16, None), ARG,
          b"mmae_block_backward: the previous block's scale needs dx_in_bf16"),
+    ]
+    # dropout: a rate outside [0, 1]; a rate > 0 without a seed; the previous block's rate without the hand-off it applies
+    # to; attention dropout without a seed
+    bad_rate, no_seed, prev_only = L.BlockDropout(), L.BlockDropout(), L.BlockDropout()
+    bad_rate.mlp_p, bad_rate.seed = 1.5, 16
+    no_seed.attn_p = 0.1
+    prev_only.prev_mlp_p, prev_only.prev_seed = 0.1, 16
+    cases += [
+        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None,
+                                        ctypes.byref(bad_rate), ctypes.byref(bp), 16, 16, None), ARG,
+         b"mmae_block_forward: dropout rates must lie in [0, 1]"),
+        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None,
+                                        ctypes.byref(no_seed), ctypes.byref(bp), 16, 16, None), ARG,
+         b"mmae_block_forward: dropout needs a seed"),
+        (lambda: lib.mmae_block_forward(16, None, None, 16, None, 2, 8, 128, 2, 512, 1e-6, None, None, None,
+                                        ctypes.byref(prev_only), ctypes.byref(bp), 16, 16, None), ARG,
+         b"mmae_block_forward: the previous block's dropout needs its seed and the hand-off"),
+        (lambda: lib.mmae_block_backward(16, 16, None, 16, None, None, 2, 8, 128, 2, 512, None, None, None,
+                                         ctypes.byref(prev_only), ctypes.byref(bp), ctypes.byref(bg), 16, 16, None), ARG,
+         b"mmae_block_backward: the previous block's dropout needs its seed and the hand-off"),
+        (lambda: lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, 16, 1, 1, 8, 8, 64, 0.1, 0.1, None, None), ARG,
+         b"mmae_attention_forward: dropout p in [0, 1] and, when p > 0, a seed are required"),
+        (lambda: lib.mmae_attention_backward(16, 64, 16, 64, 16, 64, 16, 64, 16, 64, 16, 16, 16, 64, 16, 64, 16, 64,
+                                             1, 1, 8, 8, 64, 0.1, 0.1, None, None), ARG,
+         b"mmae_attention_backward: dropout p in [0, 1] and, when p > 0, a seed are required"),
     ]
     assert lib.mmae_block_saved_x_mid(None, 2, 8, 128, 2, 512) is None
     # mmae_last_error() holds the message of the most recent failure: read it right after each call

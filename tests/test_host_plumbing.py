@@ -219,7 +219,7 @@ def test_train_step_eager_and_sampling_options(stub):
     assert a.shape == (64, 3) and bool(((a > 0.5).sum(1) >= 1).all())      # never the all-zero task subset (:150)
 
 
-def test_block_stack_hand_off_arguments(monkeypatch):
+def test_block_stack_hand_off_call_arguments(monkeypatch):
     """BlockFunction wires consecutive blocks through raw pointers: block i+1 must receive block i's x_mid (inside
     block i's `saved` buffer) as x_in and the shared MLP-output buffer as x_add; only the last block writes x_out; in backward
     block i+1 writes bf16(dx) into the buffer block i then reads, and its column sums into block i's fc2 bias gradient."""
@@ -256,15 +256,15 @@ def test_block_stack_hand_off_arguments(monkeypatch):
     fwd = [a for n, a in calls if n == "mmae_block_forward"]
     mids = [a for n, a in calls if n == "mmae_block_saved_x_mid"]
     assert len(fwd) == 4 and len(mids) == 3
-    # args: x_in, x_add, x_sum, x_out, y_out, ..., saved (index 15)
+    # args: x_in, x_add, x_sum, x_out, y_out, ..., saved (index 16)
     assert fwd[0][0] == x.data_ptr() and fwd[0][1] is None and fwd[0][2] is None        # first block: plain input
     y_buf = fwd[0][4]
     assert y_buf is not None and fwd[0][3] is None                                       # not the last: y_out, no x_out
     for i in (1, 2, 3):
-        assert fwd[i][0] == fwd[i - 1][15] + 64                  # x_in = x_mid of the block before (inside ITS saved buffer)
+        assert fwd[i][0] == fwd[i - 1][16] + 64                  # x_in = x_mid of the block before (inside ITS saved buffer)
         assert fwd[i][1] == y_buf and fwd[i][2] is not None      # x_add = the MLP branch output; the sum is materialised
     assert fwd[3][3] == out.data_ptr() and fwd[3][4] is None    # the last block adds by itself
-    assert len({a[15] for a in fwd}) == 4 and len({a[2] for a in fwd[1:]}) == 3          # own saved / x_sum buffers
+    assert len({a[16] for a in fwd}) == 4 and len({a[2] for a in fwd[1:]}) == 3          # own saved / x_sum buffers
     out.sum().backward()
     bwd = [a for n, a in calls if n == "mmae_block_backward"]
     assert len(bwd) == 4
