@@ -123,7 +123,8 @@ int mmae_transpose_bf16(const void* src, int64_t ld_src, void* dst, int64_t ld_d
 
 /* ------------------------------------------------------------------------------------------------
  * LayerNorm (fp32 statistics; eps given).  nn.LayerNorm(eps=1e-6): multimae/multimae_utils.py:222,225 and
- * multimae/output_adapters.py:120-122.  D must be a multiple of 128, <= 1024.
+ * multimae/output_adapters.py:120-122.  D must be a multiple of 32, <= 1024; the fused-add form and the bf16 copy /
+ * column sums of the _ex backward need a multiple of 128 (other widths return MMAE_ERR_UNSUPPORTED).
  *   forward : y = (x-mean)*rstd*gamma+beta, written as bf16 (GEMM operand) and/or fp32; saves mean/rstd.
  *   backward: dx = dx_resid(optional) + LN'(dy); dgamma/dbeta are ACCUMULATED (+=) with fp32 atomics.
  * ---------------------------------------------------------------------------------------------- */
@@ -439,7 +440,7 @@ int mmae_clshead_backward(const float* dout, int B, int N, int D, int C, int mea
  * multimae/output_adapter_utils.py:19-57), split like SpatialOutputAdapter: proj -> block x depth -> tail.
  * The feature map (Hf, Wf) = (nh*s, nw*s), s = sqrt(preds_per_patch), is held as the fp32 [P, C] view of the proj_dec output
  * (P = B*nh*nw*s*s): row (b*n + t)*s*s + a*s + c' is pixel ((t / nw)*s + a, (t % nw)*s + c') of sample b, n = nh*nw.
- * C must be a multiple of 128, at most 1024.  GEMMs take bf16 operands (registered weight mirrors when there are any) and
+ * C must be a multiple of 32, at most 1024.  GEMMs take bf16 operands (registered weight mirrors when there are any) and
  * accumulate in fp32.  Backward WRITES the activation gradient and ACCUMULATES (+=) the parameter gradients; the activation
  * gradients and the depthwise-conv parameter gradients are computed without atomics (bitwise repeatable).  `saved` (from
  * forward to backward) and `ws` are sized by the *_bytes queries.

@@ -1,5 +1,6 @@
 // Semantic-segmentation head of fine-tuning: ConvNeXtAdapter.forward (multimae/output_adapters.py:481-573, ConvNeXtBlock in
-// multimae/output_adapter_utils.py:19-57):
+// multimae/output_adapter_utils.py:19-57); also the depth head of run_finetuning_depth.py --output_adapter convnext
+// (preds_per_patch 64: C = 96 channels per pixel, s = 8, K = 1):
 //   x = proj_dec(cat_t encoder_tokens[:, task t])                     Linear [B, n, D*T] -> [B, n, E]
 //   x = rearrange(x, "b (nh nw) (ph pw c) -> b c (nh ph) (nw pw)")    s = ph = pw = sqrt(preds_per_patch), C = E / (s*s)
 //   x = x + pwconv2(GELU(pwconv1(LN(dwconv7x7(x)))))  x depth           depthwise 7x7 (pad 3, bias), LN over channels
@@ -419,8 +420,8 @@ TailWs tl_ws(void* base, int64_t P, int C, int K) {
 
 int check_geo(const char* what, int B, int nh, int nw, int s, int C) {
   MMAE_CHECK(B > 0 && nh > 0 && nw > 0 && s > 0, MMAE_ERR_ARG, "%s: bad shape B=%d nh=%d nw=%d s=%d", what, B, nh, nw, s);
-  MMAE_CHECK(C % 128 == 0 && C > 0 && C <= 1024, MMAE_ERR_UNSUPPORTED,
-             "%s: C=%d channels per pixel must be a multiple of 128, at most 1024 (the LayerNorm kernels)", what, C);
+  MMAE_CHECK(C % 32 == 0 && C > 0 && C <= 1024, MMAE_ERR_UNSUPPORTED,
+             "%s: C=%d channels per pixel must be a multiple of 32, at most 1024 (the LayerNorm kernels)", what, C);
   MMAE_CHECK(int64_t(B) * nh * nw * s * s < (int64_t(1) << 31), MMAE_ERR_UNSUPPORTED, "%s: too many pixels", what);
   return MMAE_OK;
 }

@@ -245,10 +245,190 @@ __global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_kernel(const void* __res
   }
 }
 
+// ------------------------------------------------------------------------------------------------ narrow rows
+// D = NW * 32 with D % 128 != 0 (the ConvNeXt head of depth fine-tuning: 6144 / 64 = 96 channels per pixel).  Lane l holds
+// elements l + 32 i, so every warp-wide load or store is one coalesced 128-byte (fp32) / 64-byte (bf16) run of the row.
+// Same arithmetic as the float4 kernels (two-pass statistics in fp32, the same backward formula and partial-row layout);
+// only the plain forms: no fused add, drop path or dropout in front of the forward, no bf16 copy / column sums of dx.
+// ptxas (sm_90a, 256 threads, no spills): fwd 18 (NW = 1) .. 48 (NW = 31) registers, 28 at D = 96; bwd 32 .. 252 (f32 dy) /
+// 255 (bf16 dy), 40 at D = 96.
+template <int NW>
+__global__ void __launch_bounds__(LN_WARPS * 32) ln_fwd_narrow_kernel(const float* __restrict__ x, int64_t ldx,
+                                                                      const float* __restrict__ gamma,
+                                                                      const float* __restrict__ beta,
+                                                                      bf16* __restrict__ y_bf16, int64_t ldy,
+                                                                      float* __restrict__ y_f32, int64_t ldyf,
+                                                                      float* __restrict__ mean_out,
+                                                                      float* __restrict__ rstd_out, int M, float eps) {
+  pdl_prologue();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int row = blockIdx.x * LN_WARPS + warp;
+  if (row >= M) return;
+  constexpr int D = NW * 32;
+  const float* xr = x + int64_t(row) * ldx;
+  float v[NW];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < NW; ++i) {
+    v[i] = __ldg(xr + i * 32 + lane);
+    s += v[i];
+  }
+  const float mean = warp_sum(s) * (1.0f / D);
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < NW; ++i) {
+    const float a = v[i] - mean;
+    q += a * a;
+  }
+  const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + eps);
+  if (lane == 0) {
+    if (mean_out) mean_out[row] = mean;
+    if (rstd_out) rstd_out[row] = rstd;
+  }
+#pragma unroll
+  for (int i = 0; i < NW; ++i) {
+    const int c = i * 32 + lane;
+    const float o = (v[i] - mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
+    if (y_bf16) y_bf16[int64_t(row) * ldy + c] = __float2bfloat16_rn(o);
+    if (y_f32) y_f32[int64_t(row) * ldyf + c] = o;
+  }
+}
+
+template <int NW, bool DY_BF16>
+__device__ __forceinline__ void ln_narrow_load(float (&xv)[NW], float (&dv)[NW], const void* dy_, int64_t lddy,
+                                               const float* x, int64_t ldx, int row, int lane) {
+#pragma unroll
+  for (int i = 0; i < NW; ++i) {
+    const int c = i * 32 + lane;
+    xv[i] = __ldg(x + int64_t(row) * ldx + c);
+    if constexpr (DY_BF16)
+      dv[i] = __bfloat162float(reinterpret_cast<const bf16*>(dy_)[int64_t(row) * lddy + c]);
+    else
+      dv[i] = __ldg(reinterpret_cast<const float*>(dy_) + int64_t(row) * lddy + c);
+  }
+}
+
+// Persistent like ln_bwd_kernel (one wave, warps stride over the rows; up to D = 512 the next row's loads are issued
+// before the current row's reductions); the block's dgamma / dbeta go to its row of [dgamma | dbeta | -] partial sums
+// for colred_finalize.
+template <int NW, bool DY_BF16>
+__global__ void __launch_bounds__(LN_WARPS * 32) ln_bwd_narrow_kernel(const void* __restrict__ dy_, int64_t lddy,
+                                                                      const float* __restrict__ x, int64_t ldx,
+                                                                      const float* __restrict__ mean_in,
+                                                                      const float* __restrict__ rstd_in,
+                                                                      const float* __restrict__ gamma,
+                                                                      const float* __restrict__ dx_resid, int64_t ldr,
+                                                                      float* __restrict__ dx, int64_t lddx,
+                                                                      float* __restrict__ partial, int M) {
+  pdl_prologue();
+  constexpr int D = NW * 32;
+  __shared__ float red[LN_WARPS][32];
+  __shared__ float sgamma[D];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < D; i += LN_WARPS * 32) sgamma[i] = __ldg(gamma + i);
+  __syncthreads();
+  float dg[NW], db[NW];
+#pragma unroll
+  for (int i = 0; i < NW; ++i) dg[i] = db[i] = 0.f;
+  const int row_stride = gridDim.x * LN_WARPS;
+  int row = blockIdx.x * LN_WARPS + warp;
+  // above 16 x 32 columns a second row in registers would spill, and one row already keeps 2 x NW loads in flight
+  constexpr bool PREFETCH = NW <= 16;
+  float xc[NW], dc[NW], xn[NW], dn[NW];
+  float mean = 0.f, rstd = 0.f, mean_n = 0.f, rstd_n = 0.f;
+  if (PREFETCH && row < M) {
+    ln_narrow_load<NW, DY_BF16>(xc, dc, dy_, lddy, x, ldx, row, lane);
+    mean = __ldg(mean_in + row);
+    rstd = __ldg(rstd_in + row);
+  }
+  for (; row < M; row += row_stride) {
+    const int row_n = row + row_stride;
+    if constexpr (PREFETCH) {
+      if (row_n < M) {
+        ln_narrow_load<NW, DY_BF16>(xn, dn, dy_, lddy, x, ldx, row_n, lane);
+        mean_n = __ldg(mean_in + row_n);
+        rstd_n = __ldg(rstd_in + row_n);
+      }
+    } else {
+      ln_narrow_load<NW, DY_BF16>(xc, dc, dy_, lddy, x, ldx, row, lane);
+      mean = __ldg(mean_in + row);
+      rstd = __ldg(rstd_in + row);
+    }
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < NW; ++i) {
+      const float xh = (xc[i] - mean) * rstd;
+      const float g = dc[i] * sgamma[i * 32 + lane];
+      s1 += g;
+      s2 += g * xh;
+      dg[i] += dc[i] * xh;
+      db[i] += dc[i];
+    }
+    const float c1 = warp_sum(s1) * (1.0f / D), c2 = warp_sum(s2) * (1.0f / D);
+#pragma unroll
+    for (int i = 0; i < NW; ++i) {
+      const int c = i * 32 + lane;
+      const float xh = (xc[i] - mean) * rstd;
+      float o = rstd * (dc[i] * sgamma[c] - c1 - xh * c2);
+      if (dx_resid) o += __ldg(dx_resid + int64_t(row) * ldr + c);
+      dx[int64_t(row) * lddx + c] = o;
+    }
+    if constexpr (PREFETCH) {
+#pragma unroll
+      for (int i = 0; i < NW; ++i) {
+        xc[i] = xn[i];
+        dc[i] = dn[i];
+      }
+      mean = mean_n;
+      rstd = rstd_n;
+    }
+  }
+#pragma unroll
+  for (int pass = 0; pass < 2; ++pass) {
+    float* dst = partial + (int64_t(blockIdx.x) * 3 + pass) * D;
+#pragma unroll
+    for (int i = 0; i < NW; ++i) {
+      __syncthreads();
+      red[warp][lane] = pass == 0 ? dg[i] : db[i];
+      __syncthreads();
+      if (warp == 0) {
+        float a = red[0][lane];
+#pragma unroll
+        for (int w = 1; w < LN_WARPS; ++w) a += red[w][lane];
+        dst[i * 32 + lane] = a;
+      }
+    }
+  }
+}
+
+// the widths the narrow kernels are instantiated for: every multiple of 32 up to 1024 that is not a multiple of 128
+#define LN_NARROW_WIDTHS(X)                                                                                             \
+  X(1) X(2) X(3) X(5) X(6) X(7) X(9) X(10) X(11) X(13) X(14) X(15) X(17) X(18) X(19) X(21) X(22) X(23) X(25) X(26) X(27) \
+  X(29) X(30) X(31)
+
 }  // namespace
 }  // namespace mmae
 
 using namespace mmae;
+
+static int ln_forward_narrow(const float* x, int64_t ldx, const float* gamma, const float* beta, bf16* y_bf16, int64_t ldy,
+                             float* y_f32, int64_t ldyf, float* mean, float* rstd, int M, int D, float eps, void* stream) {
+  dim3 grid(ceil_div(M, LN_WARPS)), block(LN_WARPS * 32);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+#define LNN_CASE(NW)                                                                                                  \
+  case NW:                                                                                                            \
+    launch_k(ln_fwd_narrow_kernel<NW>, grid, block, 0, st, x, ldx, gamma, beta, y_bf16, ldy, y_f32, ldyf, mean, rstd, M, \
+             eps);                                                                                                    \
+    break;
+  switch (D / 32) {
+    LN_NARROW_WIDTHS(LNN_CASE)
+    default: MMAE_CHECK(false, MMAE_ERR_UNSUPPORTED, "mmae_layernorm_forward: unsupported D=%d", D);
+  }
+#undef LNN_CASE
+  count_launch();
+  MMAE_LAUNCH_OK();
+  return MMAE_OK;
+}
 
 static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int64_t ldadd, float* x_sum, int64_t ldsum,
                            const float* gamma, const float* beta, void* y_bf16, int64_t ldy, float* y_f32, int64_t ldyf,
@@ -257,8 +437,14 @@ static int ln_forward_impl(const float* x, int64_t ldx, const bf16* addend, int6
   MMAE_CHECK(x && gamma && beta && (y_bf16 || y_f32) && M > 0, MMAE_ERR_ARG, "mmae_layernorm_forward: bad args");
   MMAE_CHECK(!add_scale || (addend && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
              "mmae_add_layernorm_forward: a row scale needs an addend and rows-per-sample dividing M=%d", M);
+  if (D % 128 != 0 && D % 32 == 0 && D > 0 && D <= 1024) {
+    MMAE_CHECK(!addend && !x_sum && !add_scale && !drop.seed, MMAE_ERR_UNSUPPORTED,
+               "mmae_add_layernorm_forward: D=%d: the fused add / drop path / dropout forms need a multiple of 128", D);
+    return ln_forward_narrow(x, ldx, gamma, beta, reinterpret_cast<bf16*>(y_bf16), ldy, y_f32, ldyf, mean, rstd, M, D, eps,
+                             stream);
+  }
   MMAE_CHECK(D % 128 == 0 && D <= 1024 && ldx % 4 == 0 && ldy % 4 == 0 && ldyf % 4 == 0, MMAE_ERR_UNSUPPORTED,
-             "mmae_layernorm_forward: D=%d must be a multiple of 128 and <= 1024", D);
+             "mmae_layernorm_forward: D=%d must be a multiple of 128 (of 32 for the plain form) and <= 1024", D);
   dim3 grid(ceil_div(M, LN_WARPS)), block(LN_WARPS * 32);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   bf16* yb = reinterpret_cast<bf16*>(y_bf16);
@@ -303,6 +489,31 @@ extern "C" int mmae_add_layernorm_forward(const float* x, int64_t ldx, const voi
                                       gamma, beta, reinterpret_cast<bf16*>(y_bf16), ldy, mean, rstd, M, D, eps, stream);
 }
 
+static int ln_backward_narrow(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx, const float* mean,
+                              const float* rstd, const float* gamma, const float* dx_resid, int64_t ldr, float* dx,
+                              int64_t lddx, float* dgamma, float* dbeta, int M, int D, void* stream) {
+  MMAE_CHECK(dgamma && dbeta, MMAE_ERR_ARG, "mmae_layernorm_backward: dgamma / dbeta are required");
+  // one wave, resident blocks per SM as for the float4 kernels of the same width
+  const int per_sm = D <= 256 ? 3 : (D <= 384 ? 2 : 1);
+  dim3 grid(std::min(ceil_div(M, LN_WARPS), sm_count() * per_sm)), block(LN_WARPS * 32);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  float* partial = colred_scratch(size_t(grid.x) * 3 * D, st);
+  if (!partial) return MMAE_ERR_CUDA;
+#define LNBN_CASE(NW)                                                                                                 \
+  case NW:                                                                                                            \
+    launch_k(dy_is_bf16 ? ln_bwd_narrow_kernel<NW, true> : ln_bwd_narrow_kernel<NW, false>, grid, block, 0, st, dy, lddy, x, \
+             ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, partial, M);                                            \
+    break;
+  switch (D / 32) {
+    LN_NARROW_WIDTHS(LNBN_CASE)
+    default: MMAE_CHECK(false, MMAE_ERR_UNSUPPORTED, "mmae_layernorm_backward: unsupported D=%d", D);
+  }
+#undef LNBN_CASE
+  count_launch();
+  MMAE_LAUNCH_OK();
+  return colred_finalize(partial, grid.x, 3 * D, D, dgamma, dbeta, nullptr, st);
+}
+
 static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const float* x, int64_t ldx, const float* mean,
                             const float* rstd, const float* gamma, const float* dx_resid, int64_t ldr, float* dx,
                             int64_t lddx, float* dgamma, float* dbeta, bf16* dx_bf16, int64_t lddxb, float* dx_colsum,
@@ -312,8 +523,15 @@ static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const 
   MMAE_CHECK(!out_scale || (dx_bf16 && rows_per_sample > 0 && M % rows_per_sample == 0), MMAE_ERR_ARG,
              "mmae_layernorm_backward_ex: a row scale needs the bf16 output and rows-per-sample dividing M=%d", M);
   MMAE_CHECK(!drop.seed || dx_bf16, MMAE_ERR_ARG, "mmae_layernorm_backward_ex: a dropout mask needs the bf16 output");
+  if (D % 128 != 0 && D % 32 == 0 && D > 0 && D <= 1024) {
+    MMAE_CHECK(!dx_bf16 && !dx_colsum && !out_scale && !drop.seed, MMAE_ERR_UNSUPPORTED,
+               "mmae_layernorm_backward_ex: D=%d: the bf16 copy / column sums of dx need a multiple of 128", D);
+    return ln_backward_narrow(dy, dy_is_bf16, lddy, x, ldx, mean, rstd, gamma, dx_resid, ldr, dx, lddx, dgamma, dbeta, M, D,
+                              stream);
+  }
   MMAE_CHECK(D % 128 == 0 && D <= 1024 && ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0 && ldr % 4 == 0,
-             MMAE_ERR_UNSUPPORTED, "mmae_layernorm_backward: D=%d must be a multiple of 128 and <= 1024", D);
+             MMAE_ERR_UNSUPPORTED, "mmae_layernorm_backward: D=%d must be a multiple of 128 (of 32 for the plain form) and "
+             "<= 1024", D);
   // one wave: resident blocks per SM follow from the register footprint of the per-lane column accumulators
   static const int tune = []() {
     const char* e = getenv("MMAE_TUNE_LNB");

@@ -3,7 +3,8 @@
   SpatialOutputAdapter (:33-282) - the pre-training decoder, executed as DecoderHeadFunction -> Block x depth ->
                                    DecoderTailFunction;
   LinearOutputAdapter (:285-356) - the classification head of fine-tuning (run_finetuning_cls.py), one ClsHeadFunction;
-  ConvNeXtAdapter (:481-573)     - the semantic-segmentation head of fine-tuning (run_finetuning_semseg.py), executed as
+  ConvNeXtAdapter (:481-573)     - the dense head of semantic-segmentation and depth fine-tuning (run_finetuning_semseg.py,
+                                   run_finetuning_depth.py --output_adapter convnext), executed as
                                    ConvNeXtProjFunction -> ConvNeXtBlockFunction x depth -> ConvNeXtTailFunction.
 
   SegmenterMaskTransformerAdapter (:359-478) - the Segmenter head of the same script (--output_adapter segmenter),
@@ -273,14 +274,19 @@ class ConvNeXtBlock(nn.Module):
                 self.pwconv1.bias, self.pwconv2.weight, self.pwconv2.bias)
 
 
+# ConvNeXtAdapter: the most output channels of a head whose width may be any multiple of 32 (Kp = 8 in the tail)
+NARROW_HEAD_MAX_OUTPUTS = 8
+
+
 class ConvNeXtAdapter(nn.Module):
     """Output adapter with ConvNeXt blocks for semantic segmentation: proj_dec of the main tasks' tokens, reshaped into a
     (nh*s) x (nw*s) map of embed_dim / preds_per_patch channels (s = sqrt(preds_per_patch)), `depth` ConvNeXt blocks, a 1x1
     conv to num_classes and a bilinear upsample to the image size.  Extra keyword arguments (stride_level, ...) are
     ignored, as by the reference.
 
-    The kernels keep the map as a [pixels, channels] matrix whose LayerNorm needs embed_dim / preds_per_patch to be a
-    multiple of 128 and at most 1024 (384 in every shipped semseg config); other widths raise here."""
+    The kernels keep the map as a [pixels, channels] matrix whose LayerNorm needs embed_dim / preds_per_patch to be at most
+    1024 and a multiple of 128 (384 in every shipped semseg config) or, for a regression head of at most
+    NARROW_HEAD_MAX_OUTPUTS output channels, a multiple of 32 (96 in run_finetuning_depth.py); other widths raise here."""
 
     def __init__(self, num_classes, embed_dim: int = 6144, preds_per_patch: int = 16, main_tasks: Iterable[str] = ('rgb',),
                  patch_size: int = 16, depth: int = 4, interpolate_mode: str = 'bilinear', **kwargs):
@@ -292,10 +298,16 @@ class ConvNeXtAdapter(nn.Module):
             raise ValueError("ConvNeXtAdapter: embed_dim=%d is not divisible by preds_per_patch=%d"
                              % (embed_dim, preds_per_patch))
         class_dim = embed_dim // preds_per_patch
-        if class_dim % 128 != 0 or class_dim > 1024:
+        # widths that are a multiple of 32 but not of 128 are for the dense-regression heads (depth: one output channel),
+        # whose class map fits the tail's single 8-column block; heads with more outputs (the semseg classifiers) keep the
+        # multiple-of-128 rule
+        narrow_ok = num_classes <= NARROW_HEAD_MAX_OUTPUTS and class_dim % 32 == 0
+        if not 0 < class_dim <= 1024 or (class_dim % 128 != 0 and not narrow_ok):
             raise NotImplementedError(
-                "ConvNeXtAdapter: embed_dim / preds_per_patch = %d channels; the CUDA head needs a multiple of 128, at most "
-                "1024 (e.g. embed_dim=6144 with preds_per_patch=16)" % class_dim)
+                "ConvNeXtAdapter: embed_dim / preds_per_patch = %d channels for %d outputs; the CUDA head needs a multiple of "
+                "128, at most 1024 (e.g. embed_dim=6144 with preds_per_patch=16), or a multiple of 32, at most 1024, for a "
+                "head of at most %d output channels (e.g. the depth head: preds_per_patch=64, 96 channels)"
+                % (class_dim, num_classes, NARROW_HEAD_MAX_OUTPUTS))
         if interpolate_mode != 'bilinear':
             raise NotImplementedError("ConvNeXtAdapter: interpolate_mode=%r; only 'bilinear' is implemented"
                                       % (interpolate_mode,))
