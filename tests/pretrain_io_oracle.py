@@ -3,7 +3,8 @@
 * embed / ctxproj / dectail: plain float64 of the module's arithmetic.  The tests feed dyadic values chosen so that every
   fp32 sum the kernels form is exact; bf16 roundings of exact values are applied where the kernels store bf16.
 * decoder head: float64 with a bf16 rounding wherever dechead_forward_impl / dechead_backward_impl store a bf16 tensor
-  (RoundFwd on values, RoundBwd on the gradient operands), in both GELU modes of mmae_set_fuse_gelu.
+  (RoundFwd on values, RoundBwd on the gradient operands), in both GELU modes of mmae_set_fuse_gelu; with round=False,
+  plain float64 (the fp32 tier, mmae_dechead_f32_*).
 
 Everything runs on whatever device its inputs are on (the bench-sized cases run it on the GPU in float64)."""
 import math
@@ -143,6 +144,11 @@ class RoundBwd(torch.autograd.Function):
 rf, rb = RoundFwd.apply, RoundBwd.apply
 
 
+def roundings(round):
+    """(rf, rb), or two identities for the plain float64 reference (round=False)"""
+    return (rf, rb) if round else ((lambda x: x), (lambda x: x))
+
+
 class Attention(torch.autograd.Function):
     """softmax(q k^T s) v per head, float64, with the backward's row term delta = rowsum(dO * O) formed from the stored
     bf16 output O as the kernel forms it (not from the float64 P)."""
@@ -162,6 +168,13 @@ class Attention(torch.autograd.Function):
         dp = do @ v.transpose(-1, -2)
         ds = p * (dp - (do * o_b).sum(-1, keepdim=True))
         return ds @ k * ctx.scale, ds.transpose(-1, -2) @ q * ctx.scale, dv, None
+
+
+def attention(q, k, v, scale, round=True):
+    """Attention with the kernels' backward row term (round=True), else plain float64 autograd."""
+    if round:
+        return Attention.apply(q, k, v, scale)
+    return torch.softmax(q @ k.transpose(-1, -2) * scale, -1) @ v
 
 
 def gelu(x):
@@ -211,10 +224,12 @@ def build_queries_context(ctx, ix, mask_token, task_emb, pos, mutate=None):
     return q, context
 
 
-def dechead_reference(ctx, ix, prm, H, eps, fuse_gelu, dout, mutate=None):
+def dechead_reference(ctx, ix, prm, H, eps, fuse_gelu, dout, mutate=None, round=True):
     """Forward and backward of the decoder head from the fp32 context projection `ctx` [B, T+G, Dd] (a float64 leaf, or
     the caller's rounded proj_context of an encoder-output leaf).  prm: float64 leaves (requires_grad) named as
-    DecHeadParams' fields, task_emb a list.  Runs backward(dout); returns (x_out, queries) - queries with its .grad."""
+    DecHeadParams' fields, task_emb a list.  Runs backward(dout); returns (x_out, queries) - queries with its .grad.
+    round=False: no bf16 rounding anywhere and plain attention (fuse_gelu then has no effect)."""
+    rf, rb = roundings(round)
     B, Nc, Dd = ctx.shape
     dh = Dd // H
     queries, context = build_queries_context(ctx, ix, prm["mask_token"], prm["task_emb"], prm["pos"], mutate)
@@ -228,12 +243,12 @@ def dechead_reference(ctx, ix, prm, H, eps, fuse_gelu, dout, mutate=None):
     qh = q.reshape(B, P, H, dh).transpose(1, 2)
     kh = k.reshape(B, Nc, H, dh).transpose(1, 2)
     vh = v.reshape(B, Nc, H, dh).transpose(1, 2)
-    o = rb(rf(Attention.apply(qh, kh, vh, 1.0 / math.sqrt(dh)).transpose(1, 2).reshape(B, P, Dd)))
+    o = rb(rf(attention(qh, kh, vh, 1.0 / math.sqrt(dh), round).transpose(1, 2).reshape(B, P, Dd)))
     x0 = rb(o @ rf(prm["proj_w"]).t()) + prm["proj_b"]
     h = rb(rf(_ln(x0, prm["out_norm_w"], prm["out_norm_b"], eps)))
     zp = h @ rf(prm["fc1_w"]).t() + prm["fc1_b"]
     z = rb(rf(zp))
-    if fuse_gelu:
+    if fuse_gelu and round:
         # GELU in the fc1 epilogue on the fp32 pre-activation (value from zp); fc2's dgrad applies GELU'(bf16 z) to its
         # fp32 accumulator before the one bf16 store (gradient through z)
         gz = gelu(z)
