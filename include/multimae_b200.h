@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 18
+#define MMAE_ABI_VERSION 19
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -698,6 +698,27 @@ int mmae_cls_augment_batch(const void* packed_host, const void* packed, int64_t 
  * ---------------------------------------------------------------------------------------------- */
 int mmae_jpeg_decode_batch(const void* packed_host, void* packed, int64_t host_bytes, int64_t packed_bytes,
                            int num_images, int64_t desc_offset, void* scratch, int64_t scratch_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Pre-training PNG decode (MMAE_GPU_JPEG) — a pixel rectangle of Image.open(f) (then convert('RGB') for rgb,
+ * convert('P') for semseg), bitwise as Pillow decodes it, for non-interlaced PNGs without tRNS: 8-bit gray, RGB or
+ * palette for rgb (kind 0), 16-bit gray for depth (kind 1), 8-bit gray or palette for semseg (kind 2).
+ * multimae_b200/png.py parses the chunks on the host.
+ *
+ * `packed` (packed_bytes, 16-byte aligned) starts with the host_bytes of `packed_host`.  At desc_offset * 16 in it:
+ * int32 descriptors [num_images][16] = {width, height, bit depth, colour type, kind, zlib stream / 16 (the IDAT payloads
+ * joined), its bytes, palette / 16 (uint8 [256][3], rgb from palette only), rectangle first row, first column, rows,
+ * columns, output / 16, scratch offset / 16, unused...}.  Each rectangle is written at its output offset, which must lie
+ * past host_bytes, after the previous image's output: uint8 [rows][columns][3] (kind 0), uint16 (1), uint8 (2).
+ * `scratch`: each image's inflated rows (height * (1 + row bytes), 16-byte aligned), at the running sum of the images
+ * before it.  status (device int32 [num_images]) receives 0 for an image decoded as zlib and Pillow decode it, non-zero
+ * when the stream is anything but a well-formed zlib stream of exactly the image's rows with a matching Adler-32, or a
+ * row has a filter type above 4; such an image's rectangle is not written, and the caller decodes it with Pillow.
+ * Two launches for the whole batch; every descriptor, range and offset is checked on the host first.
+ * ---------------------------------------------------------------------------------------------- */
+int mmae_png_decode_batch(const void* packed_host, void* packed, int64_t host_bytes, int64_t packed_bytes,
+                          int num_images, int64_t desc_offset, void* scratch, int64_t scratch_bytes, int* status,
+                          void* stream);
 
 /* image <-> token layout helpers ('b (nh nw) (c ph pw) <-> b c (nh ph) (nw pw)') */
 int mmae_unpatchify(const float* tokens, int64_t ld_tok, float* image, int B, int C, int nh, int nw, int P,

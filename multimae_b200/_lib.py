@@ -225,6 +225,8 @@ SIGNATURES = {
                                        ctypes.POINTER(c_int), c_void_p, c_i64, c_void_p, ctypes.POINTER(c_float),
                                        ctypes.POINTER(c_float), c_void_p]),
     "mmae_jpeg_decode_batch": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_int, c_i64, c_void_p, c_i64, c_void_p]),
+    "mmae_png_decode_batch": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_int, c_i64, c_void_p, c_i64, c_void_p,
+                                      c_void_p]),
     "mmae_unpatchify": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_unpatchify_bf16": (c_int, [c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mmae_patchify_bf16": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -304,7 +306,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 18
+ABI_VERSION = 19
 
 
 def lib():

@@ -23,12 +23,16 @@ opt-in through the overlay launcher:
                          RandomResizedCropAndInterpolation, RandomHorizontalFlip and RandAugment and crop; the GPU
                          (mmae_cls_augment_batch) resizes, flips, applies the RandAugment ops and normalises, bitwise
                          as Pillow does.
-  * MMAE_GPU_JPEG=1      (with MMAE_GPU_AUGMENT=1) also wraps `build_dataset`: a dataset built with one of those
-                         transforms loads its files with jpeg_loader, which hands the JPEGs the kernels decode
-                         (multimae_b200/jpeg.py) to the transform still compressed; mmae_jpeg_decode_batch decodes the
-                         rectangle each sample needs, bitwise as Pillow's Image.open(f).convert('RGB').  Other files are
-                         decoded by Pillow on the workers.  Off by default: the decode saves worker CPU, but its
-                         sequential entropy decode bounds a loader at about 1,400 samples/s (INTEGRATION.md).
+  * MMAE_GPU_JPEG=1      (with MMAE_GPU_AUGMENT=1) decodes on the GPU where the kernels can.  It wraps `build_dataset`: a
+                         dataset built with one of those transforms loads its files with jpeg_loader, which hands the
+                         JPEGs the kernels decode (multimae_b200/jpeg.py) to the transform still compressed;
+                         mmae_jpeg_decode_batch decodes the rectangle each sample needs, bitwise as Pillow's
+                         Image.open(f).convert('RGB').  And the pre-training dataset loads every domain with
+                         load_pretrain_image: rgb JPEGs as above, and the rgb, depth and semseg PNGs of the forms
+                         multimae_b200/png.py lists, which mmae_png_decode_batch inflates, unfilters and expands on the
+                         copy stream, bitwise as the reference's Image.open + convert.  Other files are decoded by
+                         Pillow on the workers.  Off by default: the decode saves worker CPU, but its sequential
+                         entropy decode and inflate bound a loader (INTEGRATION.md).
 """
 import functools
 import io
@@ -41,7 +45,7 @@ import numpy as np
 import torch
 from torch.utils.data import DataLoader, Dataset
 
-from . import jpeg
+from . import jpeg, png
 
 
 class SyntheticMultiTaskDataset(Dataset):
@@ -275,7 +279,8 @@ def _weights_table_bytes(kind, n_in, bounds, w):
 
 class Crops:
     """What CropOnlyTransform hands the collate function for one sample: the uint8 / uint16 crop of every task (dict order of
-    the dataset), the flip flag and the crop size."""
+    the dataset), the flip flag and the crop size.  Under MMAE_GPU_JPEG a task's entry may instead be
+    (JpegSource or PngSource, (first row, first column, rows, columns)): the rectangle the GPU decodes in its place."""
 
     def __init__(self, arrays, flip, h, w):
         self.arrays, self.flip, self.h, self.w = arrays, flip, h, w
@@ -316,7 +321,7 @@ class CropOnlyTransform:
                                  % (getattr(img, "filename", "") or "<in memory>", img.mode))
             if ijhw is None:
                 ijhw = random_resized_crop_params(img.height, img.width)
-            arrays[task] = _crop(np.asarray(img), *ijhw)
+            arrays[task] = _crop_source(img, task, ijhw)
         return Crops(arrays, flip, ijhw[2], ijhw[3])
 
     def collate(self, samples):
@@ -326,18 +331,26 @@ class CropOnlyTransform:
 
 class PackedBatch:
     """One batch of crops in one host buffer: int32 descriptors [batch, tasks, DESC_FIELDS] at offset 0, then the
-    resampling tables, then the crops, every section 16-byte aligned (offsets in the descriptors count 16-byte units)."""
+    resampling tables (the first `check_bytes`), then the crops, every section 16-byte aligned (offsets in the
+    descriptors count 16-byte units).  With compressed samples (MMAE_GPU_JPEG), also their JPEG / PNG descriptors and
+    data, `jpeg` = (descriptor offset / 16, images, coefficient blocks, plane bytes) and `png` = (descriptor offset / 16,
+    images, inflated bytes): their crops are decoded into a device-only tail, `device_bytes` long in all, and
+    `png_files` holds (path, task, output offset, rectangle) of each PNG for Pillow to decode when the kernels do not."""
 
-    def __init__(self, buffer, tasks, batch, size, map4, scratch_bytes, mean, std):
+    def __init__(self, buffer, tasks, batch, size, map4, scratch_bytes, mean, std, check_bytes=None, jpeg=None,
+                 png=None, png_files=(), device_bytes=None):
         self.buffer, self.tasks, self.batch, self.size, self.map4 = buffer, tasks, batch, size, map4
         self.scratch_bytes, self.mean, self.std = scratch_bytes, mean, std
+        self.check_bytes, self.jpeg, self.png, self.png_files = check_bytes, jpeg, png, list(png_files)
+        self.device_bytes = device_bytes
 
     def pin_memory(self):
         self.buffer = self.buffer.pin_memory()
         return self
 
     def to_device(self, device, pool=None):
-        """Upload the buffer and run the resampling kernels on the current stream: {task: tensor} on `device`."""
+        """Upload the buffer and run the resampling kernels on the current stream: {task: tensor} on `device`.  With
+        PNG samples, the current stream is synchronised once after the decode, to read its status words."""
         from . import kernels
         host = self.buffer
         if not host.is_pinned():
@@ -349,9 +362,57 @@ class PackedBatch:
                     pool["bufs"]["packed"] = stage
             stage[:n].copy_(host)
             host = stage[:n]
-        dev = host.to(device, non_blocking=True)
-        return kernels.augment_batch(host, dev, self.tasks, self.batch, self.size, self.map4, self.scratch_bytes, self.mean,
-                                     self.std)
+        if self.device_bytes is None:
+            dev = host.to(device, non_blocking=True)
+            check = host
+        else:
+            dev = torch.empty(self.device_bytes, dtype=torch.uint8, device=device)
+            dev[:host.numel()].copy_(host, non_blocking=True)
+            if self.jpeg is not None:
+                kernels.jpeg_decode_batch(host, dev, *self.jpeg)
+            if self.png is not None:
+                status = kernels.png_decode_batch(host, dev, *self.png).cpu()   # synchronises the stream
+                for k in torch.nonzero(status).flatten().tolist():
+                    self._decode_with_pillow(k, dev)
+            # mmae_augment_batch reads the descriptors and tables on the host: a buffer of the device's length whose
+            # first check_bytes are the host's (the pages past them are never touched)
+            check = None if pool is None else pool["bufs"].get("check")
+            if check is None or check.numel() < self.device_bytes:
+                check = torch.empty(self.device_bytes, dtype=torch.uint8)
+                if pool is not None:
+                    pool["bufs"]["check"] = check
+            check = check[:self.device_bytes]
+            check[:self.check_bytes].copy_(host[:self.check_bytes])
+        return kernels.augment_batch(check, dev, self.tasks, self.batch, self.size, self.map4, self.scratch_bytes,
+                                     self.mean, self.std)
+
+    def _decode_with_pillow(self, k, dev):
+        """The crop of PNG `k` decoded by Pillow, as the reference loads the file, into its place in `dev`; raises what
+        Pillow raises, naming the file."""
+        path, task, off, (i, j, h, w) = self.png_files[k]
+        try:
+            a = np.asarray(_load_with_pillow(path, task))
+        except Exception as e:
+            raise type(e)("%s: %s" % (path, e)) from e
+        crop = torch.from_numpy(np.array(_crop(a, i, j, h, w)).reshape(-1).view(np.uint8))
+        dev[off:off + crop.numel()].copy_(crop)
+
+
+def jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes):
+    """Fill the mmae_jpeg_decode_batch descriptor `jd` of JpegSource `src` and rectangle `rect` (first row, first
+    column, rows, columns), placing its data with put(array) and its tables with cached(key, make); returns the
+    running (coefficient blocks, plane bytes) after it.  The output field is left to the caller."""
+    jd[:11] = (src.width, src.height, src.ncomp, src.hmax, src.vmax, src.restart,
+               put(np.frombuffer(src.data, np.uint8, src.scan[1] - src.scan[0], src.scan[0])),
+               src.scan[1] - src.scan[0], len(src.intervals), put(src.intervals),
+               cached(("quant", src.quant.tobytes()), lambda: src.quant))
+    for t, key in enumerate(k for pair in src.tables for k in pair):
+        jd[11 + t] = cached(("huffman", key), lambda: np.frombuffer(jpeg.huffman_table_bytes(key), np.uint8))
+    jd[17:21] = rect
+    mpr, mcu0, mcu1, bpm, wins = jpeg.geometry(src.width, src.height, src.ncomp, src.hmax, src.vmax, *rect)
+    jd[22], jd[23] = coef_blocks, plane_bytes // 16
+    return (coef_blocks + (mcu1 - mcu0) * mpr * bpm,
+            plane_bytes + sum((r1 - r0) * (c1 - c0) * 64 for r0, r1, c0, c1 in wins))
 
 
 def pack_batch(crops, size, mean, std):
@@ -369,11 +430,13 @@ def pack_batch(crops, size, mean, std):
         pos = _align16(pos + a.nbytes)
         return off // 16
 
-    def table(kind, n_in, n_out):
-        key = (kind, n_in, n_out)
+    def cached(key, make):
         if key not in tables:
-            tables[key] = put(_table_bytes(kind, n_in, n_out))
+            tables[key] = put(make())
         return tables[key]
+
+    def table(kind, n_in, n_out):
+        return cached((kind, n_in, n_out), lambda: _table_bytes(kind, n_in, n_out))
 
     map4 = table(TABLE_NEAREST, size, size4)
     scratch = 0
@@ -382,27 +445,124 @@ def pack_batch(crops, size, mean, std):
             raise ValueError("MMAE_GPU_AUGMENT: every sample of a batch must carry the tasks %s" % tasks)
         for t, task in enumerate(tasks):
             kind = AUGMENT_KINDS[task]
-            a = c.arrays[task]
             tk = TABLE_NEAREST if kind == 2 else TABLE_BICUBIC
             d = desc[b, t]
             d[0], d[2], d[3], d[4] = kind, c.h, c.w, int(c.flip)
-            d[1] = put(a)
             d[5], d[6] = table(tk, c.w, size), table(tk, c.h, size)
             if kind != 2:
                 d[7] = scratch // 16
                 scratch = _align16(scratch + c.h * size * _CHANNELS[kind] * _ITEMSIZE[kind])
+    check_bytes = pos
+    jpegs = [(b, t) for b, c in enumerate(crops) for t, task in enumerate(tasks)
+             if isinstance(c.arrays[task], tuple) and isinstance(c.arrays[task][0], jpeg.JpegSource)]
+    pngs = [(b, t) for b, c in enumerate(crops) for t, task in enumerate(tasks)
+            if isinstance(c.arrays[task], tuple) and isinstance(c.arrays[task][0], png.PngSource)]
+    jdesc = np.zeros((len(jpegs), JPEG_FIELDS), np.int32)
+    pdesc = np.zeros((len(pngs), PNG_FIELDS), np.int32)
+    jdesc_offset = put(jdesc) if jpegs else 0
+    pdesc_offset = put(pdesc) if pngs else 0
+    for b, c in enumerate(crops):
+        for t, task in enumerate(tasks):
+            if not isinstance(c.arrays[task], tuple):
+                desc[b, t, 1] = put(c.arrays[task])
+    coef_blocks = plane_bytes = 0
+    for jd, (b, t) in zip(jdesc, jpegs):
+        src, rect = crops[b].arrays[tasks[t]]
+        coef_blocks, plane_bytes = jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes)
+    raw = 0
+    for pd, (b, t) in zip(pdesc, pngs):
+        src, rect = crops[b].arrays[tasks[t]]
+        pd[:8] = (src.width, src.height, src.depth, src.ctype, AUGMENT_KINDS[tasks[t]],
+                  put(np.frombuffer(src.stream, np.uint8)), len(src.stream),
+                  cached(("palette", src.palette), lambda: np.frombuffer(src.palette, np.uint8)) if src.palette else 0)
+        pd[8:12] = rect
+        pd[13] = raw // 16
+        raw = _align16(raw + src.height * (1 + src.width * (3 if src.ctype == 2 else src.depth // 8)))
+    tail = pos
+    png_files = []
+    for rows, items, field in ((jdesc, jpegs, 21), (pdesc, pngs, 12)):   # the decoded crops: on the device only
+        for r, (b, t) in zip(rows, items):
+            kind = AUGMENT_KINDS[tasks[t]]
+            desc[b, t, 1] = r[field] = tail // 16
+            if field == 12:
+                png_files.append((crops[b].arrays[tasks[t]][0].path, tasks[t], tail, tuple(r[8:12])))
+            tail = _align16(tail + crops[b].h * crops[b].w * _CHANNELS[kind] * _ITEMSIZE[kind])
     buf = torch.empty(pos, dtype=torch.uint8)
     flat = buf.numpy()
     flat[:desc.nbytes] = desc.reshape(-1).view(np.uint8)
     for off, a in pieces:
         flat[off:off + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
-    return PackedBatch(buf, tasks, B, size, map4, scratch, mean, std)
+    if not jpegs and not pngs:
+        return PackedBatch(buf, tasks, B, size, map4, scratch, mean, std)
+    return PackedBatch(buf, tasks, B, size, map4, scratch, mean, std, check_bytes,
+                       (jdesc_offset, len(jpegs), coef_blocks, plane_bytes) if jpegs else None,
+                       (pdesc_offset, len(pngs), raw) if pngs else None, png_files, tail)
 
 
-def build_gpu_augment_dataset(args, stock):
-    """MMAE_GPU_AUGMENT's build_multimae_pretraining_dataset: the reference's MultiTaskImageFolder with a CropOnlyTransform,
-    or `stock(args)` (the reference's builder), with one printed line, when a domain has no GPU augmentation or there is
-    no CUDA device."""
+def _load_with_pillow(path, task):
+    """The image MultiTaskImageFolder loads for `task`: Image.open, then convert('RGB') for rgb and convert('P') for
+    semseg."""
+    from PIL import Image
+    img = Image.open(path)
+    img = img.convert("RGB") if task == "rgb" else img
+    return img.convert("P") if "semseg" in task else img
+
+
+def load_pretrain_image(path, task):
+    """MMAE_GPU_JPEG's loader of one pre-training file: the JpegSource (rgb) or PngSource of a file the kernels decode,
+    else what the reference loads (_load_with_pillow, raising what it raises)."""
+    with open(path, "rb") as f:
+        data = f.read()
+    if png.is_png(data):
+        src = png.parse(data, task, path)
+    else:
+        src = jpeg.parse(data) if task == "rgb" else None
+    return src if src is not None else _load_with_pillow(path, task)
+
+
+def _crop_source(img, task, ijhw):
+    """CropOnlyTransform's crop of `img`: a slice of the decoded image, or for a compressed source the source and the
+    rectangle, which lies inside the image unless the domains' sizes differ (then the worker decodes it)."""
+    i, j, h, w = ijhw
+    if isinstance(img, (jpeg.JpegSource, png.PngSource)):
+        if i >= 0 and j >= 0 and i + h <= img.height and j + w <= img.width:
+            return img, (i, j, h, w)
+        if isinstance(img, png.PngSource):
+            img = _load_with_pillow(img.path, task)
+        else:
+            from PIL import Image
+            img = Image.open(io.BytesIO(img.data)).convert("RGB")
+    return _crop(np.asarray(img), i, j, h, w)
+
+
+class CompressedMultiTaskImages(Dataset):
+    """MMAE_GPU_JPEG's pre-training dataset: the samples of the reference's MultiTaskImageFolder `folder`, each domain
+    loaded with load_pretrain_image, then `folder.transform` (a CropOnlyTransform)."""
+
+    def __init__(self, folder):
+        self.folder, self.transform = folder, folder.transform
+
+    def __len__(self):
+        return len(self.folder)
+
+    def __getattr__(self, name):
+        if name == "folder":
+            raise AttributeError(name)
+        return getattr(self.folder, name)
+
+    def __getitem__(self, index):
+        sample, target = {}, None
+        for task in self.folder.tasks:
+            path, target = self.folder.samples[task][index]
+            sample[task] = load_pretrain_image(path, task)
+        target_transform = getattr(self.folder, "target_transform", None)
+        return self.transform(sample), target_transform(target) if target_transform is not None else target
+
+
+def build_gpu_augment_dataset(args, stock, compressed=False):
+    """MMAE_GPU_AUGMENT's build_multimae_pretraining_dataset: the reference's MultiTaskImageFolder with a CropOnlyTransform
+    (`compressed`, MMAE_GPU_JPEG: wrapped in CompressedMultiTaskImages), or `stock(args)` (the reference's builder), with
+    one printed line, when a domain has no GPU augmentation or there is no CUDA device."""
     import utils.datasets as ud  # type: ignore  (the reference's module)
     other = [d for d in args.all_domains if d not in AUGMENT_KINDS]
     if other:
@@ -411,7 +571,8 @@ def build_gpu_augment_dataset(args, stock):
     if not torch.cuda.is_available():
         print("MMAE_GPU_AUGMENT: CUDA is not available; keeping the reference transform")
         return stock(args)
-    return ud.MultiTaskImageFolder(args.data_path, args.all_domains, transform=CropOnlyTransform(args))
+    folder = ud.MultiTaskImageFolder(args.data_path, args.all_domains, transform=CropOnlyTransform(args))
+    return CompressedMultiTaskImages(folder) if compressed else folder
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -421,6 +582,7 @@ def build_gpu_augment_dataset(args, stock):
 # ---------------------------------------------------------------------------------------------------------------------
 TABLE_BILINEAR = 3          # same layout as TABLE_BICUBIC
 JPEG_FIELDS = 32            # int32 fields of a JPEG sample's descriptor (include/multimae_b200.h, mmae_jpeg_decode_batch)
+PNG_FIELDS = 16             # int32 fields of a PNG sample's descriptor (mmae_png_decode_batch)
 _TABLE_OF = {FILTER_BILINEAR: TABLE_BILINEAR, FILTER_BICUBIC: TABLE_BICUBIC}
 (OP_IDENTITY, OP_INVERT, OP_POSTERIZE, OP_SOLARIZE, OP_SOLARIZE_ADD, OP_AUTOCONTRAST, OP_EQUALIZE, OP_COLOR, OP_CONTRAST,
  OP_BRIGHTNESS, OP_SHARPNESS, OP_AFFINE, OP_TRANSPOSE) = range(13)
@@ -839,17 +1001,7 @@ def pack_cls_batch(samples, size, mean, std, fill):
         else:
             src, rect = s.jpeg
             jd = jdesc[len(jpeg_out)]
-            jd[:11] = (src.width, src.height, src.ncomp, src.hmax, src.vmax, src.restart,
-                       put(np.frombuffer(src.data, np.uint8, src.scan[1] - src.scan[0], src.scan[0])),
-                       src.scan[1] - src.scan[0], len(src.intervals), put(src.intervals),
-                       table(("quant", src.quant.tobytes()), lambda: src.quant))
-            for t, key in enumerate(k for pair in src.tables for k in pair):
-                jd[11 + t] = table(("huffman", key), lambda: np.frombuffer(jpeg.huffman_table_bytes(key), np.uint8))
-            jd[17:21] = rect
-            mpr, mcu0, mcu1, bpm, wins = jpeg.geometry(src.width, src.height, src.ncomp, src.hmax, src.vmax, *rect)
-            jd[22], jd[23] = coef_blocks, plane_bytes // 16
-            coef_blocks += (mcu1 - mcu0) * mpr * bpm
-            plane_bytes += sum((r1 - r0) * (c1 - c0) * 64 for r0, r1, c0, c1 in wins)
+            coef_blocks, plane_bytes = jpeg_fields(jd, src, rect, put, table, coef_blocks, plane_bytes)
             jpeg_out.append((d, jd, h * w * 3))
         kind = _TABLE_OF[s.filter]
         if s.rows is None:
@@ -989,11 +1141,12 @@ def install():
                 import torch.utils.data as tud
                 import utils.datasets as ud  # type: ignore  (the reference's module)
                 stock = ud.build_multimae_pretraining_dataset
-                ud.build_multimae_pretraining_dataset = functools.partial(build_gpu_augment_dataset, stock=stock)
                 if hasattr(ud, "build_transform"):      # build_dataset (classification) looks it up at call time
                     ud.build_transform = functools.partial(build_gpu_cls_transform, stock=ud.build_transform)
-                jpeg_on = os.environ.get("MMAE_GPU_JPEG", "0") == "1" and hasattr(ud, "build_dataset")
-                if jpeg_on:
+                jpeg_on = os.environ.get("MMAE_GPU_JPEG", "0") == "1"
+                build = functools.partial(build_gpu_augment_dataset, stock=stock)
+                ud.build_multimae_pretraining_dataset = functools.partial(build, compressed=True) if jpeg_on else build
+                if jpeg_on and hasattr(ud, "build_dataset"):
                     ud.build_dataset = functools.partial(build_gpu_cls_dataset, stock=ud.build_dataset)
                 tud.DataLoader = _AugmentingDataLoader
                 did += ["gpu_augment", "gpu_jpeg"] if jpeg_on else ["gpu_augment"]

@@ -178,6 +178,21 @@ def jpeg_decode_batch(host, dev, desc_offset, num_images, coef_blocks, plane_byt
             "mmae_jpeg_decode_batch")
 
 
+def png_decode_batch(host, dev, desc_offset, num_images, raw_bytes):
+    """Decode the PNG rectangles of one packed pre-training batch (multimae_b200.data.pack_batch: `host` its uint8 host
+    buffer, `dev` the device buffer, whose first host.numel() bytes are its copy) into dev's tail, on the current
+    stream.  Returns the int32 [num_images] device status words (0: decoded; otherwise the rectangle is not written)."""
+    _need_cuda(dev)
+    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() <= dev.numel()
+    nbytes = max(int(raw_bytes), 16)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev.device)
+    status = torch.empty(int(num_images), dtype=torch.int32, device=dev.device)
+    L.check(L.lib().mmae_png_decode_batch(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), int(num_images),
+                                          int(desc_offset), scratch.data_ptr(), nbytes, status.data_ptr(),
+                                          L.current_stream()), "mmae_png_decode_batch")
+    return status
+
+
 def cls_augment_batch(host, dev, batch, size, layers, ops_offset, inter_bytes, mean, std, fill, jpeg=None):
     """Resample, flip, RandAugment and normalise one packed classification batch (multimae_b200.data.pack_cls_batch) on
     the current stream: fp32 [B, 3, S, S].  `jpeg` = (descriptor offset / 16, images, coefficient blocks, plane bytes)
