@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 19
+#define MMAE_ABI_VERSION 20
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -689,12 +689,16 @@ int mmae_cls_augment_batch(const void* packed_host, const void* packed, int64_t 
  * none), entropy-coded data / 16, its bytes, restart intervals, their int32 [n][2] byte ranges in the data / 16,
  * int32 [components][64] natural-order quantisers / 16, DC / AC Huffman table / 16 of components 0..2 (6 fields),
  * rectangle first row, first column, rows, columns, output / 16, coefficient scratch offset (blocks of 64 int16),
- * plane scratch offset / 16, unused...}.  Huffman tables: int32 lookup[512] of the next 9 bits (length << 8 | symbol,
+ * plane scratch offset / 16, subsequence record offset, unused...}.  Huffman tables: int32 lookup[512] of the next 9 bits (length << 8 | symbol,
  * 0 for longer codes), int32 maxcode[18], int32 valoffset[18], uint8 symbols[256].  Each rectangle is written as uint8
  * [rows][columns][3] at its output offset, which must lie past host_bytes, after the previous image's output.
  * `scratch`: the coefficients of the MCU rows each rectangle needs (int16 [blocks][64]), then, 256-byte aligned, the
- * uint8 planes of the blocks it needs per component; both offsets are the running sums over the images in order.
- * One memset and 3 launches for the whole batch; every descriptor, range, table and offset is checked on the host first.
+ * uint8 planes of the blocks it needs per component, then, 256-byte aligned, 48-byte subsequence records of the
+ * parallel entropy decode, data bytes / 256 + restart intervals of them per image; the three offsets are the running
+ * sums over the images in order.  Restart intervals of 16 KiB to 256 MiB of entropy-coded data are decoded in parallel
+ * (one CTA each, self-synchronising Huffman decode); shorter ones, and any interval where that decode meets corrupt
+ * data or does not end on the interval's last MCU, by one thread each with libjpeg-turbo's corrupt-data semantics.
+ * One memset and 4 launches for the whole batch; every descriptor, range, table and offset is checked on the host first.
  * ---------------------------------------------------------------------------------------------- */
 int mmae_jpeg_decode_batch(const void* packed_host, void* packed, int64_t host_bytes, int64_t packed_bytes,
                            int num_images, int64_t desc_offset, void* scratch, int64_t scratch_bytes, void* stream);

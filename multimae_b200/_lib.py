@@ -306,7 +306,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 19
+ABI_VERSION = 20
 
 
 def lib():

@@ -398,10 +398,10 @@ class PackedBatch:
         dev[off:off + crop.numel()].copy_(crop)
 
 
-def jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes):
+def jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes, slots):
     """Fill the mmae_jpeg_decode_batch descriptor `jd` of JpegSource `src` and rectangle `rect` (first row, first
     column, rows, columns), placing its data with put(array) and its tables with cached(key, make); returns the
-    running (coefficient blocks, plane bytes) after it.  The output field is left to the caller."""
+    running (coefficient blocks, plane bytes, subsequence records) after it.  The output field is left to the caller."""
     jd[:11] = (src.width, src.height, src.ncomp, src.hmax, src.vmax, src.restart,
                put(np.frombuffer(src.data, np.uint8, src.scan[1] - src.scan[0], src.scan[0])),
                src.scan[1] - src.scan[0], len(src.intervals), put(src.intervals),
@@ -410,9 +410,10 @@ def jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes):
         jd[11 + t] = cached(("huffman", key), lambda: np.frombuffer(jpeg.huffman_table_bytes(key), np.uint8))
     jd[17:21] = rect
     mpr, mcu0, mcu1, bpm, wins = jpeg.geometry(src.width, src.height, src.ncomp, src.hmax, src.vmax, *rect)
-    jd[22], jd[23] = coef_blocks, plane_bytes // 16
+    jd[22], jd[23], jd[24] = coef_blocks, plane_bytes // 16, slots
     return (coef_blocks + (mcu1 - mcu0) * mpr * bpm,
-            plane_bytes + sum((r1 - r0) * (c1 - c0) * 64 for r0, r1, c0, c1 in wins))
+            plane_bytes + sum((r1 - r0) * (c1 - c0) * 64 for r0, r1, c0, c1 in wins),
+            slots + jpeg.subsequence_slots(src.scan[1] - src.scan[0], len(src.intervals)))
 
 
 def pack_batch(crops, size, mean, std):
@@ -465,10 +466,10 @@ def pack_batch(crops, size, mean, std):
         for t, task in enumerate(tasks):
             if not isinstance(c.arrays[task], tuple):
                 desc[b, t, 1] = put(c.arrays[task])
-    coef_blocks = plane_bytes = 0
+    coef_blocks = plane_bytes = slots = 0
     for jd, (b, t) in zip(jdesc, jpegs):
         src, rect = crops[b].arrays[tasks[t]]
-        coef_blocks, plane_bytes = jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes)
+        coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes, slots)
     raw = 0
     for pd, (b, t) in zip(pdesc, pngs):
         src, rect = crops[b].arrays[tasks[t]]
@@ -988,7 +989,7 @@ def pack_cls_batch(samples, size, mean, std, fill):
     jdesc = np.zeros((njpeg, JPEG_FIELDS), np.int32)
     jdesc_offset = put(jdesc) if njpeg else 0
     jpeg_out = []                                # (descriptor row, JPEG descriptor row, crop bytes) of each JPEG
-    coef_blocks = plane_bytes = 0
+    coef_blocks = plane_bytes = slots = 0
     inter = 0
     for b, s in enumerate(samples):
         if len(s.ops) != layers or (s.rows is None) != (samples[0].rows is None):
@@ -1001,7 +1002,7 @@ def pack_cls_batch(samples, size, mean, std, fill):
         else:
             src, rect = s.jpeg
             jd = jdesc[len(jpeg_out)]
-            coef_blocks, plane_bytes = jpeg_fields(jd, src, rect, put, table, coef_blocks, plane_bytes)
+            coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, put, table, coef_blocks, plane_bytes, slots)
             jpeg_out.append((d, jd, h * w * 3))
         kind = _TABLE_OF[s.filter]
         if s.rows is None:

@@ -26,6 +26,11 @@ LOOKAHEAD = 9                  # bits resolved by one lookup in the kernels' Huf
 TABLE_BYTES = 4 * (512 + 18 + 18) + 256
 _SAMPLINGS = ((1, 1), (2, 1), (2, 2))
 MAX_SIDE = 65500               # libjpeg-turbo's JPEG_MAX_DIMENSION
+SUB_BYTES = 512                # bytes of entropy-coded data per subsequence of the parallel decode (csrc/jpeg.cu)
+SLOT_BYTES = 256               # bytes of entropy-coded data per subsequence record reserved in the decode's scratch
+PARALLEL_MIN_BYTES = 16384     # shorter restart intervals are decoded by one thread
+PARALLEL_MAX_BYTES = 1 << 28   # so are longer ones (bit positions in int32)
+SUB_RECORD_BYTES = 48          # one subsequence's record in the decode's scratch
 _MARKER = re.compile(rb"\xff[^\x00]")
 
 
@@ -220,3 +225,27 @@ def geometry(width, height, ncomp, hmax, vmax, y0, x0, rh, rw):
         mcu0 = win[0] // vs if mcu0 is None else min(mcu0, win[0] // vs)
         mcu1 = max(mcu1, (win[1] - 1) // vs + 1)
     return mpr, mcu0, mcu1, bpm, wins
+
+
+def parallel_interval(nbytes):
+    """Whether the kernels decode a restart interval of `nbytes` bytes of entropy-coded data in parallel (one CTA,
+    subsequences of SUB_BYTES) rather than with one thread; csrc/jpeg.cu's jpeg_parallel_interval.  Corrupt data in
+    such an interval still sends it to the one-thread decode."""
+    return PARALLEL_MIN_BYTES <= nbytes < PARALLEL_MAX_BYTES
+
+
+def subsequence_slots(data_bytes, nint):
+    """Subsequence records an image of `data_bytes` bytes of entropy-coded data in `nint` restart intervals reserves in
+    the decode's scratch: interval k's start at (its first byte) // SLOT_BYTES + k."""
+    return data_bytes // SLOT_BYTES + nint
+
+
+def subsequences(segment):
+    """The subsequences the parallel decode cuts one restart interval's bytes into, as the kernel computes them:
+    [(first byte, its index with the stuffed zero bytes removed)], one per SUB_BYTES, moved one byte on where it would
+    start on the zero of an FF 00 pair."""
+    seg = np.frombuffer(segment, np.uint8)
+    n = len(seg)
+    starts = [r + 1 if 0 < r < n and seg[r - 1] == 0xFF else r for r in range(0, n, SUB_BYTES)]
+    ff = np.concatenate([[0], np.cumsum(seg == 0xFF)])
+    return [(r, r - int(ff[r])) for r in starts]

@@ -4,9 +4,11 @@ All compute happens in libmultimae_b200.so; tensors must be CUDA tensors.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib as L
+from . import jpeg
 
 
 def _need_cuda(*ts):
@@ -160,22 +162,34 @@ def cls_scratch_bytes(inter_bytes, batch, size, layers):
     return a(inter_bytes) + (2 * a(batch * size * size * 3) + batch * 1024 * 4 if layers else 0)
 
 
-def jpeg_scratch_bytes(coef_blocks, plane_bytes):
-    """Scratch of mmae_jpeg_decode_batch: int16 coefficients [coef_blocks][64], then (256-byte aligned) the planes."""
-    return (int(coef_blocks) * 128 + 255) // 256 * 256 + int(plane_bytes)
+def jpeg_scratch_bytes(coef_blocks, plane_bytes, slots=0):
+    """Scratch of mmae_jpeg_decode_batch: int16 coefficients [coef_blocks][64], then the planes, then the parallel
+    decode's `slots` subsequence records, each section 256-byte aligned."""
+    a = lambda n: (int(n) + 255) // 256 * 256  # noqa: E731
+    return a(int(coef_blocks) * 128) + a(plane_bytes) + int(slots) * jpeg.SUB_RECORD_BYTES
+
+
+def jpeg_subsequence_slots(host, desc_offset, num_images):
+    """The subsequence records the descriptors in `host` (uint8 tensor or array) reserve: the last image's offset
+    (field 24, running over the images) plus its own."""
+    buf = host.numpy() if isinstance(host, torch.Tensor) else host
+    d = buf[int(desc_offset) * 16:].view(np.int32)[(int(num_images) - 1) * 32:int(num_images) * 32]
+    return int(d[24]) + jpeg.subsequence_slots(int(d[7]), int(d[8]))
 
 
 def jpeg_decode_batch(host, dev, desc_offset, num_images, coef_blocks, plane_bytes):
     """Decode the JPEG rectangles of one packed classification batch (multimae_b200.data.pack_cls_batch: `host` its
     uint8 host buffer, `dev` the device buffer, whose first host.numel() bytes are its copy) into dev's tail, on the
-    current stream."""
+    current stream.  Returns the scratch (its subsequence records tell which restart intervals the parallel decode
+    took)."""
     _need_cuda(dev)
     assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() <= dev.numel()
-    nbytes = jpeg_scratch_bytes(coef_blocks, plane_bytes)
+    nbytes = jpeg_scratch_bytes(coef_blocks, plane_bytes, jpeg_subsequence_slots(host, desc_offset, num_images))
     scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev.device)
     L.check(L.lib().mmae_jpeg_decode_batch(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), int(num_images),
                                            int(desc_offset), scratch.data_ptr(), nbytes, L.current_stream()),
             "mmae_jpeg_decode_batch")
+    return scratch
 
 
 def png_decode_batch(host, dev, desc_offset, num_images, raw_bytes):

@@ -1,6 +1,7 @@
 """Time the GPU JPEG decode of classification fine-tuning (MMAE_GPU_AUGMENT, mmae_jpeg_decode_batch) on one GPU.
 
     python scripts/gpu_time_jpeg_decode.py [--images 512] [--iters 50] [--loader-batches 24] [--steps 20] [--rounds 3]
+                                           [--restart-rows N] [--baseline-lib PATH]
 
 Same images and config as scripts/gpu_time_cls_augment.py: a seeded folder of quality-90 4:2:0 JPEGs of 300 to 600
 pixels per side, input 224, --aa rand-m9-mstd0.5-inc1, bicubic, eval crop_pct 0.875.  "before" is the switch as it
@@ -17,7 +18,11 @@ Prints one JSON line per figure:
     128, 224 x 224, drop_path 0.1, bf16 autocast, AdamW) alone, and with the train batch's decode running back to back
     on a second stream beside it, as a loader's copy stream would: CUDA events on each stream give the step's time and
     the decode's time per call; --rounds rounds of --steps steps, alone and beside alternating.  The decode is kept
-    busy for the whole window (its calls are queued ahead of the steps)."""
+    busy for the whole window (its calls are queued ahead of the steps).
+
+--restart-rows N writes the JPEGs with a restart marker every N MCU rows.  --baseline-lib runs mmae_jpeg_decode_batch
+of another build of the library (an earlier commit's) on the same packed batches, alternating with this one, and
+reports both calls' CUDA-event times and whether their decoded rectangles are bitwise equal."""
 import argparse
 import functools
 import os
@@ -103,8 +108,54 @@ def step_beside_decode(decode, steps, rounds, dev):
     return out
 
 
+def write_tree(root, n, restart_rows, seed=0):
+    """C.write_tree's images, optionally with restart markers."""
+    from PIL import Image
+    rng = np.random.default_rng(seed)
+    for k in range(n):
+        d = os.path.join(root, "class_%d" % (k % 4))
+        os.makedirs(d, exist_ok=True)
+        h, w = int(rng.integers(300, 601)), int(rng.integers(300, 601))
+        Image.fromarray(C.O.make_image(int(rng.integers(1 << 30)), h, w)).save(
+            os.path.join(d, "%05d.jpg" % k), quality=90, **({"restart_marker_rows": restart_rows} if restart_rows else {}))
+
+
+def baseline_call(path):
+    """mmae_jpeg_decode_batch of the library at `path`, as kernels.jpeg_decode_batch calls it (same scratch size)."""
+    import ctypes
+    from multimae_b200 import _lib as L
+    lib = ctypes.CDLL(path)
+    f = lib.mmae_jpeg_decode_batch
+    f.restype = ctypes.c_int
+    f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int64,
+                  ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+
+    def call(host, dev, desc_offset, num_images, coef_blocks, plane_bytes):
+        n = kernels.jpeg_scratch_bytes(coef_blocks, plane_bytes,
+                                       kernels.jpeg_subsequence_slots(host, desc_offset, num_images))
+        scratch = torch.empty(n, dtype=torch.uint8, device=dev.device)
+        assert f(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), num_images, desc_offset,
+                 scratch.data_ptr(), n, L.current_stream()) == 0
+    return call
+
+
+def time_calls(call, iters):
+    for _ in range(5):
+        call()
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for _ in range(iters):
+        call()
+    t1.record()
+    torch.cuda.synchronize()
+    return t0.elapsed_time(t1) / iters
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--restart-rows", type=int, default=0)
+    ap.add_argument("--baseline-lib", default=None)
     ap.add_argument("--images", type=int, default=512)
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--loader-batches", type=int, default=24)
@@ -117,7 +168,8 @@ def main():
     import utils.datasets as ud
     stock = ud.build_transform
     with tempfile.TemporaryDirectory() as root:
-        C.write_tree(root, a.images)
+        write_tree(root, a.images, a.restart_rows)
+        base = baseline_call(a.baseline_lib) if a.baseline_lib else None
         for is_train in (True, False):
             _, ds = datasets(ud, stock, root, is_train)
             random.seed(0)
@@ -147,14 +199,29 @@ def main():
             kern = {}
             for ev in prof.events():
                 if ev.device_type == torch.autograd.DeviceType.CUDA and "jpeg_" in ev.name:
-                    name = next(k for k in ("entropy", "idct", "color") if k in ev.name)
+                    name = next(k for k in ("parallel", "entropy", "idct", "color") if k in ev.name)
                     kern[name] = kern.get(name, 0.0) + ev.device_time / 1e3 / a.iters
+            if base is not None:
+                devbuf[host.numel():].zero_()
+                call()
+                ours = devbuf.clone()
+                devbuf[host.numel():].zero_()
+                base(host, devbuf, *packed.jpeg)
+                torch.cuda.synchronize()
+                same = bool(torch.equal(ours[host.numel():], devbuf[host.numel():]))
+                times = {"this": [], "baseline": []}
+                for _ in range(3):
+                    times["this"].append(round(time_calls(call, a.iters), 4))
+                    times["baseline"].append(round(time_calls(lambda: base(host, devbuf, *packed.jpeg), a.iters), 4))
+                C.emit(figure="decode_call_ms_vs_baseline", transform="train" if is_train else "eval", batch=128,
+                       restart_rows=a.restart_rows, call_event_ms=times, bitwise_equal=same)
             if is_train:
                 rounds = step_beside_decode(call, a.steps, a.rounds, dev)
                 C.emit(figure="step_beside_decode", batch=128, steps=a.steps,
                        step_ms_alone=[round(r[0], 3) for r in rounds], step_ms_beside=[round(r[1], 3) for r in rounds],
                        decode_ms_per_call_beside=[round(r[2], 3) for r in rounds])
             C.emit(figure="decode_per_batch", transform="train" if is_train else "eval", batch=128,
+                   restart_rows=a.restart_rows,
                    kernels_ms={k: round(v, 4) for k, v in kern.items()}, kernels_total_ms=round(sum(kern.values()), 4),
                    call_event_ms=round(t0.elapsed_time(t1) / a.iters, 4), iters=a.iters,
                    compressed_bytes=int(sum(int(x) for x in host.numpy()[packed.jpeg[0] * 16:].view(np.int32)[

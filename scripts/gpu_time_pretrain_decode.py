@@ -101,6 +101,8 @@ def main():
     ap.add_argument("--loader-batches", type=int, default=12)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--baseline-lib", default=None,
+                    help="also time mmae_jpeg_decode_batch of this build of the library (an earlier commit's)")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
@@ -136,6 +138,23 @@ def main():
                 kt[m.group(0)] = kt.get(m.group(0), 0.0) + e.device_time_total / 1e3 / a.iters
         emit(figure="decode kernels per batch of 128 (ms)", batch=128, png_images=packed.png[1],
              jpeg_images=packed.jpeg[1], kernels=kt)
+        if a.baseline_lib:
+            import gpu_time_jpeg_decode as G
+            base = G.baseline_call(a.baseline_lib)
+            tail[host.numel():].zero_()
+            decode()
+            ours = tail.clone()
+            tail[host.numel():].zero_()
+            base(host, tail, *packed.jpeg)
+            kernels.png_decode_batch(host, tail, *packed.png)
+            torch.cuda.synchronize()
+            times = {"this": [], "baseline": []}
+            for _ in range(3):
+                times["this"].append(round(G.time_calls(lambda: kernels.jpeg_decode_batch(host, tail, *packed.jpeg),
+                                                        a.iters), 4))
+                times["baseline"].append(round(G.time_calls(lambda: base(host, tail, *packed.jpeg), a.iters), 4))
+            emit(figure="jpeg decode call per batch of 128 (ms) vs baseline", call_event_ms=times,
+                 bitwise_equal=bool(torch.equal(ours, tail)))
         for task in ("depth", "semseg"):
             rects = [after[i][0].arrays[task] for i in range(128)]
             sub = [D.Crops({task: r}, False, *r[1][2:]) for r in rects]
