@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 20
+#define MMAE_ABI_VERSION 21
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -636,24 +636,27 @@ int mmae_adamw_step_groups(const MmaeAdamwSegment* segs_host, int count, const d
  * depth 'I;16', horizontal then vertical pass, rounded and clipped between the passes as Pillow does), TF.hflip, and
  * TF.normalize(TF.to_tensor(rgb)) / depth / 2**16; semseg ('P', NEAREST) is resized to out_size, then to out_size / 4.
  *
- * `packed` (device) and `packed_host` (its host copy, read for validation only) hold, 16-byte aligned:
+ * `packed` (packed_bytes) holds, 16-byte aligned, and its first host_bytes mirror `packed_host` (read on the host for
+ * validation):
  *   at offset 0, int32 descriptors [batch][num_tasks][8] = {kind, crop offset / 16, crop h, crop w, flip,
  *   column table offset / 16, row table offset / 16, intermediate offset / 16 in `scratch`};
  *   tables: int32 header {n_in, n_out, ksize, type}, then for type 1 (BICUBIC) int32 bounds [n_out][2] = {first tap,
  *   tap count}, int32 22-bit fixed-point weights [n_out][ksize], double weights [n_out][ksize] (8-byte aligned), and for
  *   type 2 (NEAREST) int32 source indices [n_out];
  *   crops: kind 0 (rgb) uint8 [h][w][3], kind 1 (depth) uint16 [h][w], kind 2 (semseg) uint8 [h][w].
- * rgb / depth items use BICUBIC tables crop w -> out_size (columns) and crop h -> out_size (rows) and an intermediate of
+ * Descriptors and tables (map4_offset's included) lie in the host part; a crop may lie past it, in a device-only tail
+ * (where mmae_jpeg_decode_batch and mmae_png_decode_batch write the decoded rectangles).  rgb / depth items use BICUBIC tables crop w -> out_size (columns) and crop h -> out_size (rows) and an intermediate of
  * h x out_size pixels in `scratch`; semseg items use NEAREST tables, composed with the NEAREST table at map4_offset
  * (out_size -> out_size / 4).  out_host[t] (HOST array of num_tasks device pointers) receives task t: fp32
  * [batch, 3, S, S] (rgb), fp32 [batch, 1, S, S] (depth) or int64 [batch, S/4, S/4] (semseg); kinds_host[t] is its kind.
  * mean_host / std_host: 3 floats each (rgb).  Two launches (one per pass) for the whole batch, no atomics.  Every
  * descriptor and table is checked on the host before the first launch: kinds, crop sizes in [1, 32768], offsets and table
- * lengths inside the buffers, table sizes matching the crop, tap ranges and indices inside their input.
+ * lengths inside their parts of the buffers, table sizes matching the crop, tap ranges and indices inside their input.
  * ---------------------------------------------------------------------------------------------- */
-int mmae_augment_batch(const void* packed_host, const void* packed, int64_t packed_bytes, int batch, int num_tasks,
-                       const int* kinds_host, int out_size, int64_t map4_offset, void* scratch, int64_t scratch_bytes,
-                       void* const* out_host, const float* mean_host, const float* std_host, void* stream);
+int mmae_augment_batch(const void* packed_host, const void* packed, int64_t host_bytes, int64_t packed_bytes, int batch,
+                       int num_tasks, const int* kinds_host, int out_size, int64_t map4_offset, void* scratch,
+                       int64_t scratch_bytes, void* const* out_host, const float* mean_host, const float* std_host,
+                       void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Classification fine-tuning augmentation (MMAE_GPU_AUGMENT) — the pixel half of utils/datasets.py:build_transform:

@@ -218,9 +218,9 @@ SIGNATURES = {
     "mmae_adamw_step_groups": (c_int, [ctypes.POINTER(AdamwSegment), c_int, ctypes.POINTER(ctypes.c_double),
                                        ctypes.POINTER(ctypes.c_double), c_int, ctypes.c_double, ctypes.c_double,
                                        ctypes.c_double, c_void_p, c_void_p, c_void_p]),
-    "mmae_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_int, c_int, ctypes.POINTER(c_int), c_int, c_i64, c_void_p,
-                                   c_i64, ctypes.POINTER(c_void_p), ctypes.POINTER(c_float), ctypes.POINTER(c_float),
-                                   c_void_p]),
+    "mmae_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_int, c_int, ctypes.POINTER(c_int), c_int, c_i64,
+                                   c_void_p, c_i64, ctypes.POINTER(c_void_p), ctypes.POINTER(c_float),
+                                   ctypes.POINTER(c_float), c_void_p]),
     "mmae_cls_augment_batch": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_int, c_int, c_i64, c_int,
                                        ctypes.POINTER(c_int), c_void_p, c_i64, c_void_p, ctypes.POINTER(c_float),
                                        ctypes.POINTER(c_float), c_void_p]),
@@ -306,7 +306,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 20
+ABI_VERSION = 21
 
 
 def lib():

@@ -51,7 +51,7 @@ __device__ __forceinline__ int aug_store16(double ss) {
 }
 
 // A crop sample.  kCoherent: through L2 only (ld.global.cg), for crops the previous kernel of the stream wrote (the JPEG
-// decode's tail): a programmatically launched dependent may otherwise hit a stale L1 line (runtime.cu, MMAE_PDL).
+// / PNG decode's tail): a programmatically launched dependent may otherwise hit a stale L1 line (runtime.cu, MMAE_PDL).
 template <bool kCoherent, typename T>
 __device__ __forceinline__ int aug_src(const T* p) {
   if constexpr (kCoherent) return int(__ldcg(p));
@@ -120,6 +120,7 @@ __device__ __forceinline__ void aug_vertical_rgb(const uint8_t* tab, const int* 
 
 // Vertical pass: column x of the scratch image (h x S) -> the S x S output, flipped and normalised; semseg items gather
 // their S/4 x S/4 labels through the nearest maps.
+template <bool kCoherent>
 __global__ void __launch_bounds__(AUG_THREADS) augment_vertical_kernel(const uint8_t* __restrict__ buf,
                                                                        const int* __restrict__ desc,
                                                                        const uint8_t* scratch, int S,
@@ -146,7 +147,8 @@ __global__ void __launch_bounds__(AUG_THREADS) augment_vertical_kernel(const uin
     for (int idx = blockIdx.x * AUG_THREADS + threadIdx.x; idx < S4 * S4; idx += stride) {
       const int y4 = idx / S4, x4 = idx - y4 * S4;
       const int xs = map4[x4];
-      o[idx] = int64_t(src[int64_t(mh[map4[y4]]) * w + mw[flip ? S - 1 - xs : xs]]);
+      const uint8_t* p = &src[int64_t(mh[map4[y4]]) * w + mw[flip ? S - 1 - xs : xs]];
+      o[idx] = int64_t(kCoherent ? __ldcg(p) : *p);   // through L2 when kCoherent, as aug_src
     }
     return;
   }
@@ -175,34 +177,66 @@ __global__ void __launch_bounds__(AUG_THREADS) augment_vertical_kernel(const uin
   }
 }
 
-// Host-side check of one table in the host copy of the packed buffer.
-int check_table(const uint8_t* host, int64_t bytes, int64_t off16, int kind, int n_in, int n_out, int item,
-                std::unordered_set<int64_t>& seen) {
+// Host-side check of one table in the host part (`host_bytes` long) of the packed buffer; `fn` names the entry point.
+int check_table(const char* fn, const uint8_t* host, int64_t host_bytes, int64_t off16, int kind, int n_in, int n_out,
+                int item, std::unordered_set<int64_t>& seen) {
   const int64_t off = off16 * 16;
-  MMAE_CHECK(off16 >= 0 && off + 16 <= bytes, MMAE_ERR_ARG, "mmae_augment_batch: item %d: table offset out of range", item);
+  MMAE_CHECK(off16 >= 0 && off + 16 <= host_bytes, MMAE_ERR_ARG, "%s: item %d: table offset out of range", fn, item);
   const int* hd = reinterpret_cast<const int*>(host + off);
   MMAE_CHECK(hd[3] == kind && hd[0] == n_in && hd[1] == n_out, MMAE_ERR_ARG,
-             "mmae_augment_batch: item %d: table at %lld is {in %d, out %d, kind %d}, expected {%d, %d, %d}", item,
-             (long long)off, hd[0], hd[1], hd[3], n_in, n_out, kind);
+             "%s: item %d: table at %lld is {in %d, out %d, kind %d}, expected {%d, %d, %d}", fn, item, (long long)off,
+             hd[0], hd[1], hd[3], n_in, n_out, kind);
   if (!seen.insert(off).second) return MMAE_OK;
   const int* body = hd + 4;
   if (kind == AUG_TABLE_NEAREST) {
-    MMAE_CHECK(off + 16 + 4 * int64_t(n_out) <= bytes, MMAE_ERR_ARG, "mmae_augment_batch: item %d: table is truncated",
-               item);
+    MMAE_CHECK(off + 16 + 4 * int64_t(n_out) <= host_bytes, MMAE_ERR_ARG, "%s: item %d: table is truncated", fn, item);
     for (int i = 0; i < n_out; ++i)
       MMAE_CHECK(body[i] >= 0 && body[i] < n_in, MMAE_ERR_ARG,
-                 "mmae_augment_batch: item %d: nearest index %d of %d -> %d out of range", item, i, n_in, n_out);
+                 "%s: item %d: nearest index %d of %d -> %d out of range", fn, item, i, n_in, n_out);
     return MMAE_OK;
   }
   const int ksize = hd[2];
-  MMAE_CHECK(ksize >= 1 && ksize <= 4 * AUG_MAX_EXTENT + 1, MMAE_ERR_ARG, "mmae_augment_batch: item %d: bad tap count %d",
-             item, ksize);
-  MMAE_CHECK(off + aug_bicubic_bytes(n_out, ksize) <= bytes, MMAE_ERR_ARG,
-             "mmae_augment_batch: item %d: table is truncated", item);
+  MMAE_CHECK(ksize >= 1 && ksize <= 4 * AUG_MAX_EXTENT + 1, MMAE_ERR_ARG, "%s: item %d: bad tap count %d", fn, item,
+             ksize);
+  MMAE_CHECK(off + aug_bicubic_bytes(n_out, ksize) <= host_bytes, MMAE_ERR_ARG, "%s: item %d: table is truncated", fn,
+             item);
   for (int i = 0; i < n_out; ++i) {
     const int lo = body[2 * i], cnt = body[2 * i + 1];
     MMAE_CHECK(lo >= 0 && cnt >= 0 && cnt <= ksize && lo + cnt <= n_in, MMAE_ERR_ARG,
-               "mmae_augment_batch: item %d: taps [%d, %d + %d) of output %d outside %d inputs", item, lo, lo, cnt, i, n_in);
+               "%s: item %d: taps [%d, %d + %d) of output %d outside %d inputs", fn, item, lo, lo, cnt, i, n_in);
+  }
+  return MMAE_OK;
+}
+
+// Host-side checks of item i shared by both entry points: crop size and flip, the crop inside the buffer (host part or
+// device tail), its two tables of type tk (crop extent -> S) inside the host part, and for rgb / depth the intermediate
+// offset; inter_end and max_rows grow to the end of its intermediate in the scratch and to its crop height.
+int check_item(const char* fn, const uint8_t* host, int64_t host_bytes, int64_t packed_bytes, int i, int tk, int S,
+               std::unordered_set<int64_t>& seen, int64_t& inter_end, int64_t& max_rows) {
+  const int* d = reinterpret_cast<const int*>(host) + int64_t(i) * AUG_DESC;
+  const int kind = d[0], h = d[2], w = d[3];
+  MMAE_CHECK(h >= 1 && w >= 1 && h <= AUG_MAX_EXTENT && w <= AUG_MAX_EXTENT && (d[4] == 0 || d[4] == 1), MMAE_ERR_ARG,
+             "%s: item %d: bad crop %d x %d / flip %d", fn, i, h, w, d[4]);
+  const int64_t px = kind == 0 ? 3 : kind == 1 ? 2 : 1;   // bytes per pixel
+  MMAE_CHECK(d[1] >= 0 && int64_t(d[1]) * 16 + int64_t(h) * w * px <= packed_bytes, MMAE_ERR_ARG,
+             "%s: item %d: crop outside the buffer", fn, i);
+  int rc;
+  if ((rc = check_table(fn, host, host_bytes, d[5], tk, w, S, i, seen)) != MMAE_OK) return rc;
+  if ((rc = check_table(fn, host, host_bytes, d[6], tk, h, S, i, seen)) != MMAE_OK) return rc;
+  if (kind == 2) return MMAE_OK;
+  MMAE_CHECK(d[7] >= 0, MMAE_ERR_ARG, "%s: item %d: bad intermediate offset", fn, i);
+  inter_end = std::max<int64_t>(inter_end, int64_t(d[7]) * 16 + int64_t(h) * S * px);
+  max_rows = std::max<int64_t>(max_rows, h);
+  return MMAE_OK;
+}
+
+// Host-side check of TF.normalize's mean / std (3 floats each) into `norm`.
+int check_norm(const char* fn, const float* mean_host, const float* std_host, AugNorm& norm) {
+  for (int c = 0; c < 3; ++c) {
+    MMAE_CHECK(isfinite(mean_host[c]) && isfinite(std_host[c]) && std_host[c] != 0.0f, MMAE_ERR_ARG,
+               "%s: bad mean / std of channel %d", fn, c);
+    norm.mean[c] = mean_host[c];
+    norm.std[c] = std_host[c];
   }
   return MMAE_OK;
 }
@@ -520,9 +554,9 @@ int check_cls_op(const ClsOp& op, int item, int layer) {
 
 using namespace mmae;
 
-extern "C" int mmae_augment_batch(const void* packed_host, const void* packed, int64_t packed_bytes, int batch,
-                                  int num_tasks, const int* kinds_host, int out_size, int64_t map4_offset, void* scratch,
-                                  int64_t scratch_bytes, void* const* out_host, const float* mean_host,
+extern "C" int mmae_augment_batch(const void* packed_host, const void* packed, int64_t host_bytes, int64_t packed_bytes,
+                                  int batch, int num_tasks, const int* kinds_host, int out_size, int64_t map4_offset,
+                                  void* scratch, int64_t scratch_bytes, void* const* out_host, const float* mean_host,
                                   const float* std_host, void* stream) {
   MMAE_CHECK(packed_host && packed && kinds_host && out_host, MMAE_ERR_ARG, "mmae_augment_batch: null pointer");
   MMAE_CHECK(batch >= 1 && num_tasks >= 1 && num_tasks <= MMAE_MAX_TASKS && int64_t(batch) * num_tasks <= 65535,
@@ -532,9 +566,12 @@ extern "C" int mmae_augment_batch(const void* packed_host, const void* packed, i
   MMAE_CHECK(scratch_bytes >= 0 && (scratch_bytes == 0 || scratch), MMAE_ERR_ARG, "mmae_augment_batch: bad scratch");
   MMAE_CHECK(((reinterpret_cast<uintptr_t>(packed) | reinterpret_cast<uintptr_t>(scratch)) & 15) == 0, MMAE_ERR_ARG,
              "mmae_augment_batch: buffers must be 16-byte aligned");
+  MMAE_CHECK(host_bytes >= 0 && host_bytes <= packed_bytes, MMAE_ERR_ARG,
+             "mmae_augment_batch: host part of %lld bytes, buffer of %lld", (long long)host_bytes,
+             (long long)packed_bytes);
   const int64_t desc_bytes = int64_t(batch) * num_tasks * AUG_DESC * 4;
-  MMAE_CHECK(packed_bytes >= desc_bytes, MMAE_ERR_ARG, "mmae_augment_batch: %lld bytes cannot hold %lld of descriptors",
-             (long long)packed_bytes, (long long)desc_bytes);
+  MMAE_CHECK(host_bytes >= desc_bytes, MMAE_ERR_ARG, "mmae_augment_batch: %lld bytes cannot hold %lld of descriptors",
+             (long long)host_bytes, (long long)desc_bytes);
   bool rgb = false;
   for (int t = 0; t < num_tasks; ++t) {
     MMAE_CHECK(kinds_host[t] >= 0 && kinds_host[t] <= 2, MMAE_ERR_ARG, "mmae_augment_batch: task %d: bad kind %d", t,
@@ -545,37 +582,24 @@ extern "C" int mmae_augment_batch(const void* packed_host, const void* packed, i
   }
   MMAE_CHECK(!rgb || (mean_host && std_host), MMAE_ERR_ARG, "mmae_augment_batch: rgb needs mean and std");
   AugNorm norm = {};
-  for (int c = 0; rgb && c < 3; ++c) {
-    MMAE_CHECK(isfinite(mean_host[c]) && isfinite(std_host[c]) && std_host[c] != 0.0f, MMAE_ERR_ARG,
-               "mmae_augment_batch: bad mean / std of channel %d", c);
-    norm.mean[c] = mean_host[c];
-    norm.std[c] = std_host[c];
-  }
+  int rc;
+  if (rgb && (rc = check_norm("mmae_augment_batch", mean_host, std_host, norm)) != MMAE_OK) return rc;
   const uint8_t* host = static_cast<const uint8_t*>(packed_host);
   std::unordered_set<int64_t> seen;
-  int rc = check_table(host, packed_bytes, map4_offset, AUG_TABLE_NEAREST, out_size, out_size / 4, -1, seen);
+  rc = check_table("mmae_augment_batch", host, host_bytes, map4_offset, AUG_TABLE_NEAREST, out_size, out_size / 4, -1,
+                   seen);
   if (rc != MMAE_OK) return rc;
-  int64_t max_rows = 0;
-  const int* desc = reinterpret_cast<const int*>(host);
+  int64_t inter_end = 0, max_rows = 0;
   for (int i = 0; i < batch * num_tasks; ++i) {
-    const int* d = desc + int64_t(i) * AUG_DESC;
-    const int kind = d[0], h = d[2], w = d[3];
+    const int kind = reinterpret_cast<const int*>(host)[int64_t(i) * AUG_DESC];
     MMAE_CHECK(kind == kinds_host[i % num_tasks], MMAE_ERR_ARG, "mmae_augment_batch: item %d: kind %d, task kind %d", i,
                kind, kinds_host[i % num_tasks]);
-    MMAE_CHECK(h >= 1 && w >= 1 && h <= AUG_MAX_EXTENT && w <= AUG_MAX_EXTENT && (d[4] == 0 || d[4] == 1), MMAE_ERR_ARG,
-               "mmae_augment_batch: item %d: bad crop %d x %d / flip %d", i, h, w, d[4]);
-    const int esize = kind == 1 ? 2 : 1, ch = kind == 0 ? 3 : 1;
-    MMAE_CHECK(d[1] >= 0 && int64_t(d[1]) * 16 + int64_t(h) * w * ch * esize <= packed_bytes, MMAE_ERR_ARG,
-               "mmae_augment_batch: item %d: crop outside the buffer", i);
-    const int tk = kind == 2 ? AUG_TABLE_NEAREST : AUG_TABLE_BICUBIC;
-    if ((rc = check_table(host, packed_bytes, d[5], tk, w, out_size, i, seen)) != MMAE_OK) return rc;
-    if ((rc = check_table(host, packed_bytes, d[6], tk, h, out_size, i, seen)) != MMAE_OK) return rc;
-    if (kind != 2) {
-      MMAE_CHECK(d[7] >= 0 && int64_t(d[7]) * 16 + int64_t(h) * out_size * ch * esize <= scratch_bytes, MMAE_ERR_ARG,
-                 "mmae_augment_batch: item %d: intermediate outside the scratch buffer", i);
-      max_rows = std::max<int64_t>(max_rows, h);
-    }
+    rc = check_item("mmae_augment_batch", host, host_bytes, packed_bytes, i,
+                    kind == 2 ? AUG_TABLE_NEAREST : AUG_TABLE_BICUBIC, out_size, seen, inter_end, max_rows);
+    if (rc != MMAE_OK) return rc;
   }
+  MMAE_CHECK(inter_end <= scratch_bytes, MMAE_ERR_ARG, "mmae_augment_batch: scratch of %lld bytes, %lld needed",
+             (long long)scratch_bytes, (long long)inter_end);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const uint8_t* buf = static_cast<const uint8_t*>(packed);
   const int* desc_dev = reinterpret_cast<const int*>(buf);
@@ -583,16 +607,17 @@ extern "C" int mmae_augment_batch(const void* packed_host, const void* packed, i
   for (int t = 0; t < num_tasks; ++t) outs.p[t] = out_host[t];
   const unsigned items = unsigned(batch * num_tasks);
   const int64_t cap = 1024;
+  const bool coherent = host_bytes < packed_bytes;   // crops past the host part: written by the JPEG / PNG decode
   if (max_rows > 0) {
     const int64_t bx = std::min<int64_t>((max_rows * out_size + AUG_THREADS - 1) / AUG_THREADS, cap);
-    launch_k(augment_horizontal_kernel<false>, dim3(unsigned(bx), items), AUG_THREADS, 0, st, buf, desc_dev,
-             static_cast<uint8_t*>(scratch), out_size);
+    launch_k(coherent ? augment_horizontal_kernel<true> : augment_horizontal_kernel<false>, dim3(unsigned(bx), items),
+             AUG_THREADS, 0, st, buf, desc_dev, static_cast<uint8_t*>(scratch), out_size);
     count_launch();
     MMAE_LAUNCH_OK();
   }
   const int64_t bx = std::min<int64_t>((int64_t(out_size) * out_size + AUG_THREADS - 1) / AUG_THREADS, cap);
-  launch_k(augment_vertical_kernel, dim3(unsigned(bx), items), AUG_THREADS, 0, st, buf, desc_dev,
-           static_cast<const uint8_t*>(scratch), out_size, num_tasks,
+  launch_k(coherent ? augment_vertical_kernel<true> : augment_vertical_kernel<false>, dim3(unsigned(bx), items),
+           AUG_THREADS, 0, st, buf, desc_dev, static_cast<const uint8_t*>(scratch), out_size, num_tasks,
            reinterpret_cast<const int*>(buf + map4_offset * 16) + 4, outs, norm);
   count_launch();
   MMAE_LAUNCH_OK();
@@ -614,13 +639,11 @@ extern "C" int mmae_cls_augment_batch(const void* packed_host, const void* packe
              MMAE_ERR_ARG, "mmae_cls_augment_batch: buffers must be 16-byte aligned");
   AugNorm norm = {};
   ClsFill fill = {};
+  int rc = check_norm("mmae_cls_augment_batch", mean_host, std_host, norm);
+  if (rc != MMAE_OK) return rc;
   for (int c = 0; c < 3; ++c) {
-    MMAE_CHECK(isfinite(mean_host[c]) && isfinite(std_host[c]) && std_host[c] != 0.0f, MMAE_ERR_ARG,
-               "mmae_cls_augment_batch: bad mean / std of channel %d", c);
     MMAE_CHECK(fill_host[c] >= 0 && fill_host[c] <= 255, MMAE_ERR_ARG, "mmae_cls_augment_batch: bad fill %d",
                fill_host[c]);
-    norm.mean[c] = mean_host[c];
-    norm.std[c] = std_host[c];
     fill.c[c] = fill_host[c];
   }
   const int S = out_size;
@@ -633,27 +656,18 @@ extern "C" int mmae_cls_augment_batch(const void* packed_host, const void* packe
              "mmae_cls_augment_batch: op records [%lld, +%lld) overlap the descriptors or leave the %lld-byte host part",
              (long long)(ops_offset * 16), (long long)ops_bytes, (long long)host_bytes);
   const uint8_t* host = static_cast<const uint8_t*>(packed_host);
-  const int* desc = reinterpret_cast<const int*>(host);
   std::unordered_set<int64_t> seen;
-  int64_t inter_end = 0;
-  int rc;
+  int64_t inter_end = 0, max_rows = 0;
   for (int i = 0; i < batch; ++i) {
-    const int* d = desc + int64_t(i) * AUG_DESC;
-    const int h = d[2], w = d[3];
+    const int* d = reinterpret_cast<const int*>(host) + int64_t(i) * AUG_DESC;
     MMAE_CHECK(d[0] == 0, MMAE_ERR_ARG, "mmae_cls_augment_batch: item %d: kind %d, expected 0 (rgb)", i, d[0]);
-    MMAE_CHECK(h >= 1 && w >= 1 && h <= AUG_MAX_EXTENT && w <= AUG_MAX_EXTENT && (d[4] == 0 || d[4] == 1), MMAE_ERR_ARG,
-               "mmae_cls_augment_batch: item %d: bad crop %d x %d / flip %d", i, h, w, d[4]);
-    MMAE_CHECK(d[1] >= 0 && int64_t(d[1]) * 16 + int64_t(h) * w * 3 <= packed_bytes, MMAE_ERR_ARG,
-               "mmae_cls_augment_batch: item %d: crop outside the buffer", i);
     MMAE_CHECK(d[5] >= 0 && int64_t(d[5]) * 16 + 16 <= host_bytes, MMAE_ERR_ARG,
                "mmae_cls_augment_batch: item %d: table offset out of range", i);
     const int tk = reinterpret_cast<const int*>(host + int64_t(d[5]) * 16)[3];
     MMAE_CHECK(tk == AUG_TABLE_BICUBIC || tk == AUG_TABLE_BILINEAR, MMAE_ERR_ARG,
                "mmae_cls_augment_batch: item %d: table type %d", i, tk);
-    if ((rc = check_table(host, host_bytes, d[5], tk, w, S, i, seen)) != MMAE_OK) return rc;
-    if ((rc = check_table(host, host_bytes, d[6], tk, h, S, i, seen)) != MMAE_OK) return rc;
-    MMAE_CHECK(d[7] >= 0, MMAE_ERR_ARG, "mmae_cls_augment_batch: item %d: bad intermediate offset", i);
-    inter_end = std::max<int64_t>(inter_end, int64_t(d[7]) * 16 + int64_t(h) * S * 3);
+    rc = check_item("mmae_cls_augment_batch", host, host_bytes, packed_bytes, i, tk, S, seen, inter_end, max_rows);
+    if (rc != MMAE_OK) return rc;
     for (int l = 0; l < num_layers; ++l) {
       ClsOp op;
       memcpy(&op, host + ops_offset * 16 + (int64_t(i) * num_layers + l) * int64_t(sizeof(ClsOp)), sizeof(ClsOp));
@@ -672,12 +686,10 @@ extern "C" int mmae_cls_augment_batch(const void* packed_host, const void* packe
   const uint8_t* buf = static_cast<const uint8_t*>(packed);
   const int* desc_dev = reinterpret_cast<const int*>(buf);
   uint8_t* sc = static_cast<uint8_t*>(scratch);
-  int64_t max_rows = 0;
-  for (int i = 0; i < batch; ++i) max_rows = std::max<int64_t>(max_rows, desc[int64_t(i) * AUG_DESC + 2]);
   const int64_t cap = 1024;
   const int64_t bx_h = std::min<int64_t>((max_rows * S + AUG_THREADS - 1) / AUG_THREADS, cap);
-  // crops past the host part were written by mmae_jpeg_decode_batch's last kernel
-  launch_k(host_bytes < packed_bytes ? augment_horizontal_kernel<true> : augment_horizontal_kernel<false>,
+  const bool coherent = host_bytes < packed_bytes;   // crops past the host part: written by the JPEG decode
+  launch_k(coherent ? augment_horizontal_kernel<true> : augment_horizontal_kernel<false>,
            dim3(unsigned(bx_h), unsigned(batch)), AUG_THREADS, 0, st, buf, desc_dev, sc, S);
   count_launch();
   MMAE_LAUNCH_OK();
@@ -685,8 +697,9 @@ extern "C" int mmae_cls_augment_batch(const void* packed_host, const void* packe
   if (num_layers == 0) {
     AugOutputs outs = {};
     outs.p[0] = out;
-    launch_k(augment_vertical_kernel, dim3(bx, unsigned(batch)), AUG_THREADS, 0, st, buf, desc_dev,
-             static_cast<const uint8_t*>(sc), S, 1, static_cast<const int*>(nullptr), outs, norm);
+    launch_k(coherent ? augment_vertical_kernel<true> : augment_vertical_kernel<false>, dim3(bx, unsigned(batch)),
+             AUG_THREADS, 0, st, buf, desc_dev, static_cast<const uint8_t*>(sc), S, 1, static_cast<const int*>(nullptr),
+             outs, norm);
     count_launch();
     MMAE_LAUNCH_OK();
     return MMAE_OK;

@@ -45,7 +45,7 @@ import numpy as np
 import torch
 from torch.utils.data import DataLoader, Dataset
 
-from . import jpeg, png
+from . import jpeg, kernels, png
 
 
 class SyntheticMultiTaskDataset(Dataset):
@@ -71,9 +71,9 @@ class SyntheticMultiTaskDataset(Dataset):
 
 
 def _to_device(batch, device, pool):
-    """Recursively copy the tensors of `batch` to `device` through pinned staging buffers (non-blocking); a PackedBatch is
-    uploaded and resampled on the current stream."""
-    if isinstance(batch, (PackedBatch, PackedClsBatch)):
+    """Recursively copy the tensors of `batch` to `device` through pinned staging buffers (non-blocking); a packed batch
+    (PackedBatch, PackedClsBatch) is uploaded, decoded and resampled on the current stream."""
+    if isinstance(batch, _Packed):
         return batch.to_device(device, pool)
     if isinstance(batch, torch.Tensor):
         if batch.is_cuda:
@@ -329,29 +329,57 @@ class CropOnlyTransform:
                 torch.tensor([s[1] for s in samples])]
 
 
-class PackedBatch:
-    """One batch of crops in one host buffer: int32 descriptors [batch, tasks, DESC_FIELDS] at offset 0, then the
-    resampling tables (the first `check_bytes`), then the crops, every section 16-byte aligned (offsets in the
-    descriptors count 16-byte units).  With compressed samples (MMAE_GPU_JPEG), also their JPEG / PNG descriptors and
-    data, `jpeg` = (descriptor offset / 16, images, coefficient blocks, plane bytes) and `png` = (descriptor offset / 16,
-    images, inflated bytes): their crops are decoded into a device-only tail, `device_bytes` long in all, and
-    `png_files` holds (path, task, output offset, rectangle) of each PNG for Pillow to decode when the kernels do not."""
+class _Packer:
+    """Lays out one packed batch: arrays at 16-byte aligned offsets of the host part (put; each table once, cached),
+    then, past it, the device-only tail where the decode writes the crops of compressed samples (device)."""
 
-    def __init__(self, buffer, tasks, batch, size, map4, scratch_bytes, mean, std, check_bytes=None, jpeg=None,
-                 png=None, png_files=(), device_bytes=None):
-        self.buffer, self.tasks, self.batch, self.size, self.map4 = buffer, tasks, batch, size, map4
-        self.scratch_bytes, self.mean, self.std = scratch_bytes, mean, std
-        self.check_bytes, self.jpeg, self.png, self.png_files = check_bytes, jpeg, png, list(png_files)
-        self.device_bytes = device_bytes
+    def __init__(self):
+        self.pieces, self.pos, self.tables, self.end = [], 0, {}, 0
+
+    def put(self, a):
+        """Place `a` (copied by buffer(), so it may still be filled in) in the host part; returns its offset / 16."""
+        off = self.pos
+        self.pieces.append((off, a))
+        self.pos = _align16(off + a.nbytes)
+        return off // 16
+
+    def cached(self, key, make):
+        if key not in self.tables:
+            self.tables[key] = self.put(make())
+        return self.tables[key]
+
+    def device(self, nbytes):
+        """Reserve `nbytes` of the device-only tail (after the last put); returns its offset / 16."""
+        off = max(self.end, self.pos)
+        self.end = _align16(off + nbytes)
+        return off // 16
+
+    def buffer(self):
+        """(the host part as a uint8 tensor, the device buffer's length)."""
+        buf = torch.empty(self.pos, dtype=torch.uint8)
+        flat = buf.numpy()
+        for off, a in self.pieces:
+            flat[off:off + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
+        return buf, max(self.end, self.pos)
+
+
+class _Packed:
+    """A batch packed into one host buffer for the GPU (_Packer's layout).  Its device copy is `device_bytes` long: the
+    host part, then the tail where the decode writes the crops of compressed samples (MMAE_GPU_JPEG).  `jpeg` =
+    (descriptor offset / 16, images, coefficient blocks, plane bytes) and `png` = (descriptor offset / 16, images,
+    inflated bytes) when the batch has such samples; `png_files` holds (path, task, output offset, rectangle) of each
+    PNG for Pillow to decode when the kernels do not."""
+
+    def __init__(self, buffer, device_bytes, jpeg=None, png=None, png_files=()):
+        self.buffer, self.device_bytes, self.jpeg, self.png, self.png_files = buffer, device_bytes, jpeg, png, png_files
 
     def pin_memory(self):
         self.buffer = self.buffer.pin_memory()
         return self
 
     def to_device(self, device, pool=None):
-        """Upload the buffer and run the resampling kernels on the current stream: {task: tensor} on `device`.  With
+        """Upload the buffer, decode the compressed samples and run the resampling kernels on the current stream.  With
         PNG samples, the current stream is synchronised once after the decode, to read its status words."""
-        from . import kernels
         host = self.buffer
         if not host.is_pinned():
             n = host.numel()
@@ -362,29 +390,15 @@ class PackedBatch:
                     pool["bufs"]["packed"] = stage
             stage[:n].copy_(host)
             host = stage[:n]
-        if self.device_bytes is None:
-            dev = host.to(device, non_blocking=True)
-            check = host
-        else:
-            dev = torch.empty(self.device_bytes, dtype=torch.uint8, device=device)
-            dev[:host.numel()].copy_(host, non_blocking=True)
-            if self.jpeg is not None:
-                kernels.jpeg_decode_batch(host, dev, *self.jpeg)
-            if self.png is not None:
-                status = kernels.png_decode_batch(host, dev, *self.png).cpu()   # synchronises the stream
-                for k in torch.nonzero(status).flatten().tolist():
-                    self._decode_with_pillow(k, dev)
-            # mmae_augment_batch reads the descriptors and tables on the host: a buffer of the device's length whose
-            # first check_bytes are the host's (the pages past them are never touched)
-            check = None if pool is None else pool["bufs"].get("check")
-            if check is None or check.numel() < self.device_bytes:
-                check = torch.empty(self.device_bytes, dtype=torch.uint8)
-                if pool is not None:
-                    pool["bufs"]["check"] = check
-            check = check[:self.device_bytes]
-            check[:self.check_bytes].copy_(host[:self.check_bytes])
-        return kernels.augment_batch(check, dev, self.tasks, self.batch, self.size, self.map4, self.scratch_bytes,
-                                     self.mean, self.std)
+        dev = torch.empty(self.device_bytes, dtype=torch.uint8, device=device)
+        dev[:host.numel()].copy_(host, non_blocking=True)
+        if self.jpeg is not None:
+            kernels.jpeg_decode_batch(host, dev, *self.jpeg)
+        if self.png is not None:
+            status = kernels.png_decode_batch(host, dev, *self.png).cpu()   # synchronises the stream
+            for k in torch.nonzero(status).flatten().tolist():
+                self._decode_with_pillow(k, dev)
+        return self.resample(host, dev)
 
     def _decode_with_pillow(self, k, dev):
         """The crop of PNG `k` decoded by Pillow, as the reference loads the file, into its place in `dev`; raises what
@@ -398,10 +412,27 @@ class PackedBatch:
         dev[off:off + crop.numel()].copy_(crop)
 
 
-def jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes, slots):
+class PackedBatch(_Packed):
+    """One pre-training batch: int32 descriptors [batch, tasks, DESC_FIELDS] at offset 0, then the resampling tables,
+    then the JPEG / PNG descriptors and data and the crops (offsets in the descriptors count 16-byte units)."""
+
+    def __init__(self, buffer, device_bytes, tasks, batch, size, map4, scratch_bytes, mean, std, jpeg=None, png=None,
+                 png_files=()):
+        super().__init__(buffer, device_bytes, jpeg, png, png_files)
+        self.tasks, self.batch, self.size, self.map4 = tasks, batch, size, map4
+        self.scratch_bytes, self.mean, self.std = scratch_bytes, mean, std
+
+    def resample(self, host, dev):
+        """{task: tensor} of the uploaded and decoded batch on dev's device."""
+        return kernels.augment_batch(host, dev, self.tasks, self.batch, self.size, self.map4, self.scratch_bytes,
+                                     self.mean, self.std)
+
+
+def jpeg_fields(jd, src, rect, packer, coef_blocks, plane_bytes, slots):
     """Fill the mmae_jpeg_decode_batch descriptor `jd` of JpegSource `src` and rectangle `rect` (first row, first
-    column, rows, columns), placing its data with put(array) and its tables with cached(key, make); returns the
-    running (coefficient blocks, plane bytes, subsequence records) after it.  The output field is left to the caller."""
+    column, rows, columns), placing its data and tables with `packer` (_Packer); returns the running (coefficient
+    blocks, plane bytes, subsequence records) after it.  The output field is left to the caller."""
+    put, cached = packer.put, packer.cached
     jd[:11] = (src.width, src.height, src.ncomp, src.hmax, src.vmax, src.restart,
                put(np.frombuffer(src.data, np.uint8, src.scan[1] - src.scan[0], src.scan[0])),
                src.scan[1] - src.scan[0], len(src.intervals), put(src.intervals),
@@ -422,22 +453,11 @@ def pack_batch(crops, size, mean, std):
     B, T = len(crops), len(tasks)
     size4 = int(size * 0.25)
     desc = np.zeros((B, T, DESC_FIELDS), np.int32)
-    pieces, pos, tables = [], _align16(desc.nbytes), {}
-
-    def put(a):
-        nonlocal pos
-        off = pos
-        pieces.append((off, a))
-        pos = _align16(pos + a.nbytes)
-        return off // 16
-
-    def cached(key, make):
-        if key not in tables:
-            tables[key] = put(make())
-        return tables[key]
+    P = _Packer()
+    P.put(desc)
 
     def table(kind, n_in, n_out):
-        return cached((kind, n_in, n_out), lambda: _table_bytes(kind, n_in, n_out))
+        return P.cached((kind, n_in, n_out), lambda: _table_bytes(kind, n_in, n_out))
 
     map4 = table(TABLE_NEAREST, size, size4)
     scratch = 0
@@ -453,51 +473,41 @@ def pack_batch(crops, size, mean, std):
             if kind != 2:
                 d[7] = scratch // 16
                 scratch = _align16(scratch + c.h * size * _CHANNELS[kind] * _ITEMSIZE[kind])
-    check_bytes = pos
     jpegs = [(b, t) for b, c in enumerate(crops) for t, task in enumerate(tasks)
              if isinstance(c.arrays[task], tuple) and isinstance(c.arrays[task][0], jpeg.JpegSource)]
     pngs = [(b, t) for b, c in enumerate(crops) for t, task in enumerate(tasks)
             if isinstance(c.arrays[task], tuple) and isinstance(c.arrays[task][0], png.PngSource)]
     jdesc = np.zeros((len(jpegs), JPEG_FIELDS), np.int32)
     pdesc = np.zeros((len(pngs), PNG_FIELDS), np.int32)
-    jdesc_offset = put(jdesc) if jpegs else 0
-    pdesc_offset = put(pdesc) if pngs else 0
+    jdesc_offset = P.put(jdesc) if jpegs else 0
+    pdesc_offset = P.put(pdesc) if pngs else 0
     for b, c in enumerate(crops):
         for t, task in enumerate(tasks):
             if not isinstance(c.arrays[task], tuple):
-                desc[b, t, 1] = put(c.arrays[task])
+                desc[b, t, 1] = P.put(c.arrays[task])
     coef_blocks = plane_bytes = slots = 0
     for jd, (b, t) in zip(jdesc, jpegs):
         src, rect = crops[b].arrays[tasks[t]]
-        coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, put, cached, coef_blocks, plane_bytes, slots)
+        coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, P, coef_blocks, plane_bytes, slots)
     raw = 0
     for pd, (b, t) in zip(pdesc, pngs):
         src, rect = crops[b].arrays[tasks[t]]
-        pd[:8] = (src.width, src.height, src.depth, src.ctype, AUGMENT_KINDS[tasks[t]],
-                  put(np.frombuffer(src.stream, np.uint8)), len(src.stream),
-                  cached(("palette", src.palette), lambda: np.frombuffer(src.palette, np.uint8)) if src.palette else 0)
+        stream = P.put(np.frombuffer(src.stream, np.uint8))
+        palette = P.cached(("palette", src.palette), lambda: np.frombuffer(src.palette, np.uint8)) if src.palette else 0
+        pd[:8] = src.width, src.height, src.depth, src.ctype, AUGMENT_KINDS[tasks[t]], stream, len(src.stream), palette
         pd[8:12] = rect
         pd[13] = raw // 16
         raw = _align16(raw + src.height * (1 + src.width * (3 if src.ctype == 2 else src.depth // 8)))
-    tail = pos
     png_files = []
     for rows, items, field in ((jdesc, jpegs, 21), (pdesc, pngs, 12)):   # the decoded crops: on the device only
         for r, (b, t) in zip(rows, items):
             kind = AUGMENT_KINDS[tasks[t]]
-            desc[b, t, 1] = r[field] = tail // 16
+            desc[b, t, 1] = r[field] = P.device(crops[b].h * crops[b].w * _CHANNELS[kind] * _ITEMSIZE[kind])
             if field == 12:
-                png_files.append((crops[b].arrays[tasks[t]][0].path, tasks[t], tail, tuple(r[8:12])))
-            tail = _align16(tail + crops[b].h * crops[b].w * _CHANNELS[kind] * _ITEMSIZE[kind])
-    buf = torch.empty(pos, dtype=torch.uint8)
-    flat = buf.numpy()
-    flat[:desc.nbytes] = desc.reshape(-1).view(np.uint8)
-    for off, a in pieces:
-        flat[off:off + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
-    if not jpegs and not pngs:
-        return PackedBatch(buf, tasks, B, size, map4, scratch, mean, std)
-    return PackedBatch(buf, tasks, B, size, map4, scratch, mean, std, check_bytes,
+                png_files.append((crops[b].arrays[tasks[t]][0].path, tasks[t], int(r[field]) * 16, tuple(r[8:12])))
+    return PackedBatch(*P.buffer(), tasks, B, size, map4, scratch, mean, std,
                        (jdesc_offset, len(jpegs), coef_blocks, plane_bytes) if jpegs else None,
-                       (pdesc_offset, len(pngs), raw) if pngs else None, png_files, tail)
+                       (pdesc_offset, len(pngs), raw) if pngs else None, png_files)
 
 
 def _load_with_pillow(path, task):
@@ -925,43 +935,20 @@ class ClsEvalTransform(_ClsTransform):
         return "ClsEvalTransform(resize=%d, center crop %d; resampled on the GPU)" % (self.resize, self.input_size)
 
 
-class PackedClsBatch:
-    """One classification batch in one host buffer: int32 descriptors [batch, DESC_FIELDS] (pack_batch's layout with one
-    task), then the op records OP_DTYPE [batch, layers], then the tables, then the crops, every section 16-byte
-    aligned.  With JPEG samples, also their descriptors (JPEG_FIELDS int32 each), entropy-coded data, intervals and
-    tables, and `jpeg` = (descriptor offset / 16, images, coefficient blocks, plane bytes): their crops are decoded
-    into a device-only tail, `device_bytes` long in all."""
+class PackedClsBatch(_Packed):
+    """One classification batch: int32 descriptors [batch, DESC_FIELDS] (pack_batch's layout with one task), then the
+    op records OP_DTYPE [batch, layers], then the JPEG descriptors (JPEG_FIELDS int32 each), then each sample's crop or
+    JPEG data and its tables."""
 
-    def __init__(self, buffer, batch, size, layers, ops_offset, inter_bytes, mean, std, fill, jpeg=None,
-                 device_bytes=None):
-        self.buffer, self.batch, self.size, self.layers, self.ops_offset = buffer, batch, size, layers, ops_offset
+    def __init__(self, buffer, device_bytes, batch, size, layers, ops_offset, inter_bytes, mean, std, fill, jpeg=None):
+        super().__init__(buffer, device_bytes, jpeg)
+        self.batch, self.size, self.layers, self.ops_offset = batch, size, layers, ops_offset
         self.inter_bytes, self.mean, self.std, self.fill = inter_bytes, mean, std, fill
-        self.jpeg, self.device_bytes = jpeg, device_bytes
 
-    def pin_memory(self):
-        self.buffer = self.buffer.pin_memory()
-        return self
-
-    def to_device(self, device, pool=None):
-        """Upload the buffer and run the kernels on the current stream: fp32 [B, 3, S, S] on `device`."""
-        from . import kernels
-        host = self.buffer
-        if not host.is_pinned():
-            n = host.numel()
-            stage = None if pool is None else pool["bufs"].get("packed")
-            if stage is None or stage.numel() < n:
-                stage = torch.empty(n + n // 4, dtype=torch.uint8).pin_memory()
-                if pool is not None:
-                    pool["bufs"]["packed"] = stage
-            stage[:n].copy_(host)
-            host = stage[:n]
-        if self.jpeg is None:
-            dev = host.to(device, non_blocking=True)
-        else:
-            dev = torch.empty(self.device_bytes, dtype=torch.uint8, device=device)
-            dev[:host.numel()].copy_(host, non_blocking=True)
+    def resample(self, host, dev):
+        """fp32 [B, 3, S, S] of the uploaded and decoded batch on dev's device."""
         return kernels.cls_augment_batch(host, dev, self.batch, self.size, self.layers, self.ops_offset,
-                                         self.inter_bytes, self.mean, self.std, self.fill, self.jpeg)
+                                         self.inter_bytes, self.mean, self.std, self.fill)
 
 
 def pack_cls_batch(samples, size, mean, std, fill):
@@ -970,24 +957,12 @@ def pack_cls_batch(samples, size, mean, std, fill):
     layers = len(samples[0].ops)
     desc = np.zeros((B, DESC_FIELDS), np.int32)
     ops = np.zeros((B, layers), OP_DTYPE)
-    ops_offset = _align16(desc.nbytes)
-    pieces, pos, tables = [], _align16(ops_offset + ops.nbytes), {}
-
-    def put(a):
-        nonlocal pos
-        off = pos
-        pieces.append((off, a))
-        pos = _align16(pos + a.nbytes)
-        return off // 16
-
-    def table(key, make):
-        if key not in tables:
-            tables[key] = put(make())
-        return tables[key]
-
+    P = _Packer()
+    P.put(desc)
+    ops_offset = P.put(ops)
     njpeg = sum(s.jpeg is not None for s in samples)
     jdesc = np.zeros((njpeg, JPEG_FIELDS), np.int32)
-    jdesc_offset = put(jdesc) if njpeg else 0
+    jdesc_offset = P.put(jdesc) if njpeg else 0
     jpeg_out = []                                # (descriptor row, JPEG descriptor row, crop bytes) of each JPEG
     coef_blocks = plane_bytes = slots = 0
     inter = 0
@@ -998,39 +973,31 @@ def pack_cls_batch(samples, size, mean, std, fill):
         d = desc[b]
         d[0], d[2], d[3], d[4] = 0, h, w, int(s.flip)
         if s.jpeg is None:
-            d[1] = put(s.crop)
+            d[1] = P.put(s.crop)
         else:
             src, rect = s.jpeg
             jd = jdesc[len(jpeg_out)]
-            coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, put, table, coef_blocks, plane_bytes, slots)
+            coef_blocks, plane_bytes, slots = jpeg_fields(jd, src, rect, P, coef_blocks, plane_bytes, slots)
             jpeg_out.append((d, jd, h * w * 3))
         kind = _TABLE_OF[s.filter]
         if s.rows is None:
-            d[5] = table((kind, w, size), lambda: _weights_table_bytes(kind, w, *resample_coeffs(s.filter, w, size)))
-            d[6] = table((kind, h, size), lambda: _weights_table_bytes(kind, h, *resample_coeffs(s.filter, h, size)))
+            d[5] = P.cached((kind, w, size), lambda: _weights_table_bytes(kind, w, *resample_coeffs(s.filter, w, size)))
+            d[6] = P.cached((kind, h, size), lambda: _weights_table_bytes(kind, h, *resample_coeffs(s.filter, h, size)))
         else:
             for field, (n_in, n_res, start), extent in ((5, s.cols, w), (6, s.rows, h)):
                 def make(n_in=n_in, n_res=n_res, start=start, extent=extent):
                     b_, _, ws, _, e = sliced_table(s.filter, n_in, n_res, start, size)
                     assert e == extent
                     return _weights_table_bytes(kind, extent, b_, ws)
-                d[field] = table((kind, n_in, n_res, start), make)
+                d[field] = P.cached((kind, n_in, n_res, start), make)
         d[7] = inter // 16
         inter = _align16(inter + h * size * 3)
         for l, op in enumerate(s.ops):
             ops[b, l] = (op.kind, op.filter, op.iarg, 0, op.factor, op.matrix)
-    tail = pos
     for d, jd, nbytes in jpeg_out:               # the decoded crops: past the host part, on the device only
-        d[1] = jd[21] = tail // 16
-        tail = _align16(tail + nbytes)
-    buf = torch.empty(pos, dtype=torch.uint8)
-    flat = buf.numpy()
-    flat[:desc.nbytes] = desc.reshape(-1).view(np.uint8)
-    flat[ops_offset:ops_offset + ops.nbytes] = ops.reshape(-1).view(np.uint8)
-    for off, a in pieces:
-        flat[off:off + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
+        d[1] = jd[21] = P.device(nbytes)
     jp = (jdesc_offset, njpeg, coef_blocks, plane_bytes) if njpeg else None
-    return PackedClsBatch(buf, B, size, layers, ops_offset // 16, inter, mean, std, fill, jp, tail)
+    return PackedClsBatch(*P.buffer(), B, size, layers, ops_offset, inter, mean, std, fill, jp)
 
 
 def cls_fallback_reason(is_train, args):

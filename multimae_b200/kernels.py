@@ -136,10 +136,11 @@ AUGMENT_KINDS = {"rgb": 0, "depth": 1, "semseg": 2, "semseg_coco": 2}     # task
 
 
 def augment_batch(host, dev, tasks, batch, size, map4, scratch_bytes, mean, std):
-    """Resample one packed batch (multimae_b200.data.pack_batch: `host` its uint8 host buffer, `dev` the device copy) on
-    the current stream: {task: fp32 [B,3,S,S] (rgb) | fp32 [B,1,S,S] (depth) | int64 [B,S/4,S/4] (semseg)}."""
+    """Resample one packed batch (multimae_b200.data.pack_batch: `host` its uint8 host buffer, `dev` the device buffer,
+    whose first host.numel() bytes are its copy and whose tail holds the decoded crops) on the current stream:
+    {task: fp32 [B,3,S,S] (rgb) | fp32 [B,1,S,S] (depth) | int64 [B,S/4,S/4] (semseg)}."""
     _need_cuda(dev)
-    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() == dev.numel()
+    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() <= dev.numel()
     kinds = [AUGMENT_KINDS[t] for t in tasks]
     T, S = len(tasks), int(size)
     outs = {}
@@ -148,10 +149,10 @@ def augment_batch(host, dev, tasks, batch, size, map4, scratch_bytes, mean, std)
         outs[t] = torch.empty(shape, dtype=torch.int64 if k == 2 else torch.float32, device=dev.device)
     scratch = torch.empty(max(int(scratch_bytes), 16), dtype=torch.uint8, device=dev.device)
     ptrs = (ctypes.c_void_p * T)(*[outs[t].data_ptr() for t in tasks])
-    L.check(L.lib().mmae_augment_batch(host.data_ptr(), dev.data_ptr(), host.numel(), batch, T, (ctypes.c_int * T)(*kinds),
-                                       S, int(map4), scratch.data_ptr(), int(scratch_bytes), ptrs,
-                                       (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std), L.current_stream()),
-            "mmae_augment_batch")
+    L.check(L.lib().mmae_augment_batch(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), batch, T,
+                                       (ctypes.c_int * T)(*kinds), S, int(map4), scratch.data_ptr(), int(scratch_bytes),
+                                       ptrs, (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std),
+                                       L.current_stream()), "mmae_augment_batch")
     return outs
 
 
@@ -178,7 +179,7 @@ def jpeg_subsequence_slots(host, desc_offset, num_images):
 
 
 def jpeg_decode_batch(host, dev, desc_offset, num_images, coef_blocks, plane_bytes):
-    """Decode the JPEG rectangles of one packed classification batch (multimae_b200.data.pack_cls_batch: `host` its
+    """Decode the JPEG rectangles of one packed batch (multimae_b200.data.pack_batch or pack_cls_batch: `host` its
     uint8 host buffer, `dev` the device buffer, whose first host.numel() bytes are its copy) into dev's tail, on the
     current stream.  Returns the scratch (its subsequence records tell which restart intervals the parallel decode
     took)."""
@@ -207,15 +208,11 @@ def png_decode_batch(host, dev, desc_offset, num_images, raw_bytes):
     return status
 
 
-def cls_augment_batch(host, dev, batch, size, layers, ops_offset, inter_bytes, mean, std, fill, jpeg=None):
-    """Resample, flip, RandAugment and normalise one packed classification batch (multimae_b200.data.pack_cls_batch) on
-    the current stream: fp32 [B, 3, S, S].  `jpeg` = (descriptor offset / 16, images, coefficient blocks, plane bytes)
-    first decodes the batch's JPEG rectangles into the device-only tail of `dev` (jpeg_decode_batch)."""
+def cls_augment_batch(host, dev, batch, size, layers, ops_offset, inter_bytes, mean, std, fill):
+    """Resample, flip, RandAugment and normalise one packed classification batch (multimae_b200.data.pack_cls_batch;
+    `host` and `dev` as in augment_batch) on the current stream: fp32 [B, 3, S, S]."""
     _need_cuda(dev)
-    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8
-    assert host.numel() == dev.numel() if jpeg is None else host.numel() <= dev.numel()
-    if jpeg is not None:
-        jpeg_decode_batch(host, dev, *jpeg)
+    assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() <= dev.numel()
     S = int(size)
     out = torch.empty((batch, 3, S, S), dtype=torch.float32, device=dev.device)
     nbytes = cls_scratch_bytes(inter_bytes, batch, S, layers)

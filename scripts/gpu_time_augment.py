@@ -109,11 +109,9 @@ def main():
             packed = crop.collate([gpu_ds[k % len(gpu_ds)] for k in range(B)])[0]
             host = packed.buffer.pin_memory()
             devbuf = host.to(dev)
-            from multimae_b200 import kernels
 
-            def call():
-                return kernels.augment_batch(host, devbuf, packed.tasks, packed.batch, packed.size, packed.map4,
-                                             packed.scratch_bytes, packed.mean, packed.std)
+            def call():                      # the resampling kernels alone, on the uploaded buffer
+                return packed.resample(host, devbuf)
             for _ in range(5):
                 call()
             torch.cuda.synchronize()

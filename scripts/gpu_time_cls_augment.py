@@ -110,12 +110,9 @@ def main():
             packed, _ = ds.transform.collate([ds[k] for k in range(128)])
             host = packed.buffer.pin_memory()
             devbuf = host.to(dev)
-            from multimae_b200 import kernels
 
-            def call():
-                return kernels.cls_augment_batch(host, devbuf, packed.batch, packed.size, packed.layers,
-                                                 packed.ops_offset, packed.inter_bytes, packed.mean, packed.std,
-                                                 packed.fill)
+            def call():                      # the resampling kernels alone, on the uploaded buffer
+                return packed.resample(host, devbuf)
             for _ in range(5):
                 call()
             torch.cuda.synchronize()

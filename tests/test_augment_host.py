@@ -268,7 +268,7 @@ def test_depth_that_is_not_16_bit_is_refused():
 
 
 # ---- 5. C ABI ------------------------------------------------------------------------------------------------------
-def test_entry_point_validates_before_any_launch():
+def test_entry_point_validates_host_part_and_tail_before_any_launch():
     lib = L.lib()
     S = 64
     crops = [D.Crops({"rgb": np.zeros((20, 30, 3), np.uint8), "depth": np.zeros((20, 30), np.uint16),
@@ -277,10 +277,11 @@ def test_entry_point_validates_before_any_launch():
     good = pb.buffer.clone()
     base = 1 << 20                 # fake, 16-byte aligned device addresses: nothing is launched
 
-    def call(buf=None, nbytes=None, batch=1, T=3, kinds=(0, 1, 2), size=S, map4=None, scratch=base, sbytes=None,
-             outs=(base, base, base), mean=AO.DEFAULT_MEAN, std=AO.DEFAULT_STD, dev=base):
+    def call(buf=None, hbytes=None, pbytes=None, batch=1, T=3, kinds=(0, 1, 2), size=S, map4=None, scratch=base,
+             sbytes=None, outs=(base, base, base), mean=AO.DEFAULT_MEAN, std=AO.DEFAULT_STD, dev=base):
         buf = good if buf is None else buf
-        return lib.mmae_augment_batch(buf.data_ptr(), dev, buf.numel() if nbytes is None else nbytes, batch, T,
+        return lib.mmae_augment_batch(buf.data_ptr(), dev, buf.numel() if hbytes is None else hbytes,
+                                      buf.numel() if pbytes is None else pbytes, batch, T,
                                       (ctypes.c_int * len(kinds))(*kinds), size, pb.map4 if map4 is None else map4,
                                       scratch, pb.scratch_bytes if sbytes is None else sbytes,
                                       (ctypes.c_void_p * len(outs))(*outs), (ctypes.c_float * 3)(*mean),
@@ -298,7 +299,9 @@ def test_entry_point_validates_before_any_launch():
         (dict(T=9, kinds=(0,) * 9, outs=(base,) * 9), "task count"),
         (dict(size=2), "output size"),
         (dict(dev=base + 4), "16-byte aligned"),
-        (dict(nbytes=64), "cannot hold"),
+        (dict(hbytes=64), "cannot hold"),
+        (dict(pbytes=good.numel() - 16), "host part"),
+        (dict(hbytes=int(rgb_desc[0, 5]) * 16), "table offset out of range"),      # a table in the device tail
         (dict(kinds=(0, 1, 3)), "bad kind"),
         (dict(kinds=(1, 0, 2)), "kind"),
         (dict(outs=(base, 0, base)), "output pointer"),
@@ -309,6 +312,7 @@ def test_entry_point_validates_before_any_launch():
         (dict(buf=patched(d0 + 8, 0)), "bad crop"),
         (dict(buf=patched(d0 + 16, 2)), "flip"),
         (dict(buf=patched(d0 + 4, (good.numel() // 16))), "crop outside"),
+        (dict(buf=patched(d0 + 4, (good.numel() // 16)), pbytes=good.numel() + 1024), "crop outside"),  # past the tail
         (dict(buf=patched(d0 + 12, 31)), "expected"),
         (dict(buf=patched(rgb_desc[0, 5] * 16 + 16, 29)), "taps"),
         (dict(buf=patched(rgb_desc[2, 5] * 16 + 16, 30)), "nearest index"),

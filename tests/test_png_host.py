@@ -163,7 +163,7 @@ def _states():
     return random.getstate(), np.random.get_state()[1].tobytes(), torch.get_rng_state()
 
 
-def test_loader_makes_the_same_draws_and_packs_the_streams(tmp_path):
+def test_loader_makes_the_same_draws_and_packs_the_tables_in_the_host_part(tmp_path):
     _write_tree(str(tmp_path), np.random.default_rng(0))
     sys.path.insert(0, STANDIN)
     try:
@@ -215,7 +215,7 @@ def test_loader_makes_the_same_draws_and_packs_the_streams(tmp_path):
                     assert packed.png_files[k][:3] == (src.path, task, d[12] * 16)
                     k += 1
         assert k == packed.png[1]
-        assert int(desc[..., 5:7].max()) * 16 < packed.check_bytes            # the tables lie in the checked part
+        assert int(desc[..., 5:7].max()) * 16 < packed.buffer.numel()         # the tables lie in the host part
     finally:
         sys.path.remove(STANDIN)
         for m in [m for m in sys.modules if m == "utils" or m.startswith("utils.")]:
