@@ -35,7 +35,8 @@ int64_t mmae_launch_count(void);
  * recorded events and returns the summed algorithmic FLOPs (2*M*N*K), summed kernel milliseconds and launch count. */
 int mmae_profile_gemm(int enable);
 int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launches);
-/* text dump, one line per recorded launch: "M N K flags ms" (flags: bit0 A MN-major, bit1 B MN-major, bits 8+ split_k) */
+/* text dump, one line per recorded launch: "M N K flags ms" (flags: bit0 A MN-major, bit1 B MN-major, bit2 ping-pong
+ * kernel (variant 7), bits 8+ split_k) */
 int64_t mmae_profile_gemm_dump(char* buf_host, int64_t capacity);
 
 /* ------------------------------------------------------------------------------------------------
@@ -75,8 +76,9 @@ typedef struct mmae_gemm_epilogue {
 } mmae_gemm_epilogue;
 
 /* Kernel variant for measurements: -1 = heuristic (default), 0 / 1 / 3 / 2 = one CTA per 128 x 64 / 128 / 192 / 256
- * tile, 6 / 5 / 4 = two-CTA cluster per 256 x 128 / 192 / 256 tile (the B tile loaded once and multicast to both CTAs).
- * Env MMAE_GEMM_VARIANT sets the initial value. */
+ * tile, 6 / 5 / 4 = two-CTA cluster per 256 x 128 / 192 / 256 tile (the B tile loaded once and multicast to both CTAs),
+ * 7 = one CTA per SM whose two consumer warpgroups each own whole 128 x 128 tiles and take turns on the tensor cores
+ * (ping-pong).  Env MMAE_GEMM_VARIANT sets the initial value. */
 int mmae_gemm_set_variant(int variant);
 /* 1 (default): plain bf16 / fp32 outputs (optionally with bias / GELU) leave through shared memory + TMA tile stores, fp32
  * accumulation (split-K, accumulate) through TMA reduce-add tiles; 0: per-thread global stores / red.global adds.

@@ -8,10 +8,16 @@
 //   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled shared-memory ring, mbarrier
 //                    complete_tx); gives its registers to the consumers (setmaxnreg).  Ring slot and phase follow a
 //                    k-block count that runs across work items, so the next item's stages load during an epilogue.
-//   warpgroups 1-2 : consumers, 64 rows of the tile each: wgmma 64 x BN x 16 straight from the ring (K-major or MN-major
-//                    operands through the descriptor's transpose bit), then the fused epilogue from the accumulator
-//                    registers (bias / GELU / dGELU / residual, bf16 and fp32 outputs, red.global adds for split-K), or
-//                    for plain bf16 / fp32 outputs through a staging area of its own and TMA tile stores / reduce-adds
+//   warpgroups 1-2 : consumers: wgmma 64 x BN x 16 straight from the ring (K-major or MN-major operands through the
+//                    descriptor's transpose bit), then the fused epilogue from the accumulator registers (bias / GELU /
+//                    dGELU / residual, bf16 and fp32 outputs, red.global adds for split-K), or for plain bf16 / fp32
+//                    outputs through a staging area of their own and TMA tile stores / reduce-adds.  Two schemes:
+//     cooperative (gemm_bf16_kernel): both consumers work on every item, 64 rows each, and run its epilogue together
+//                    while the tensor cores idle.
+//     ping-pong (gemm_bf16_pingpong_kernel, BN = 128, one CTA): consumer i owns the CTA's items i, i + 2, ..., all 128
+//                    rows, and the two take turns on the mainloop, so one's epilogue runs under the other's MMAs.
+//                    ptxas: 168 registers per thread (the consumers raise theirs to 232), no spills; 230,656 bytes of
+//                    dynamic shared memory (6 x 32 KB stages + 2 x 16 KB staging), GemmCfg<128>'s.
 // CL = 2: a cluster of two CTAs along M shares the B tile - each CTA loads half of it and multicasts it to both, so a
 // 256 x BN output tile reads B from L2 once.  Both CTAs walk the same item sequence (one M-half each), so their rings
 // stay in lockstep; a stage is refilled only after the consumers of BOTH CTAs released it.
@@ -127,6 +133,160 @@ __device__ __forceinline__ void stage_pair(uint8_t* box, int r, int c, float v0,
   else *reinterpret_cast<uint32_t*>(b + r * 32 + c) = pack_bf16x2(v0, v1);
 }
 
+// TMA producer (one thread): walks the CTA's items in order and fills the ring; slot and phase follow a k-block count
+// that runs across items, so the next item's stages load while the consumers finish the current one
+template <int BN, int CL, bool A_MN, bool B_MN>
+__device__ __forceinline__ void produce(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, const CUtensorMap* tmA,
+                                        const CUtensorMap* tmB, const GemmParams& p, int rank, int first_item,
+                                        int item_stride, int num_items) {
+  using C = GemmCfg<BN>;
+  constexpr int STAGES = C::STAGES;
+  constexpr int BH = BN / CL;   // B rows (output columns) this CTA loads
+  static_assert(!B_MN || BH % 64 == 0, "MN-major B is loaded in 64-column chunks");
+  uint32_t it = 0;   // k-blocks loaded so far, over all items
+  for (int item = first_item; item < num_items; item += item_stride) {
+    const WorkItem w = decode_item<BN, CL>(item, p, rank);
+    for (int kb = 0; kb < w.nkb; ++kb, ++it) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait(&empty_bar[s], ph ^ 1u);
+      mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
+      uint8_t* sA = smem + s * C::STAGE_BYTES;
+      uint8_t* sB = sA + C::A_BYTES;
+      const int k0 = (w.kb_begin + kb) * BK;
+      if constexpr (!A_MN) {
+        tma_load_2d(sA, tmA, &full_bar[s], k0, w.m0);
+      } else {
+#pragma unroll
+        for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * (64 * BK * 2), tmA, &full_bar[s], w.m0 + c * 64, k0);
+      }
+      if constexpr (CL == 1) {
+        if constexpr (!B_MN) {
+          tma_load_2d(sB, tmB, &full_bar[s], k0, w.n0);
+        } else {
+#pragma unroll
+          for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), tmB, &full_bar[s], w.n0 + c * 64, k0);
+        }
+      } else {
+        if constexpr (!B_MN) {
+          tma_load_2d_multicast(sB + rank * BH * 128, tmB, &full_bar[s], k0, w.n0 + rank * BH, 0x3);
+        } else {
+#pragma unroll
+          for (int c = 0; c < BH / 64; ++c)
+            tma_load_2d_multicast(sB + (rank * (BH / 64) + c) * (64 * BK * 2), tmB, &full_bar[s],
+                                  w.n0 + rank * BH + c * 64, k0, 0x3);
+        }
+      }
+    }
+  }
+}
+
+// One k-block of MMAs for 64 rows of the tile: BK / 16 wgmma 64 x BN x 16 straight from ring stage `stage`, the rows
+// starting `slab` x 64 into its A tile.  `first`: the item's first k-block, whose first wgmma overwrites the accumulators.
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], const uint8_t* stage, int slab, bool first) {
+  const uint32_t a_addr = smem_u32(stage) + slab * (64 * BK * 2);
+  const uint32_t b_addr = smem_u32(stage) + GemmCfg<BN>::A_BYTES;
+#pragma unroll
+  for (int j = 0; j < BK / WG_K; ++j) {
+    const uint32_t sd = (first && j == 0) ? 0u : 1u;
+    // K-major : advance 16 elements (32 B) inside the 128 B swizzle row; a 64-row slab starts 8 KB in
+    // MN-major: advance 16 k-rows of 128 B; 64-element M/N chunks are (64 * BK * 2) bytes apart
+    const uint64_t da = A_MN ? gmma_desc_sw128(a_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
+                             : gmma_desc_sw128(a_addr + j * (WG_K * 2), 16, 1024);
+    const uint64_t db = B_MN ? gmma_desc_sw128(b_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
+                             : gmma_desc_sw128(b_addr + j * (WG_K * 2), 16, 1024);
+    if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+    else if constexpr (BN == 192) wgmma_m64n192k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+    else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+    else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+  }
+}
+
+// Fused epilogue of 64 rows x BN columns of an item's output, rows [row0, row0 + 64) and columns [n0, n0 + BN), from
+// the accumulators of one consumer warpgroup (thread t of 128).  With p.tma_store, one 64 x 32 box at a time through the
+// warpgroup's staging area `epi` (16 KB: four bf16 or two fp32 boxes in turn, `boxes` counts the boxes it issued) and
+// named barrier `bar`; otherwise straight from the registers.
+template <int BN>
+__device__ __forceinline__ void epilogue_slab(const float (&acc)[BN / 2], int row0, int n0, bool first_split,
+                                              const GemmParams& p, const CUtensorMap* tmC, uint8_t* epi,
+                                              uint32_t& boxes, int bar, int t) {
+  constexpr int EPI_BOX_BYTES = GemmCfg<BN>::EPI_BOX_BYTES;
+  const int rl = (t >> 5) * 16 + ((t & 31) >> 2);       // this thread's first row within the 64
+  if (p.tma_store) {
+    const float* bias = first_split ? p.ep.bias : nullptr;
+    const bool bf16_out = p.tma_store == 1;
+    // The bias of box b + 1 is loaded while box b is staged, so its latency is paid once per item rather than once per
+    // box behind the two named barriers.  Loaded inside the box, it made the encoder's fc1 forward (12672 x 3072 x 768,
+    // 128 x 256 tiles) take 129 us against 110 us for the fc2 dgrad of the same shape without a bias; loaded ahead, 113
+    // us (scripts/gpu_time_gemm.py, H100 SXM, 700 W power limit).
+    float2 bias_cur[4] = {}, bias_next[4] = {};
+    auto load_bias = [&](int b, float2 (&dst)[4]) {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int col = n0 + b * 32 + jj * 8 + 2 * (t & 3);
+        if (bias && col < p.N) dst[jj] = __ldg(reinterpret_cast<const float2*>(bias + col));
+      }
+    };
+    load_bias(0, bias_cur);
+#pragma unroll
+    for (int b = 0; b < BN / 32; ++b) {
+      if (n0 + b * 32 >= p.N) break;   // whole boxes right of N are neither staged nor stored
+      if (b + 1 < BN / 32) load_bias(b + 1, bias_next);
+      uint8_t* box = bf16_out ? epi + (boxes & 3) * (EPI_BOX_BYTES / 2) : epi + (boxes & 1) * EPI_BOX_BYTES;
+      if (t == 0) {   // the store that used this buffer last has read it
+        if (bf16_out) bulk_wait_read<3>();
+        else bulk_wait_read<1>();
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * b + jj;
+        const int c = jj * 8 + 2 * (t & 3);   // column within the box
+        float v[4] = {acc[4 * j] * p.ep.alpha, acc[4 * j + 1] * p.ep.alpha, acc[4 * j + 2] * p.ep.alpha,
+                      acc[4 * j + 3] * p.ep.alpha};
+        if (bias && n0 + b * 32 + c < p.N) {
+          const float2 bb = bias_cur[jj];
+          v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
+        }
+        if (p.ep.act == 1) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
+        }
+        if (bf16_out) {
+          stage_pair<bf16>(box, rl, c, v[0], v[1]);
+          stage_pair<bf16>(box, rl + 8, c, v[2], v[3]);
+        } else {
+          stage_pair<float>(box, rl, c, v[0], v[1]);
+          stage_pair<float>(box, rl + 8, c, v[2], v[3]);
+        }
+      }
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+      if (t == 0) {
+        if (p.tma_store == 3) tma_reduce_add_2d(tmC, box, n0 + b * 32, row0);
+        else tma_store_2d(tmC, box, n0 + b * 32, row0);
+        bulk_commit_group();
+      }
+      ++boxes;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) bias_cur[jj] = bias_next[jj];
+    }
+  } else {
+    const bool atomic_out = p.ep.accumulate != 0 || p.splits > 1;
+    const int row_a = row0 + rl;
+    const int row_b = row_a + 8;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (n0 + j * 8 >= p.N) break;   // N % 8 == 0: a column pair is either fully inside or fully outside
+      const int n = n0 + j * 8 + 2 * (t & 3);
+      if (row_a < p.M) epilogue_pair(acc[4 * j], acc[4 * j + 1], row_a, n, p, first_split, atomic_out);
+      if (row_b < p.M) epilogue_pair(acc[4 * j + 2], acc[4 * j + 3], row_b, n, p, first_split, atomic_out);
+    }
+  }
+}
+
+// Cooperative consumers: both warpgroups work on the same item, 64 rows each, and run its epilogue together
 template <int BN, int CL, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -136,8 +296,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   pdl_launch_dependents();   // the wait follows the barrier setup below
   using C = GemmCfg<BN>;
   constexpr int STAGES = C::STAGES;
-  constexpr int BH = BN / CL;   // B rows (output columns) this CTA loads
-  static_assert(!B_MN || BH % 64 == 0, "MN-major B is loaded in 64-column chunks");
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -169,52 +327,14 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
-      uint32_t it = 0;   // k-blocks loaded so far, over all items
-      for (int item = first_item; item < num_items; item += item_stride) {
-        const WorkItem w = decode_item<BN, CL>(item, p, rank);
-        for (int kb = 0; kb < w.nkb; ++kb, ++it) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
-          uint8_t* sA = smem + s * C::STAGE_BYTES;
-          uint8_t* sB = sA + C::A_BYTES;
-          const int k0 = (w.kb_begin + kb) * BK;
-          if constexpr (!A_MN) {
-            tma_load_2d(sA, &tmA, &full_bar[s], k0, w.m0);
-          } else {
-#pragma unroll
-            for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * (64 * BK * 2), &tmA, &full_bar[s], w.m0 + c * 64, k0);
-          }
-          if constexpr (CL == 1) {
-            if constexpr (!B_MN) {
-              tma_load_2d(sB, &tmB, &full_bar[s], k0, w.n0);
-            } else {
-#pragma unroll
-              for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), &tmB, &full_bar[s], w.n0 + c * 64, k0);
-            }
-          } else {
-            if constexpr (!B_MN) {
-              tma_load_2d_multicast(sB + rank * BH * 128, &tmB, &full_bar[s], k0, w.n0 + rank * BH, 0x3);
-            } else {
-#pragma unroll
-              for (int c = 0; c < BH / 64; ++c)
-                tma_load_2d_multicast(sB + (rank * (BH / 64) + c) * (64 * BK * 2), &tmB, &full_bar[s],
-                                      w.n0 + rank * BH + c * 64, k0, 0x3);
-            }
-          }
-        }
-      }
-    }
+    if (threadIdx.x == 0) produce<BN, CL, A_MN, B_MN>(smem, full_bar, empty_bar, &tmA, &tmB, p, rank, first_item,
+                                                      item_stride, num_items);
   } else {
     // ------------------------------------------------------------------ consumers (warpgroups 1, 2)
     setmaxnreg_inc<232>();
     const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
     const int t = threadIdx.x & 127;
-    const int rl = (t >> 5) * 16 + ((t & 31) >> 2);       // this thread's first row within the warpgroup's 64
     uint8_t* epi = smem + C::EPI_OFFSET + cw * (2 * C::EPI_BOX_BYTES);
-    const bool atomic_out = p.ep.accumulate != 0 || p.splits > 1;
     uint32_t it = 0;       // k-blocks consumed so far, over all items
     uint32_t boxes = 0;    // TMA-store boxes issued so far by this warpgroup
     // frees ring stage `s` in this CTA and, for a cluster, in the peer whose multicast also fills it
@@ -233,25 +353,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[s], ph);
-        const uint32_t a_addr = smem_u32(smem + s * C::STAGE_BYTES) + cw * (64 * BK * 2);
-        const uint32_t b_addr = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
         wgmma_fence();
-#pragma unroll
-        for (int j = 0; j < BK / WG_K; ++j) {
-          const uint32_t sd = (kb | j) != 0 ? 1u : 0u;
-          // K-major : advance 16 elements (32 B) inside the 128 B swizzle row; this warpgroup's 64 rows start 8 KB in
-          // MN-major: advance 16 k-rows of 128 B; 64-element M/N chunks are (64 * BK * 2) bytes apart
-          const uint64_t da = A_MN ? gmma_desc_sw128(a_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
-                                   : gmma_desc_sw128(a_addr + j * (WG_K * 2), 16, 1024);
-          const uint64_t db = B_MN ? gmma_desc_sw128(b_addr + j * (WG_K * 128), 64 * BK * 2, 1024)
-                                   : gmma_desc_sw128(b_addr + j * (WG_K * 2), 16, 1024);
-          if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-          else if constexpr (BN == 192) wgmma_m64n192k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-          else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-          else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-        }
+        mma_kblock<BN, A_MN, B_MN>(acc, smem + s * C::STAGE_BYTES, cw, kb == 0);
         wgmma_commit();
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
@@ -262,65 +367,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
       release((it - 1) % STAGES);   // the producer refills it with the next item's operands during the epilogue
-
-      const int row_a = w.m0 + cw * 64 + rl;
-      const int row_b = row_a + 8;
-      const bool first_split = w.split == 0;
-      if (p.tma_store) {
-        // -------------------------------------------------------------- epilogue through shared memory + TMA, one
-        // 64 x 32 box at a time through the warpgroup's staging area: 4 bf16 or 2 fp32 boxes in turn
-        const float* bias = first_split ? p.ep.bias : nullptr;
-        const bool bf16_out = p.tma_store == 1;
-#pragma unroll
-        for (int b = 0; b < BN / 32; ++b) {
-          if (w.n0 + b * 32 >= p.N) break;   // whole boxes right of N are neither staged nor stored
-          uint8_t* box = bf16_out ? epi + (boxes & 3) * (C::EPI_BOX_BYTES / 2) : epi + (boxes & 1) * C::EPI_BOX_BYTES;
-          if (t == 0) {   // the store that used this buffer last has read it
-            if (bf16_out) bulk_wait_read<3>();
-            else bulk_wait_read<1>();
-          }
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int j = 4 * b + jj;
-            const int c = jj * 8 + 2 * (t & 3);   // column within the box
-            float v[4] = {acc[4 * j] * p.ep.alpha, acc[4 * j + 1] * p.ep.alpha, acc[4 * j + 2] * p.ep.alpha,
-                          acc[4 * j + 3] * p.ep.alpha};
-            if (bias && w.n0 + b * 32 + c < p.N) {
-              const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + w.n0 + b * 32 + c));
-              v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
-            }
-            if (p.ep.act == 1) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
-            }
-            if (bf16_out) {
-              stage_pair<bf16>(box, rl, c, v[0], v[1]);
-              stage_pair<bf16>(box, rl + 8, c, v[2], v[3]);
-            } else {
-              stage_pair<float>(box, rl, c, v[0], v[1]);
-              stage_pair<float>(box, rl + 8, c, v[2], v[3]);
-            }
-          }
-          fence_proxy_async_smem();
-          asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
-          if (t == 0) {
-            if (p.tma_store == 3) tma_reduce_add_2d(&tmC, box, w.n0 + b * 32, w.m0 + cw * 64);
-            else tma_store_2d(&tmC, box, w.n0 + b * 32, w.m0 + cw * 64);
-            bulk_commit_group();
-          }
-          ++boxes;
-        }
-      } else {
-        // -------------------------------------------------------------- epilogue straight from the accumulator registers
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          if (w.n0 + j * 8 >= p.N) break;   // N % 8 == 0: a column pair is either fully inside or fully outside
-          const int n = w.n0 + j * 8 + 2 * (t & 3);
-          if (row_a < p.M) epilogue_pair(acc[4 * j], acc[4 * j + 1], row_a, n, p, first_split, atomic_out);
-          if (row_b < p.M) epilogue_pair(acc[4 * j + 2], acc[4 * j + 3], row_b, n, p, first_split, atomic_out);
-        }
-      }
+      epilogue_slab<BN>(acc, w.m0 + cw * 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
     }
     if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
   }
@@ -328,11 +375,115 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   if constexpr (CL > 1) cluster_sync_all();
 }
 
-template <int BN, int CL, bool A_MN, bool B_MN>
+// Ping-pong consumers: warpgroup i takes the CTA's items i, i + 2, i + 4, ..., all 128 rows of each (two 64-row slabs of
+// MMAs per k-step, 2 x BN / 2 accumulators per thread).  Named barriers 4 and 5 make the two take turns on the
+// mainloop: warpgroup 1 starts an item's MMAs once warpgroup 0 has issued the last of its item's, and the other way
+// round, so one warpgroup's epilogue runs while the other's MMAs keep the tensor cores busy.  The ring is the
+// cooperative kernel's, filled in the same order, but each stage has one consumer: its empty barrier takes 1 arrival.
+// Each slab sees the same wgmma sequence and epilogue as the cooperative kernel's warpgroup for it, so the two kernels'
+// outputs are bitwise equal.
+template <int BN, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                              const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+  pdl_launch_dependents();   // as in gemm_bf16_kernel
+  using C = GemmCfg<BN>;
+  constexpr int STAGES = C::STAGES;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int wg = threadIdx.x >> 7;
+  const int num_items = p.tiles_n * p.tiles_m * p.splits;
+  const int first_item = blockIdx.x;
+  const int item_stride = gridDim.x;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    if (p.tma_store) tma_prefetch_desc(&tmC);
+#pragma unroll
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 1);   // released by the one warpgroup whose item the stage holds
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) produce<BN, 1, A_MN, B_MN>(smem, full_bar, empty_bar, &tmA, &tmB, p, 0, first_item,
+                                                     item_stride, num_items);
+  } else {
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;                 // takes the CTA's items cw, cw + 2, ...
+    const int t = threadIdx.x & 127;
+    uint8_t* epi = smem + C::EPI_OFFSET + cw * (2 * C::EPI_BOX_BYTES);
+    uint32_t it = 0;       // k-blocks of the CTA's items before the current one
+    uint32_t boxes = 0;    // TMA-store boxes issued so far by this warpgroup
+    float acc[2][BN / 2];  // rows [0, 64) and [64, 128) of the tile
+
+    int j = 0;   // the item's place in the CTA's sequence
+    for (int item = first_item; item < num_items; item += item_stride, ++j) {
+      const WorkItem w = decode_item<BN, 1>(item, p, 0);
+      if ((j & 1) != cw) {   // the other warpgroup's item: its k-blocks pass through the ring before our next one
+        it += w.nkb;
+        continue;
+      }
+      // our turn on the tensor cores: the other warpgroup has issued the MMAs of the item before this one
+      if (j > 0) asm volatile("bar.sync %0, 256;" ::"r"(4 + cw) : "memory");
+      for (int kb = 0; kb < w.nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) {
+          reg_fence(acc[0][i]);
+          reg_fence(acc[1][i]);
+        }
+        wgmma_fence();
+        mma_kblock<BN, A_MN, B_MN>(acc[0], smem + s * C::STAGE_BYTES, 0, kb == 0);
+        mma_kblock<BN, A_MN, B_MN>(acc[1], smem + s * C::STAGE_BYTES, 1, kb == 0);
+        wgmma_commit();
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) {
+          reg_fence(acc[0][i]);
+          reg_fence(acc[1][i]);
+        }
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+        if (kb > 0 && t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      }
+      // hand the tensor cores to the other warpgroup's next item (the one after this), if the CTA has one
+      if (item + item_stride < num_items) asm volatile("bar.arrive %0, 256;" ::"r"(5 - cw) : "memory");
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) {
+        reg_fence(acc[0][i]);
+        reg_fence(acc[1][i]);
+      }
+      if (t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      epilogue_slab<BN>(acc[0], w.m0, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
+      epilogue_slab<BN>(acc[1], w.m0 + 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
+    }
+    if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
+  }
+}
+
+// PP: the ping-pong kernel (CL = 1), else the cooperative one
+template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                 cudaStream_t stream) {
+  static_assert(!PP || CL == 1, "the ping-pong kernel runs single CTAs");
   using C = GemmCfg<BN>;
-  auto kern = gemm_bf16_kernel<BN, CL, A_MN, B_MN>;
+  auto kern = [] {
+    if constexpr (PP) return gemm_bf16_pingpong_kernel<BN, A_MN, B_MN>;
+    else return gemm_bf16_kernel<BN, CL, A_MN, B_MN>;
+  }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(GEMM_THREADS);
@@ -366,7 +517,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   const int slots = std::min(resident, std::max(1, sm_count() / CL));
   cfg.gridDim = dim3(std::min(items, slots) * CL);
   const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K,
-                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (p.splits << 8));
+                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (p.splits << 8));
   if constexpr (CL == 1) {
     cfg.attrs = attr + 1;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
@@ -389,7 +540,7 @@ using namespace mmae;
 static int g_gemm_variant = []() {
   const char* e = getenv("MMAE_GEMM_VARIANT");
   const int v = e ? atoi(e) : -1;
-  return v >= -1 && v <= 6 ? v : -1;
+  return v >= -1 && v <= 7 ? v : -1;
 }();
 static int g_gemm_tma_store = []() {
   const char* e = getenv("MMAE_GEMM_TMA_STORE");
@@ -397,7 +548,7 @@ static int g_gemm_tma_store = []() {
 }();
 
 extern "C" int mmae_gemm_set_variant(int variant) {
-  MMAE_CHECK(variant >= -1 && variant <= 6, MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1 .. 6)", variant);
+  MMAE_CHECK(variant >= -1 && variant <= 7, MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1 .. 7)", variant);
   g_gemm_variant = variant;
   return MMAE_OK;
 }
@@ -408,15 +559,25 @@ extern "C" int mmae_gemm_set_tma_store(int enable) {
 }
 
 // variant -> tile: 0 / 1 / 3 / 2 = one CTA, BN = 64 / 128 / 192 / 256; 6 / 5 / 4 = two-CTA cluster (256-row tile, B shared
-// by multicast), BN = 128 / 192 / 256
-static int variant_bn(int v) { return v == 0 ? 64 : (v == 1 || v == 6) ? 128 : (v == 3 || v == 5) ? 192 : 256; }
+// by multicast), BN = 128 / 192 / 256; 7 = one CTA of ping-pong consumers, BN = 128
+static int variant_bn(int v) { return v == 0 ? 64 : (v == 1 || v == 6 || v == 7) ? 128 : (v == 3 || v == 5) ? 192 : 256; }
+static int variant_cl(int v) { return v >= 4 && v <= 6 ? 2 : 1; }
 
 // Fixed cost of one work item in the persistent kernel, in k-block times of its tile: its epilogue and the hand-over to
 // the next item.  scripts/gpu_time_gemm.py --fixed-cost measured 13.4, 14.0, 10.0 and 5.0 us per extra 128 x 256 fp32
 // reduce-add item at 2, 4, 8 and 12 items per SM, against 0.9 us per k-block (H100 SXM, 700 W power limit): 15 falling to
 // 5.5 k-block times as items per SM grow.  The model takes 4, near the low end, where the long-K weight gradients run;
 // 5 or more would cut fc1 / fc2's weight gradient to 5 splits of 40 k-blocks in 3 rounds, 4 keeps 9 splits of 22 in 5.
+// bf16-output items with a bias (N = 768, 3 to 12 items per SM, same card and limit) cost more: 128 x 128 tiles 9.5
+// (K = 256) and 10.3 (K = 768) k-block times of 0.353 us, 128 x 256 tiles 11.0 and 8.4 of 0.686 us.  (Measured while the
+// TMA epilogue still loaded the bias inside each staged box: see epilogue_slab.)
 constexpr int KB_PER_ITEM_FIXED = 4;
+// The ping-pong kernel (variant 7) hides part of that behind the other warpgroup's MMAs: measured as above, its 128 x 128
+// items cost 8.7 k-block times of 0.337 us past their own k-blocks at K = 256 and at K = 768 (4.29 and 6.99 us per item
+// against the cooperative 128 x 128 kernel's 4.77 and 7.87 us).  In the bench step (same card and limit) it ran the
+// decoders' bf16 forward GEMMs with N >= 768 at K = 256 4-5 % faster than the cooperative tiles, but the N = 256 and
+// dgrad (MN-major B) shapes 10-48 % slower, and the step as a whole slower than with the 128 x 192 tile alone; so the
+// model does not pick it, and variant 7 runs only when set.
 // Split-K never cuts an item below this many k-blocks, which bounds the fp32 reduce-add traffic it adds
 constexpr int MIN_KB_PER_SPLIT = 16;
 
@@ -438,19 +599,20 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time (clusters:
   // sm_count() / 2 items of 256 rows), so a launch lasts ceil(items / slots) rounds of one item, and an item costs
   // ~(k-blocks + KB_PER_ITEM_FIXED) k-block times.  A k-block of a 128 x BN tile costs ~(BN + 40): the A tile's loads
-  // and MMA issue do not shrink with BN, which makes BN = 256 the better tile whenever its rounds are as full.  The
-  // automatic split (split_k
-  // <= 0) fills the last round of the long-K weight gradients instead of leaving it mostly idle.  An explicit variant
-  // fixes the tile, an explicit split_k the split.
+  // and MMA issue do not shrink with BN, which makes wide tiles the better choice whenever their rounds are as full.
+  // 128 x 192 wins where its rounds are fuller: the encoder's N = 768 GEMMs make 99 x 4 = 396 tiles, exactly three
+  // rounds of 132 SMs, against 297 of 128 x 256 in 2.25.  The automatic split (split_k <= 0) fills the last round of the
+  // long-K weight gradients instead of leaving it mostly idle.  An explicit variant fixes the tile, an explicit split_k
+  // the split.
   int variant = g_gemm_variant;
   {
-    const int cand_var[2] = {1, 2};
-    const int nvar = variant >= 0 ? 1 : 2;
+    const int cand_var[3] = {1, 2, 3};
+    const int nvar = variant >= 0 ? 1 : 3;
     long best_cost = -1;
     int best_split = 1, best_var = variant >= 0 ? variant : 1;
     for (int i = 0; i < nvar; ++i) {
       const int v = variant >= 0 ? variant : cand_var[i];
-      const int bn = variant_bn(v), cl = v >= 4 ? 2 : 1;
+      const int bn = variant_bn(v), cl = variant_cl(v);
       if (variant < 0 && bn > 128 && N < bn) continue;
       const long tiles = long(ceil_div(tm, cl)) * ceil_div(N, bn);
       const int slots = std::max(1, sms / cl);
@@ -487,7 +649,7 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
 
   if (variant == 5 && b_mn_major) variant = 4;   // an MN-major B half must be whole 64-column chunks
   const int BNsel = variant_bn(variant);
-  const int CLsel = variant >= 4 ? 2 : 1;
+  const int CLsel = variant_cl(variant);
 
   CUtensorMap tmA, tmB;
   int rc;
@@ -529,22 +691,23 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     }
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-#define MMAE_DISPATCH(BN_, CL_)                                                                      \
-  do {                                                                                               \
-    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false>(tmA, tmB, tmC, p, st); \
-    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, CL_, false, true>(tmA, tmB, tmC, p, st);   \
-    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, true, false>(tmA, tmB, tmC, p, st);   \
-    return launch_gemm<BN_, CL_, true, true>(tmA, tmB, tmC, p, st);                                  \
+#define MMAE_DISPATCH(BN_, CL_, PP_)                                                                      \
+  do {                                                                                                    \
+    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false, PP_>(tmA, tmB, tmC, p, st); \
+    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, CL_, false, true, PP_>(tmA, tmB, tmC, p, st);   \
+    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, true, false, PP_>(tmA, tmB, tmC, p, st);   \
+    return launch_gemm<BN_, CL_, true, true, PP_>(tmA, tmB, tmC, p, st);                                  \
   } while (0)
-  if (variant == 4) MMAE_DISPATCH(256, 2);
-  if (variant == 6) MMAE_DISPATCH(128, 2);
+  if (variant == 4) MMAE_DISPATCH(256, 2, false);
+  if (variant == 6) MMAE_DISPATCH(128, 2, false);
   if (variant == 5) {
     if (!a_mn_major) return launch_gemm<192, 2, false, false>(tmA, tmB, tmC, p, st);
     return launch_gemm<192, 2, true, false>(tmA, tmB, tmC, p, st);
   }
-  if (variant == 0) MMAE_DISPATCH(64, 1);
-  if (variant == 3) MMAE_DISPATCH(192, 1);
-  if (variant == 2) MMAE_DISPATCH(256, 1);
-  MMAE_DISPATCH(128, 1);
+  if (variant == 0) MMAE_DISPATCH(64, 1, false);
+  if (variant == 3) MMAE_DISPATCH(192, 1, false);
+  if (variant == 2) MMAE_DISPATCH(256, 1, false);
+  if (variant == 7) MMAE_DISPATCH(128, 1, true);
+  MMAE_DISPATCH(128, 1, false);
 #undef MMAE_DISPATCH
 }

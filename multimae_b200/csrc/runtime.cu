@@ -272,7 +272,8 @@ extern "C" int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launch
   return MMAE_OK;
 }
 
-// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bits 8.. split_k); returns bytes written
+// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bit2 ping-pong, bits 8.. split_k); returns
+// bytes written
 extern "C" int64_t mmae_profile_gemm_dump(char* buf, int64_t cap) {
   int64_t off = 0;
   for (size_t i = 0; i < mmae::g_prof.used; ++i) {

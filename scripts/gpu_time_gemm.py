@@ -2,6 +2,7 @@
 
     python scripts/gpu_time_gemm.py               # every distinct GEMM shape / operand-major combination of the step
     python scripts/gpu_time_gemm.py --fixed-cost  # per-tile fixed cost: intercept of time over k-blocks
+    python scripts/gpu_time_gemm.py --variant 7   # the step's shapes on one tile variant (mmae_gemm_set_variant)
 
 Shapes: encoder M = 128 x 99 tokens (D 768, MLP 3072), decoders M = 128 x 196 query tokens and 128 x 99 context tokens
 (D 256, MLP 1024), with the epilogue each call has in the step: forward = bf16 out + bias, dgrad = bf16 out with an
@@ -12,7 +13,9 @@ dense BF16 rate (989 TFLOP/s).
 --fixed-cost times one 128 x 256 output tile per SM over 96 k-blocks (fp32 reduce-add output), cut into 1, 2, 4, 8 and
 12 split-K work items per SM.  The MMA work stays the same, so the time added per extra item is the fixed cost of one
 item: its epilogue, its reduce-add traffic and the hand-over between items.  (One tile per SM at K = 64 against K = 768
-does not isolate it: at K = 64 a tile's output write takes longer than its one k-block of MMAs.)"""
+does not isolate it: at K = 64 a tile's output write takes longer than its one k-block of MMAs.)  It then times
+bf16-output items with a bias, as the forward GEMMs run them, at K = 256 and 768 for each tile of VARIANT_BN
+(fixed_cost_bf16)."""
 import argparse
 import os
 import subprocess
@@ -46,6 +49,7 @@ SHAPES = [
     ("dec", "context proj wgrad", 1024, 768, DC, "wgrad"),
 ]
 PEAK_TFLOPS = 989.0
+VARIANT_BN = {1: 128, 2: 256, 7: 128}   # variants timed by --fixed-cost (7: ping-pong): their output tile width
 
 
 def timed(fn, n=50):
@@ -84,8 +88,9 @@ def gemm_call(dev, M, N, K, kind):
     return lambda: KN.gemm(A, B, a_mn=True, b_mn=True, out_f32=out, accumulate=True, split_k=0)
 
 
-def shapes():
+def shapes(variant):
     dev = torch.device("cuda:0")
+    L.lib().mmae_gemm_set_variant(variant)
     print("%-16s %-26s %6s %5s %6s %-5s %9s %7s %6s" % ("class", "gemm", "M", "N", "K", "kind", "us", "TF/s", "%989"))
     for cls, name, M, N, K, kind in SHAPES:
         us = timed(gemm_call(dev, M, N, K, kind))
@@ -113,15 +118,50 @@ def fixed_cost():
     per_item = (t[12] - t[1]) / 11
     print("fixed cost of one work item (128 x 256, fp32 reduce-add epilogue): %.2f us = %.1f k-block times (%.3f us per "
           "k-block)" % (per_item, per_item / kb, kb))
+    fixed_cost_bf16(dev, sms)
+
+
+def fixed_cost_bf16(dev, sms):
+    """bf16-output items (bias, TMA tile store) at N = 768, the encoder's width, so that the n-tiles of one A row block
+    run side by side and read it from L2 as in the step.  Per-item time = slope of the call time over items per SM
+    (3 -> 12); k-block time = slope of the per-item time over K (768 -> 3072); fixed cost = per-item time minus the item's
+    k-blocks at that rate: the epilogue and the hand-over that the tensor cores do not overlap."""
+    N = 768
+    print("%-8s %-7s %5s %10s %12s %12s %12s" % ("variant", "tile", "K", "us/item", "us/k-block", "fixed us", "fixed k-blk"))
+    for variant in sorted(VARIANT_BN):
+        bn = VARIANT_BN[variant]
+        tiles_n = N // bn
+        bias = torch.randn(N, device=dev)
+        L.lib().mmae_gemm_set_variant(variant)
+        try:
+            per_item = {}
+            for K in (256, 768, 3072):
+                B = rnd(dev, N, K)
+                t = {}
+                for n in (3, 12):   # items per SM
+                    assert sms * n % tiles_n == 0
+                    M = 128 * sms * n // tiles_n
+                    A = rnd(dev, M, K)
+                    out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+                    t[n] = timed(lambda: KN.gemm(A, B, bias=bias, out_bf16=out), n=100)
+                    del A, out
+                per_item[K] = (t[12] - t[3]) / 9
+        finally:
+            L.lib().mmae_gemm_set_variant(-1)
+        kb = (per_item[3072] - per_item[768]) / ((3072 - 768) // 64)
+        for K in (256, 768):
+            fixed = per_item[K] - K // 64 * kb
+            print("%-8d %-7s %5d %10.3f %12.3f %12.3f %12.2f" % (variant, "128x%d" % bn, K, per_item[K], kb, fixed, fixed / kb))
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--fixed-cost", action="store_true", help="time the per-tile fixed cost instead of the step's shapes")
+    ap.add_argument("--variant", type=int, default=-1, help="tile variant of every call (-1: the heuristic's choice)")
     a = ap.parse_args()
     torch.manual_seed(0)
     print("# %s (name, power limit, SM clock, max SM clock; before)" % gpu_state())
-    fixed_cost() if a.fixed_cost else shapes()
+    fixed_cost() if a.fixed_cost else shapes(a.variant)
     print("# %s (after)" % gpu_state())
 
 
