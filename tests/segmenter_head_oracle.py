@@ -6,9 +6,11 @@ from functools import partial
 import torch
 import torch.nn.functional as F
 
+import convnext_head_oracle as CX
 from convnext_head_oracle import inputs as _inputs
 from convnext_head_oracle import seg_loss  # noqa: F401  (re-exported: the criterion of run_finetuning_semseg.py)
 from helpers import formula_fill_
+from pretrain_io_oracle import _ln, roundings
 
 # segmenter_head.pt: MultiViT (dim 128, depth 2, 2 heads) on rgb + depth at 48 x 64 (3 x 4 patches), B = 2, with two heads
 # of width 128: 9 classes over both tasks' tokens (depth 2, 4 heads of 32) and 13 classes over rgb (depth 1, 2 heads of 64)
@@ -67,25 +69,57 @@ def block(x, p, q, heads, eps=1e-6, s_attn=None, s_mlp=None):
     return x + (y if s_mlp is None else y * s_mlp.view(B, 1, 1))
 
 
-def cosine_mask(P, C, gamma, beta, eps=1e-6):
+# ----------------------------------------------------------------------------------------------- entry-point parts
+# One function per entry point of segmenter_head.cu (tests/test_cuda_heads.py).  round=True: float64 with a bf16 rounding
+# wherever the kernels store bf16 (pretrain_io_oracle's rf on values, rb on gradient operands): the decoder_norm output
+# Xpc (and its gradient dXpc), patch_proj / classes_proj weights, the projections' bf16 copies the mask kernel multiplies
+# (seg_rownorm_kernel; the row norms come from the fp32 projections) and their gradients dP / dC.  Not mirrored: the mask
+# backward's bf16 Gs = dM rp rc, and its normalise backward formed from the bf16 copies.  The proj GEMM is the ConvNeXt
+# head's (convnext_head_oracle.proj); cls_emb, the class LayerNorm and the upsample are fp32.  round=False: plain float64.
+# mutate="ln_over_patches": the class LayerNorm taken over the patches instead of the classes (the sensitivity checks).
+TAIL_PARAMS = ["dec_w", "dec_b", "patch_w", "classes_w", "mask_w", "mask_b"]     # the C ABI's pointer order
+
+
+def cosine_mask(P, C, gamma, beta, eps=1e-6, round=False, mutate=None):
     """LayerNorm over the classes of the cosine of every (patch, class) pair: P [B, n, E], C [B, K, E] -> [B, n, K]."""
-    Pn = P / P.norm(dim=2, keepdim=True).clamp_min(1e-12)
-    Cn = C / C.norm(dim=2, keepdim=True).clamp_min(1e-12)
-    return F.layer_norm(Pn @ Cn.transpose(1, 2), (C.shape[1],), gamma, beta, eps)
+    rf_, _ = roundings(round)
+    m = (rf_(P) @ rf_(C).transpose(1, 2)) / P.norm(dim=2, keepdim=True).clamp_min(1e-12)
+    m = m / C.norm(dim=2).clamp_min(1e-12).unsqueeze(1)
+    if mutate == "ln_over_patches":
+        return _ln(m.transpose(1, 2), 1.0, 0.0, eps).transpose(1, 2) * gamma + beta
+    return _ln(m, gamma, beta, eps)
+
+
+def proj(enc, w, b, cls_emb, starts, n, round=True):
+    """mmae_segmenter_proj_*: enc [B, N, D] -> seq [B, n + K, E] (patch rows, then cls_emb)"""
+    x = CX.proj(enc, w, b, starts, n, round)
+    return torch.cat([x, cls_emb.expand(x.shape[0], -1, -1)], dim=1)
+
+
+def tail(x, prm, nh, nw, H, W, eps_dec=1e-6, eps_mask=1e-6, round=True, mutate=None, keep=None):
+    """mmae_segmenter_tail_*: x [B, n + K, E] -> [B, K, H, W].  prm: TAIL_PARAMS names.  keep: a dict that receives the
+    projections P, C (retaining their gradients) and the class map m [B, n, K]."""
+    rf_, rb_ = roundings(round)
+    B, n = x.shape[0], nh * nw
+    y = rb_(rf_(_ln(x, prm["dec_w"], prm["dec_b"], eps_dec)))
+    P = rb_(y[:, :n] @ rf_(prm["patch_w"]).t())
+    C = rb_(y[:, n:] @ rf_(prm["classes_w"]).t())
+    m = cosine_mask(P, C, prm["mask_w"], prm["mask_b"], eps_mask, round, mutate)
+    if keep is not None:
+        P.retain_grad()
+        C.retain_grad()
+        keep.update(P=P, C=C, m=m)
+    return CX.upsample(m.transpose(1, 2).reshape(B, -1, nh, nw), H, W)
 
 
 def segmenter_head(enc, p, starts, n, H, W, depth, heads, patch=16, eps=1e-6, prefix="output_adapters.semseg.", scales=None):
     """enc [B, N, D] -> [B, K, H, W]; `starts`: first token of each main task, `n` tokens per task; `scales`: per block
-    (s_attn, s_mlp) or None."""
-    x = torch.cat([enc[:, s0:s0 + n] for s0 in starts], dim=-1)
-    x = x @ p[prefix + "proj_dec.weight"].t() + p[prefix + "proj_dec.bias"]
-    B, K = x.shape[0], p[prefix + "cls_emb"].shape[1]
-    x = torch.cat([x, p[prefix + "cls_emb"].expand(B, -1, -1)], dim=1)
+    (s_attn, s_mlp) or None.  proj -> transformer blocks -> tail."""
+    x = proj(enc, p[prefix + "proj_dec.weight"], p[prefix + "proj_dec.bias"], p[prefix + "cls_emb"][0], starts, n, round=False)
     for i in range(depth):
         sc = scales[i] if scales is not None and scales[i] is not None else (None, None)
         x = block(x, p, "%sblocks.%d." % (prefix, i), heads, eps, *sc)
-    x = F.layer_norm(x, (x.shape[-1],), p[prefix + "decoder_norm.weight"], p[prefix + "decoder_norm.bias"], eps)
-    m = cosine_mask(x[:, :n] @ p[prefix + "patch_proj.weight"].t(), x[:, n:] @ p[prefix + "classes_proj.weight"].t(),
-                    p[prefix + "mask_norm.weight"], p[prefix + "mask_norm.bias"], eps)
-    m = m.transpose(1, 2).reshape(B, K, H // patch, W // patch)
-    return F.interpolate(m, size=(H, W), mode="bilinear", align_corners=False)
+    names = ["decoder_norm.weight", "decoder_norm.bias", "patch_proj.weight", "classes_proj.weight", "mask_norm.weight",
+             "mask_norm.bias"]
+    prm = {k: p[prefix + nm] for k, nm in zip(TAIL_PARAMS, names)}
+    return tail(x, prm, H // patch, W // patch, H, W, eps, eps, round=False)
