@@ -717,13 +717,22 @@ int mmae_jpeg_decode_batch(const void* packed_host, void* packed, int64_t host_b
  * `packed` (packed_bytes, 16-byte aligned) starts with the host_bytes of `packed_host`.  At desc_offset * 16 in it:
  * int32 descriptors [num_images][16] = {width, height, bit depth, colour type, kind, zlib stream / 16 (the IDAT payloads
  * joined), its bytes, palette / 16 (uint8 [256][3], rgb from palette only), rectangle first row, first column, rows,
- * columns, output / 16, scratch offset / 16, unused...}.  Each rectangle is written at its output offset, which must lie
- * past host_bytes, after the previous image's output: uint8 [rows][columns][3] (kind 0), uint16 (1), uint8 (2).
+ * columns, output / 16, scratch offset / 16, record offset / 16 (0 for a stream under 32 KiB), first unit}.  Each
+ * rectangle is written at its output offset, which must lie past host_bytes, after the previous image's output: uint8
+ * [rows][columns][3] (kind 0), uint16 (1), uint8 (2).
  * `scratch`: each image's inflated rows (height * (1 + row bytes), 16-byte aligned), at the running sum of the images
- * before it.  status (device int32 [num_images]) receives 0 for an image decoded as zlib and Pillow decode it, non-zero
+ * before it; then, for each stream of 32 KiB to 256 MiB (inflated in parallel), at the running sum after the rows, its
+ * records: a 64-byte stream record (int32 state: 1 decoded in parallel, 2-5 handed to the one-warp inflate; blocks;
+ * blocks walked; ...), 16 bytes per 16 KiB slice, 16 bytes per unit (slices + 8; the first unit is the running sum of
+ * the units before) and a uint16 plane of 2 bytes per inflated byte; then, when there is such a stream, 64 bytes per
+ * image of descriptors for the fallback launch.  Shorter streams, and any stream where the parallel inflate meets
+ * anything but a clean chain of blocks, are inflated by one warp each.  status (device int32 [num_images]) receives 0
+ * for an image decoded as zlib and Pillow decode it, non-zero
  * when the stream is anything but a well-formed zlib stream of exactly the image's rows with a matching Adler-32, or a
- * row has a filter type above 4; such an image's rectangle is not written, and the caller decodes it with Pillow.
- * Two launches for the whole batch; every descriptor, range and offset is checked on the host first.
+ * row has a filter type above 4; such an image's rectangle is not written, and the caller decodes it with Pillow.  A
+ * status word is the one-warp inflate's whichever path the stream took.
+ * Two launches for the whole batch without such a stream, seven with; every descriptor, range and offset is checked on
+ * the host first.
  * ---------------------------------------------------------------------------------------------- */
 int mmae_png_decode_batch(const void* packed_host, void* packed, int64_t host_bytes, int64_t packed_bytes,
                           int num_images, int64_t desc_offset, void* scratch, int64_t scratch_bytes, int* status,

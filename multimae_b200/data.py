@@ -447,6 +447,11 @@ def jpeg_fields(jd, src, rect, packer, coef_blocks, plane_bytes, slots):
             slots + jpeg.subsequence_slots(src.scan[1] - src.scan[0], len(src.intervals)))
 
 
+def _png_raw_bytes(src):
+    """The inflated bytes of PngSource `src`: its rows, each with its filter type byte."""
+    return src.height * (1 + src.width * (3 if src.ctype == 2 else src.depth // 8))
+
+
 def pack_batch(crops, size, mean, std):
     """The collate half: pack `crops` (list of Crops) for output size `size` into a PackedBatch."""
     tasks = list(crops[0].arrays)
@@ -497,7 +502,17 @@ def pack_batch(crops, size, mean, std):
         pd[:8] = src.width, src.height, src.depth, src.ctype, AUGMENT_KINDS[tasks[t]], stream, len(src.stream), palette
         pd[8:12] = rect
         pd[13] = raw // 16
-        raw = _align16(raw + src.height * (1 + src.width * (3 if src.ctype == 2 else src.depth // 8)))
+        raw = _align16(raw + _png_raw_bytes(src))
+    units = 0                            # the parallel inflate's records after the rows (0 for a one-warp stream)
+    for pd, (b, t) in zip(pdesc, pngs):
+        src = crops[b].arrays[tasks[t]][0]
+        pd[15] = units
+        if png.parallel_stream(len(src.stream)):
+            pd[14] = raw // 16
+            raw += png.record_bytes(len(src.stream), _png_raw_bytes(src))
+            units += png.units(len(src.stream))
+    if units:
+        raw += len(pngs) * png.FALLBACK_DESC_BYTES
     png_files = []
     for rows, items, field in ((jdesc, jpegs, 21), (pdesc, pngs, 12)):   # the decoded crops: on the device only
         for r, (b, t) in zip(rows, items):

@@ -193,14 +193,18 @@ def jpeg_decode_batch(host, dev, desc_offset, num_images, coef_blocks, plane_byt
     return scratch
 
 
-def png_decode_batch(host, dev, desc_offset, num_images, raw_bytes):
+def png_decode_batch(host, dev, desc_offset, num_images, raw_bytes, scratch=None):
     """Decode the PNG rectangles of one packed pre-training batch (multimae_b200.data.pack_batch: `host` its uint8 host
     buffer, `dev` the device buffer, whose first host.numel() bytes are its copy) into dev's tail, on the current
-    stream.  Returns the int32 [num_images] device status words (0: decoded; otherwise the rectangle is not written)."""
+    stream.  Returns the int32 [num_images] device status words (0: decoded; otherwise the rectangle is not written).
+    `scratch`: a uint8 device tensor of at least raw_bytes to use (its parallel inflate records tell which path each
+    stream took), else one is allocated."""
     _need_cuda(dev)
     assert host.dtype == torch.uint8 and dev.dtype == torch.uint8 and host.numel() <= dev.numel()
     nbytes = max(int(raw_bytes), 16)
-    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev.device)
+    if scratch is None:
+        scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev.device)
+    assert scratch.dtype == torch.uint8 and scratch.is_cuda and scratch.numel() >= nbytes
     status = torch.empty(int(num_images), dtype=torch.int32, device=dev.device)
     L.check(L.lib().mmae_png_decode_batch(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), int(num_images),
                                           int(desc_offset), scratch.data_ptr(), nbytes, status.data_ptr(),

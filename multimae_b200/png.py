@@ -19,6 +19,19 @@ import zlib
 from PIL import Image
 
 SIGNATURE = b"\x89PNG\r\n\x1a\n"
+# the parallel inflate (csrc/png.cu)
+SLICE_BYTES = 16384            # compressed bytes per slice: one warp searches each for a block start
+PARALLEL_MIN_BYTES = 32768     # shorter streams are inflated by one warp
+PARALLEL_MAX_BYTES = 1 << 28   # so are longer ones (bit positions in int32)
+MAX_WALKED = 8                 # blocks per stream that no slice found, decoded while confirming the chain
+STREAM_RECORD_BYTES = 64       # int32 {state, blocks, blocks walked, Adler-32 in the stream, inflated bytes, ...}
+SLICE_RECORD_BYTES = 16        # int32 {start bit or -1, end bit or -1, inflated bytes, ok | final << 1}
+BLOCK_RECORD_BYTES = 16        # int32 {start bit, end bit, output offset, inflated bytes}
+FALLBACK_DESC_BYTES = 64       # per image: its descriptor as the fallback inflate reads it
+# stream record states: the parallel decode wrote the rows, or the stream went to the one-warp inflate because
+# the walk met a block or a stream end it refuses, found more than MAX_WALKED blocks without a slice record, a block's
+# second decode disagreed with its first, or a copy reached before the first byte / the Adler-32 differed
+PATH_PARALLEL, PATH_WALK, PATH_BOUND, PATH_EXPAND, PATH_RESOLVE = 1, 2, 3, 4, 5
 _CID = re.compile(rb"\w\w\w\w")                # Pillow's is_cid
 _MODES = {(8, 0): "L", (16, 0): "I;16", (8, 2): "RGB", (8, 3): "P"}
 _DECODED = {"rgb": ("L", "RGB", "P"), "depth": ("I;16",), "semseg": ("P", "L")}
@@ -49,6 +62,28 @@ class PngSource:
 
 def is_png(data):
     return data[:8] == SIGNATURE
+
+
+def parallel_stream(nbytes):
+    """Whether mmae_png_decode_batch tries the parallel inflate on a zlib stream of `nbytes` (csrc/png.cu's
+    png_parallel); a stream it does not decode exactly is inflated by one warp after all."""
+    return PARALLEL_MIN_BYTES <= nbytes < PARALLEL_MAX_BYTES
+
+
+def slices(nbytes):
+    return -(-nbytes // SLICE_BYTES)
+
+
+def units(nbytes):
+    """Warps per parallel stream in the search and expand launches: one per slice, and room for MAX_WALKED blocks."""
+    return slices(nbytes) + MAX_WALKED
+
+
+def record_bytes(nbytes, raw):
+    """Scratch of one parallel stream of `nbytes` inflating to `raw` bytes: its stream record, slice records, block
+    records, and a uint16 plane of the inflated bytes (0-255 a byte, 256 + j byte j of the 32 KiB before the block)."""
+    return (STREAM_RECORD_BYTES + slices(nbytes) * SLICE_RECORD_BYTES + units(nbytes) * BLOCK_RECORD_BYTES
+            + (2 * raw + 15) // 16 * 16)
 
 
 def parse(data, task, path=None):

@@ -8,10 +8,13 @@ PNGs, semseg as 8-bit palette PNGs, written with Pillow's defaults; input size 2
 alone (the workers decode with Pillow), "after" adds the GPU decode (CompressedMultiTaskImages).
 
 Prints one JSON line per figure:
-  - the GPU name and power limit, read in the same run;
+  - the GPU name, power limit and SM clocks, read in the same run;
   - per batch of 128 and per domain, each decode kernel's device time from torch.profiler over --iters calls;
+  - per PNG domain: how many streams took the parallel inflate, the decode call's time, and with --baseline-lib the
+    same call of an earlier build of the library on the same packed batch, alternating, with both outputs compared;
   - worker CPU time per sample (process time, one torch thread, in this process), before and after;
-  - DataLoader samples/s at batch 128 with 10 workers, before and after, batches ending on the GPU;
+  - DataLoader samples/s at batch 128 with 10 workers, before and after, batches ending on the GPU: the first
+    20 batches (what the workers prefetch) are not timed, the next --loader-batches are;
   - the benchmark's pre-training step (bench.py's model and TrainStep, batch 128, eager) alone, and with a batch's
     upload + decode + resampling running back to back on a second stream beside it, as the loader's copy stream runs
     it: CUDA events on each stream; --rounds rounds of --steps steps, alone and beside alternating."""
@@ -80,11 +83,14 @@ class Cycle(torch.utils.data.Dataset):
         return self.ds[i % len(self.ds)]
 
 
-def loader_rate(ds, batches):
-    loader = D._AugmentingDataLoader(Cycle(ds, (batches + 2) * 128), batch_size=128, shuffle=True, num_workers=10,
-                                     drop_last=True, pin_memory=True, persistent_workers=False)
+def loader_rate(ds, batches, workers=10):
+    """Steady-state samples/s: the first 2 x workers batches (what the workers prefetch, built before the clock could
+    start) are not timed, the next `batches` are."""
+    skip = 2 * workers
+    loader = D._AugmentingDataLoader(Cycle(ds, (batches + skip) * 128), batch_size=128, shuffle=True,
+                                     num_workers=workers, drop_last=True, pin_memory=True, persistent_workers=False)
     it = iter(loader)
-    for _ in range(2):
+    for _ in range(skip):
         next(it)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -92,6 +98,39 @@ def loader_rate(ds, batches):
         next(it)
     torch.cuda.synchronize()
     return batches * 128 / (time.perf_counter() - t0)
+
+
+def baseline_png_call(path):
+    """mmae_png_decode_batch of the library at `path` (an earlier commit's), on this batch's packing and scratch size."""
+    import ctypes
+    from multimae_b200 import _lib as L
+    f = ctypes.CDLL(path).mmae_png_decode_batch
+    f.restype = ctypes.c_int
+    f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int64,
+                  ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]
+
+    def call(host, dev, desc_offset, num_images, raw_bytes):
+        scratch = torch.empty(max(raw_bytes, 16), dtype=torch.uint8, device=dev.device)
+        status = torch.empty(num_images, dtype=torch.int32, device=dev.device)
+        assert f(host.data_ptr(), dev.data_ptr(), host.numel(), dev.numel(), num_images, desc_offset,
+                 scratch.data_ptr(), max(raw_bytes, 16), status.data_ptr(), L.current_stream()) == 0
+        return status
+    return call
+
+
+def png_paths(host, png_args, scratch):
+    """{path: streams} of one decode: 'one warp' (under the size threshold), or the parallel inflate's stream state."""
+    from multimae_b200 import png as P
+    off, n, _ = png_args
+    pd = host.numpy()[off * 16:].view(np.int32)[:n * D.PNG_FIELDS].reshape(n, D.PNG_FIELDS)
+    sc = scratch.cpu().numpy()
+    names = {P.PATH_PARALLEL: "parallel", P.PATH_WALK: "fallback_walk", P.PATH_BOUND: "fallback_bound",
+             P.PATH_EXPAND: "fallback_expand", P.PATH_RESOLVE: "fallback_resolve"}
+    out = {}
+    for d in pd:
+        k = "one_warp" if not d[14] else names.get(int(sc[d[14] * 16:d[14] * 16 + 4].view(np.int32)[0]), "unknown")
+        out[k] = out.get(k, 0) + 1
+    return out
 
 
 def main():
@@ -102,12 +141,13 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--baseline-lib", default=None,
-                    help="also time mmae_jpeg_decode_batch of this build of the library (an earlier commit's)")
+                    help="also time mmae_jpeg_decode_batch and mmae_png_decode_batch of this build of the "
+                         "library (an earlier commit's)")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     dev = torch.device("cuda:0")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                       text=True).stdout.strip()
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip()
     emit(gpu=torch.cuda.get_device_name(0), nvidia_smi=q)
     import utils.datasets as ud
     with tempfile.TemporaryDirectory() as root:
@@ -162,7 +202,10 @@ def main():
             h2 = pb.buffer.pin_memory()
             t2 = torch.empty(pb.device_bytes, dtype=torch.uint8, device=dev)
             t2[:h2.numel()].copy_(h2)
-            kernels.png_decode_batch(h2, t2, *pb.png)
+            scratch = torch.empty(max(pb.png[2], 16), dtype=torch.uint8, device=dev)
+            status = kernels.png_decode_batch(h2, t2, *pb.png, scratch=scratch).cpu()
+            emit(figure="png streams per batch of 128 by path", task=task, **png_paths(h2, pb.png, scratch),
+                 nonzero_status=int(status.ne(0).sum()))
             s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             s.record()
             for _ in range(a.iters):
@@ -170,6 +213,32 @@ def main():
             e.record()
             torch.cuda.synchronize()
             emit(figure="png decode per batch of 128, CUDA events (ms)", task=task, ms=s.elapsed_time(e) / a.iters)
+            if a.baseline_lib:
+                base = baseline_png_call(a.baseline_lib)
+                t2[h2.numel():].zero_()
+                kernels.png_decode_batch(h2, t2, *pb.png)
+                ours = t2.clone()
+                t2[h2.numel():].zero_()
+                base(h2, t2, *pb.png)
+                torch.cuda.synchronize()
+                import gpu_time_jpeg_decode as G
+                times = {"this": [], "baseline": []}
+                for _ in range(3):
+                    times["this"].append(round(G.time_calls(lambda: kernels.png_decode_batch(h2, t2, *pb.png),
+                                                            a.iters), 3))
+                    times["baseline"].append(round(G.time_calls(lambda: base(h2, t2, *pb.png), a.iters), 3))
+                emit(figure="png decode call per batch of 128 (ms) vs baseline", task=task, call_event_ms=times,
+                     bitwise_equal=bool(torch.equal(ours, t2)))
+                with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                    for _ in range(a.iters):
+                        kernels.png_decode_batch(h2, t2, *pb.png)
+                    torch.cuda.synchronize()
+                kt = {}
+                for ev_ in prof.key_averages():
+                    m = re.search(r"png_\w+_kernel", ev_.key)
+                    if m:
+                        kt[m.group(0)] = round(kt.get(m.group(0), 0.0) + ev_.device_time_total / 1e3 / a.iters, 3)
+                emit(figure="png kernels per batch of 128 (ms)", task=task, kernels=kt)
         emit(figure="worker CPU per sample (ms)", before=per_sample_cpu(before, 64), after=per_sample_cpu(after, 64))
         torch.set_num_threads(min(16, os.cpu_count() or 1))
         emit(figure="DataLoader samples/s, batch 128, 10 workers", before=loader_rate(before, a.loader_batches),
@@ -211,8 +280,8 @@ def main():
                 row["step_ms_beside" if beside else "step_ms_alone"] = s0.elapsed_time(s1) / a.steps
             emit(figure="pre-training step, batch 128 (ms)", round=r, **row)
     emit(gpu=torch.cuda.get_device_name(0), nvidia_smi=subprocess.run(
-        ["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-        text=True).stdout.strip())
+        ["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+        capture_output=True, text=True).stdout.strip())
 
 
 if __name__ == "__main__":
