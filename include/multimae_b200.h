@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 21
+#define MMAE_ABI_VERSION 22
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -91,6 +91,16 @@ int mmae_set_pdl(int enable);
 /* SM budget of the SM-count-sized grids (GEMM split-K / tile choice, one-wave element-wise grids): 0 = every SM
  * (default), n = at most n.  Data-parallel runs leave NCCL's all-reduce CTAs their SMs.  Env MMAE_SM_BUDGET. */
 int mmae_set_sm_budget(int sms);
+/* 1: deterministic mode, the same bits for the same inputs, shapes and library build on any SM count or budget.  Split-K
+ * GEMMs (automatic split, split_k <= 0, or explicit) store each split's fp32 partial tile into its own slice of a
+ * per-stream workspace and one kernel adds the slices in split order onto out_f32 (the destination contract of
+ * mmae_gemm_bf16 holds: split-K adds onto out_f32 with or without accumulate); the split count is ceil(k-blocks / 32) for the
+ * automatic split and the tile choice models a 132-SM card, whatever the card or budget.  Float atomics of gradient and
+ * loss sums become per-block partials added in block order, and reductions sized by the SM count use 132.  The workspace
+ * grows on eager calls, like the column-reduction scratch: run a step eagerly before capturing a graph.  A captured graph
+ * keeps the mode it was captured in.  0 (default): the unordered forms (TMA reduce-add / red.global, atomics).  The host
+ * layer sets it from torch.are_deterministic_algorithms_enabled(). */
+int mmae_set_deterministic(int enable);
 /* 1: mmae_block_backward runs its four weight-gradient GEMMs on a library-owned side stream, forked behind the kernel
  * that produces their dY operand and joined before the call returns (the caller's stream order is unchanged);
  * 0 (default; no gain measured at the MultiMAE-B shapes): everything on the caller's stream.  Env MMAE_WGRAD_STREAM. */

@@ -154,6 +154,7 @@ SIGNATURES = {
                                            c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p,
                                            c_int, c_int, c_void_p]),
     "mmae_set_sm_budget": (c_int, [c_int]),
+    "mmae_set_deterministic": (c_int, [c_int]),
     "mmae_attention_set_tc": (c_int, [c_int]),
     "mmae_attention_forward": (c_int, [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
                                        c_int, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p]),
@@ -306,7 +307,7 @@ SIGNATURES = {
     "mmae_standardize_depth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 21
+ABI_VERSION = 22
 
 
 def lib():

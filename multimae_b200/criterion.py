@@ -21,6 +21,7 @@ class _MaskedLoss(nn.Module):
         self.label_smoothing = label_smoothing
 
     def forward(self, input, target, mask=None):
+        Fn.sync_deterministic()
         loss = Fn.MaskedLossFunction.apply(input, target, mask, self.kind, bool(self.norm_pix), self.scale_factor,
                                            float(self.label_smoothing))
         return DeferredScalar.wrap(loss)       # plain tensor unless the overlay's lazy meters are on (lazy_meters.py)

@@ -31,7 +31,7 @@ int pool_threads(int D) { return std::min(POOL_MAX_THREADS, (D / 4 + 31) / 32 * 
 
 // token runs per sample: enough CTAs for ~4 per SM, but at most one per token
 int pool_splits(int B, int N) {
-  const int want = std::max(1, ceil_div(4 * sm_count(), B));
+  const int want = std::max(1, ceil_div(4 * reduce_sm_count(), B));
   const int chunk = ceil_div(N, std::min(want, N));
   return ceil_div(N, chunk);
 }

@@ -56,6 +56,12 @@ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline size_t align_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 
 int sm_count();  // cached multiprocessor count of the current device
+// Deterministic mode (mmae_set_deterministic): split-K GEMMs add their partial tiles in split order, the float atomics
+// of the gradient and loss sums become per-block partials added in block order, and every reduction whose summation
+// order follows its grid sizes that grid by DET_SM_COUNT instead of the card's SM count or budget
+bool deterministic();
+constexpr int DET_SM_COUNT = 132;
+int reduce_sm_count();   // sm_count(), or DET_SM_COUNT in deterministic mode: sizes the grids of order-dependent reductions
 bool pdl_enabled();   // MMAE_PDL=0 / mmae_set_pdl(0) launches kernels fully serialized (A/B measurements)
 
 template <typename... KArgs, typename... Args>

@@ -425,7 +425,7 @@ static int colsum_rows_per_block(int M, int col_blocks, int blocks_per_sm) {
     return e ? atoi(e) : 0;
   }();
   if (tune > 0) blocks_per_sm = tune;
-  const int target = std::max(1, sm_count() * blocks_per_sm / std::max(col_blocks, 1));
+  const int target = std::max(1, reduce_sm_count() * blocks_per_sm / std::max(col_blocks, 1));
   int rpb = ceil_div(M, target);
   rpb = std::max(32, (rpb + 7) / 8 * 8);
   return rpb;
@@ -496,8 +496,10 @@ float* colred_scratch(size_t floats, cudaStream_t st) {
                    floats);
     return nullptr;
   }
-  cudaDeviceSynchronize();   // growing frees the old buffer: drain the device first (rare)
-  cudaFree(s->buf);
+  // The old buffer stays allocated: a CUDA graph captured before the growth still uses it.  Growth after a capture
+  // happens when a later eager step needs more, e.g. one in deterministic mode (the ordered split-K workspace).  The
+  // capacity at least doubles, so a slot leaves behind buffers that add up to less than its current one.
+  floats = std::max(floats, 2 * s->cap);
   s->buf = nullptr;
   s->cap = 0;
   if (cudaMalloc(&s->buf, (floats + COLRED_HEADER_FLOATS) * sizeof(float)) != cudaSuccess ||

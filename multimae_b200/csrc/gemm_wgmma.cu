@@ -31,6 +31,7 @@
 namespace mmae {
 
 void count_launch();
+float* colred_scratch(size_t floats, cudaStream_t st);   // the per-stream workspace pool (elementwise.cu)
 bool gemm_profile_begin(cudaStream_t st, double flops, int M, int N, int K, int flags);
 void gemm_profile_end(cudaStream_t st);
 
@@ -286,8 +287,10 @@ __device__ __forceinline__ void epilogue_slab(const float (&acc)[BN / 2], int ro
   }
 }
 
-// Cooperative consumers: both warpgroups work on the same item, 64 rows each, and run its epilogue together
-template <int BN, int CL, bool A_MN, bool B_MN>
+// Cooperative consumers: both warpgroups work on the same item, 64 rows each, and run its epilogue together.
+// ORD (ordered split-K, deterministic mode; CL = 1, p.tma_store = 2): split s stores its tile into rows
+// [s * tiles_m * BM, (s + 1) * tiles_m * BM) of the workspace map tmC, and splitk_reduce_kernel adds the slices in order.
+template <int BN, int CL, bool A_MN, bool B_MN, bool ORD = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
@@ -367,7 +370,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
       release((it - 1) % STAGES);   // the producer refills it with the next item's operands during the epilogue
-      epilogue_slab<BN>(acc, w.m0 + cw * 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
+      const int slice_row = ORD ? w.split * p.tiles_m * BM : 0;
+      epilogue_slab<BN>(acc, slice_row + w.m0 + cw * 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
     }
     if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
   }
@@ -474,15 +478,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   }
 }
 
-// PP: the ping-pong kernel (CL = 1), else the cooperative one
-template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false>
+// PP: the ping-pong kernel (CL = 1), else the cooperative one; ORD: the cooperative one's ordered split-K form
+template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false, bool ORD = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                 cudaStream_t stream) {
   static_assert(!PP || CL == 1, "the ping-pong kernel runs single CTAs");
+  static_assert(!ORD || (CL == 1 && !PP), "ordered split-K runs the single-CTA cooperative kernel");
   using C = GemmCfg<BN>;
   auto kern = [] {
     if constexpr (PP) return gemm_bf16_pingpong_kernel<BN, A_MN, B_MN>;
-    else return gemm_bf16_kernel<BN, CL, A_MN, B_MN>;
+    else return gemm_bf16_kernel<BN, CL, A_MN, B_MN, ORD>;
   }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -517,7 +522,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   const int slots = std::min(resident, std::max(1, sm_count() / CL));
   cfg.gridDim = dim3(std::min(items, slots) * CL);
   const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K,
-                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (p.splits << 8));
+                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (ORD ? 8 : 0) | (p.splits << 8));
   if constexpr (CL == 1) {
     cfg.attrs = attr + 1;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
@@ -529,6 +534,36 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   count_launch();
   MMAE_LAUNCH_OK();
   return MMAE_OK;
+}
+
+// Second pass of ordered split-K: out += ((ws[0] + ws[1]) + ... + ws[S - 1]) (+ residual), four columns per thread.
+// Like the unordered split-K, which reduce-adds every split onto out, it adds onto out whether or not accumulate is set
+// (the ABI: a split-K destination is zeroed or holds the value to accumulate onto).  Slice s of the workspace holds rows
+// [s * slice_rows, ...) of a [*, N] fp32 matrix.  Each output element has one writer: a single plain add.
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ ws, int S, int slice_rows, int M,
+                                                             int N, const float* __restrict__ residual,
+                                                             int64_t ld_residual, float* __restrict__ out,
+                                                             int64_t ld_out) {
+  pdl_prologue();
+  const int n4 = N / 4;
+  const int64_t total = int64_t(M) * n4;
+  const int64_t slice = int64_t(slice_rows) * N;
+  for (int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < total; i += int64_t(gridDim.x) * blockDim.x) {
+    const int m = int(i / n4), c = int(i - int64_t(m) * n4) * 4;
+    const float* src = ws + int64_t(m) * N + c;
+    float4 v = __ldcg(reinterpret_cast<const float4*>(src));
+    for (int s = 1; s < S; ++s) {
+      const float4 u = __ldcg(reinterpret_cast<const float4*>(src + s * slice));
+      v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
+    }
+    if (residual) {
+      const float4 r = __ldg(reinterpret_cast<const float4*>(residual + int64_t(m) * ld_residual + c));
+      v.x += r.x; v.y += r.y; v.z += r.z; v.w += r.w;
+    }
+    float4* dst = reinterpret_cast<float4*>(out + int64_t(m) * ld_out + c);
+    const float4 o = *dst;
+    *dst = make_float4(o.x + v.x, o.y + v.y, o.z + v.z, o.w + v.w);
+  }
 }
 
 }  // namespace
@@ -580,6 +615,40 @@ constexpr int KB_PER_ITEM_FIXED = 4;
 // model does not pick it, and variant 7 runs only when set.
 // Split-K never cuts an item below this many k-blocks, which bounds the fp32 reduce-add traffic it adds
 constexpr int MIN_KB_PER_SPLIT = 16;
+// Deterministic mode: the automatic split makes ceil(k-blocks / DET_KB_PER_SPLIT) splits of equal k-block counts, so
+// the split count, and with it the summation order, follows from K alone.  The bench step's long-K weight gradients
+// (K = tokens, 198 k-blocks) get 7 splits of 29 k-blocks.
+constexpr int DET_KB_PER_SPLIT = 32;
+
+// Ordered split-K (deterministic mode): each split stores its fp32 partial tile with the plain TMA-store epilogue into
+// its own slice of a [splits, tiles_m * BM, N] workspace from the per-stream pool, and splitk_reduce_kernel adds the
+// slices in split order (then residual), and adds the sum onto the output.
+template <int BN, bool A_MN, bool B_MN>
+int launch_ordered(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t st) {
+  const int slice_rows = p.tiles_m * BM;
+  const size_t floats = size_t(p.splits) * slice_rows * p.N;
+  float* ws = colred_scratch(floats, st);
+  if (!ws) {
+    set_last_error("mmae_gemm_bf16: the ordered split-K workspace of deterministic mode (mmae_set_deterministic) needs "
+                   "%zu bytes, which must be allocated outside stream capture: run the step once eagerly first",
+                   floats * sizeof(float));
+    return MMAE_ERR_CUDA;
+  }
+  CUtensorMap tmC;
+  const int rc = make_tmap_2d_store(&tmC, ws, 4, uint64_t(p.splits) * slice_rows, (uint64_t)p.N, (uint64_t)p.N);
+  if (rc) return rc;
+  const mmae_gemm_epilogue ep = p.ep;
+  p.tma_store = 2;
+  const int lrc = launch_gemm<BN, 1, A_MN, B_MN, false, true>(tmA, tmB, tmC, p, st);
+  if (lrc) return lrc;
+  const int64_t total = int64_t(p.M) * (p.N / 4);
+  const unsigned blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, int64_t(sm_count()) * 16));
+  launch_k(splitk_reduce_kernel, blocks, 256, 0, st, ws, p.splits, slice_rows, p.M, p.N, ep.residual, ep.ld_residual,
+           ep.out_f32, ep.ld_out_f32);
+  count_launch();
+  MMAE_LAUNCH_OK();
+  return MMAE_OK;
+}
 
 extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const void* B, int64_t ldb,
                               int b_mn_major, int M, int N, int K, int split_k, const mmae_gemm_epilogue* ep,
@@ -592,9 +661,11 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
              MMAE_ERR_ARG, "mmae_gemm_bf16: operands must be 16-byte aligned");
   MMAE_CHECK(ep->out_f32 || ep->out_bf16, MMAE_ERR_ARG, "mmae_gemm_bf16: no output");
   const int num_kb = ceil_div(K, BK);
-  const int sms = sm_count();
+  const bool det = deterministic();
+  const int sms = det ? DET_SM_COUNT : sm_count();   // deterministic mode: the tile choice follows the shape alone
   const int tm = ceil_div(M, BM);
   if (split_k <= 0 && !(ep->out_f32 && !ep->out_bf16 && !ep->preact_bf16 && !ep->dgelu_z && ep->act == 0)) split_k = 1;
+  if (det && split_k <= 0) split_k = ceil_div(num_kb, DET_KB_PER_SPLIT);
 
   // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time (clusters:
   // sm_count() / 2 items of 256 rows), so a launch lasts ceil(items / slots) rounds of one item, and an item costs
@@ -647,6 +718,9 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
              MMAE_ERR_ARG, "mmae_gemm_bf16: epilogue tensors need 16-byte alignment and ld %% 8 == 0");
 #undef MMAE_LD_OK
 
+  const bool ordered = det && split_k > 1;
+  // ordered split-K runs the cooperative single-CTA kernel of the same tile width
+  if (ordered) variant = (variant == 6 || variant == 7) ? 1 : (variant == 4 ? 2 : (variant == 5 ? 3 : variant));
   if (variant == 5 && b_mn_major) variant = 4;   // an MN-major B half must be whole 64-column chunks
   const int BNsel = variant_bn(variant);
   const int CLsel = variant_cl(variant);
@@ -691,6 +765,20 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     }
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (ordered) {
+#define MMAE_DISPATCH_ORD(BN_)                                                                  \
+  do {                                                                                          \
+    if (!a_mn_major && !b_mn_major) return launch_ordered<BN_, false, false>(tmA, tmB, p, st);  \
+    if (!a_mn_major && b_mn_major) return launch_ordered<BN_, false, true>(tmA, tmB, p, st);    \
+    if (a_mn_major && !b_mn_major) return launch_ordered<BN_, true, false>(tmA, tmB, p, st);    \
+    return launch_ordered<BN_, true, true>(tmA, tmB, p, st);                                    \
+  } while (0)
+    if (BNsel == 64) MMAE_DISPATCH_ORD(64);
+    if (BNsel == 192) MMAE_DISPATCH_ORD(192);
+    if (BNsel == 256) MMAE_DISPATCH_ORD(256);
+    MMAE_DISPATCH_ORD(128);
+#undef MMAE_DISPATCH_ORD
+  }
 #define MMAE_DISPATCH(BN_, CL_, PP_)                                                                      \
   do {                                                                                                    \
     if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false, PP_>(tmA, tmB, tmC, p, st); \

@@ -90,17 +90,22 @@ __global__ void __launch_bounds__(256) embed_assemble_kernel(const float* __rest
   }
 }
 
-// backward of the assembly: dC (bf16 rows of kept tokens), per-task bias grads, global-token grad
+// backward of the assembly: dC (bf16 rows of kept tokens), per-task bias grads, global-token grad.  With `partial`
+// (deterministic mode) block k writes its sums to row k of partial, [G global tokens | num_tasks biases] x D, for
+// colred_finalize to add in block order; otherwise it adds them with atomics.
 constexpr int EB_ROWS = 32;
 __global__ void __launch_bounds__(256) embed_assemble_bwd_kernel(const float* __restrict__ dx, int T, int G, int D, int B,
                                                                  const int* __restrict__ row_task,
                                                                  bf16* __restrict__ dC, mmae_embed_grads grads,
-                                                                 int num_tasks) {
+                                                                 int num_tasks, float* __restrict__ partial) {
   pdl_prologue();
   // block handles EB_ROWS consecutive sequence rows; thread c handles columns c, c+256, ...
   const int row0 = blockIdx.x * EB_ROWS;
   const int rows_total = B * (T + G);
+  float* prow = partial ? partial + int64_t(blockIdx.x) * (G + num_tasks) * D : nullptr;
   for (int c = threadIdx.x; c < D; c += blockDim.x) {
+    if (prow)   // this thread alone owns column c of the block's row
+      for (int g = 0; g < G; ++g) prow[int64_t(g) * D + c] = 0.f;
     float accb[MMAE_MAX_TASKS];
 #pragma unroll
     for (int t = 0; t < MMAE_MAX_TASKS; ++t) accb[t] = 0.f;
@@ -112,7 +117,8 @@ __global__ void __launch_bounds__(256) embed_assemble_bwd_kernel(const float* __
       if (i >= T) {
         // global tokens: at most one global-token index per flush (G is tiny); flush when it changes
         if (gidx != i - T && gidx >= 0) {
-          atomicAdd(grads.global_tokens + int64_t(gidx) * D + c, accg);
+          if (prow) prow[int64_t(gidx) * D + c] += accg;
+          else atomicAdd(grads.global_tokens + int64_t(gidx) * D + c, accg);
           accg = 0.f;
         }
         gidx = i - T;
@@ -125,6 +131,13 @@ __global__ void __launch_bounds__(256) embed_assemble_bwd_kernel(const float* __
         for (int tt = 0; tt < MMAE_MAX_TASKS; ++tt)
           if (tt == t) accb[tt] += v;
       }
+    }
+    if (prow) {
+      if (gidx >= 0) prow[int64_t(gidx) * D + c] += accg;
+#pragma unroll
+      for (int t = 0; t < MMAE_MAX_TASKS; ++t)
+        if (t < num_tasks) prow[int64_t(G + t) * D + c] = accb[t];
+      continue;
     }
     if (gidx >= 0) atomicAdd(grads.global_tokens + int64_t(gidx) * D + c, accg);
 #pragma unroll
@@ -160,6 +173,39 @@ __global__ void __launch_bounds__(256) semseg_emb_bwd_kernel(const bf16* __restr
   __syncthreads();
   for (int i = threadIdx.x; i < num_classes * E; i += blockDim.x)
     if (tab[i] != 0.f) atomicAdd(dtable + i, tab[i]);
+}
+
+// Deterministic form of semseg_emb_bwd_kernel: thread e owns column e of the CTA's table and adds its values in (row,
+// pixel) order, so no two threads touch one entry; the CTA then writes its table to row blockIdx.x of `partial`, which
+// colred_finalize adds up in CTA order.
+__global__ void __launch_bounds__(256) semseg_emb_bwd_det_kernel(const bf16* __restrict__ dA, int64_t ld_dA,
+                                                                 const int64_t* __restrict__ labels,
+                                                                 const int* __restrict__ row_task,
+                                                                 const int* __restrict__ row_patch, int task, int T,
+                                                                 int rows, int rows_per_cta, int grid_w, int grid_h,
+                                                                 int P, int E, int num_classes, float* __restrict__ partial) {
+  pdl_prologue();
+  extern __shared__ float tab[];  // [num_classes * E]
+  for (int i = threadIdx.x; i < num_classes * E; i += blockDim.x) tab[i] = 0.f;
+  __syncthreads();
+  const int r0 = blockIdx.x * rows_per_cta;
+  const int Wt = grid_w * P, Ht = grid_h * P;
+  for (int r = r0; r < min(r0 + rows_per_cta, rows); ++r) {
+    if (row_task[r] != task) continue;  // uniform per row
+    const int b = r / T, p = row_patch[r];
+    const int ph = p / grid_w, pw = p % grid_w;
+    const int64_t* lrow = labels + (int64_t(b) * Ht + ph * P) * Wt + pw * P;
+    const bf16* arow = dA + int64_t(r) * ld_dA;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+      for (int q = 0; q < P * P; ++q) {
+        const int64_t label = lrow[int64_t(q / P) * Wt + q % P];
+        if (label >= 0 && label < num_classes) tab[label * E + e] += __bfloat162float(arow[e * P * P + q]);
+      }
+    }
+  }
+  __syncthreads();
+  float* prow = partial + int64_t(blockIdx.x) * num_classes * E;
+  for (int i = threadIdx.x; i < num_classes * E; i += blockDim.x) prow[i] = tab[i];
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -466,11 +512,24 @@ int launch_embed_assemble(const float* Cmat, const mmae_embed_params& prm, const
 
 int launch_embed_assemble_bwd(const float* dx, int B, int T, int G, int D, const int* row_task, bf16* dC,
                               const mmae_embed_grads& grads, int num_tasks, cudaStream_t st) {
-  launch_k(embed_assemble_bwd_kernel, ceil_div(B * (T + G), EB_ROWS), 256, 0, st, dx, T, G, D, B, row_task, dC, grads,
-                                                                            num_tasks);
+  const int blocks = ceil_div(B * (T + G), EB_ROWS);
+  float* partial = nullptr;
+  if (deterministic()) {
+    MMAE_CHECK(G + num_tasks <= 9, MMAE_ERR_UNSUPPORTED,
+               "embedding backward: deterministic mode adds at most 9 global-token / bias gradients (G=%d, tasks=%d)", G,
+               num_tasks);
+    partial = colred_scratch(size_t(blocks) * (G + num_tasks) * D, st);
+    if (!partial) return MMAE_ERR_CUDA;
+  }
+  launch_k(embed_assemble_bwd_kernel, blocks, 256, 0, st, dx, T, G, D, B, row_task, dC, grads, num_tasks, partial);
   count_launch();
   MMAE_LAUNCH_OK();
-  return MMAE_OK;
+  if (!partial || G + num_tasks == 0) return MMAE_OK;
+  ColredDst dst;
+  for (int k = 0; k < 9; ++k) dst.p[k] = nullptr;
+  for (int g = 0; g < G; ++g) dst.p[g] = grads.global_tokens ? grads.global_tokens + int64_t(g) * D : nullptr;
+  for (int t = 0; t < num_tasks; ++t) dst.p[G + t] = grads.bias[t];
+  return colred_finalize_n(partial, blocks, (G + num_tasks) * D, D, dst, G + num_tasks, st);
 }
 
 int launch_semseg_emb_bwd(const bf16* dA, int64_t ld_dA, const int64_t* labels, const int64_t* ids_keep,
@@ -483,8 +542,23 @@ int launch_semseg_emb_bwd(const bf16* dA, int64_t ld_dA, const int64_t* labels, 
     MMAE_CUDA_OK(cudaFuncSetAttribute(semseg_emb_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     configured = true;
   }
-  const int ctas = std::min(rows, 2 * sm_count());
+  const int ctas = std::min(rows, 2 * reduce_sm_count());
   const int rows_per_cta = ceil_div(rows, ctas);
+  if (deterministic()) {
+    static bool det_configured = false;
+    if (!det_configured) {
+      MMAE_CUDA_OK(cudaFuncSetAttribute(semseg_emb_bwd_det_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+      det_configured = true;
+    }
+    const int grid = ceil_div(rows, rows_per_cta);
+    float* partial = colred_scratch(size_t(grid) * num_classes * E, st);
+    if (!partial) return MMAE_ERR_CUDA;
+    launch_k(semseg_emb_bwd_det_kernel, grid, 256, smem, st, dA, ld_dA, labels, row_task, row_patch, task, T, rows,
+             rows_per_cta, grid_w, grid_h, P, E, num_classes, partial);
+    count_launch();
+    MMAE_LAUNCH_OK();
+    return colred_finalize(partial, grid, num_classes * E, num_classes * E, dtable, nullptr, nullptr, st);
+  }
   launch_k(semseg_emb_bwd_kernel, ceil_div(rows, rows_per_cta), 256, smem, st, dA, ld_dA, labels, ids_keep, row_task,
                                                                           row_patch, task, T, rows, rows_per_cta,
                                                                           grid_w, grid_h, P, E, num_classes, dtable);

@@ -495,7 +495,7 @@ static int ln_backward_narrow(const void* dy, int dy_is_bf16, int64_t lddy, cons
   MMAE_CHECK(dgamma && dbeta, MMAE_ERR_ARG, "mmae_layernorm_backward: dgamma / dbeta are required");
   // one wave, resident blocks per SM as for the float4 kernels of the same width
   const int per_sm = D <= 256 ? 3 : (D <= 384 ? 2 : 1);
-  dim3 grid(std::min(ceil_div(M, LN_WARPS), sm_count() * per_sm)), block(LN_WARPS * 32);
+  dim3 grid(std::min(ceil_div(M, LN_WARPS), reduce_sm_count() * per_sm)), block(LN_WARPS * 32);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* partial = colred_scratch(size_t(grid.x) * 3 * D, st);
   if (!partial) return MMAE_ERR_CUDA;
@@ -539,7 +539,7 @@ static int ln_backward_impl(const void* dy, int dy_is_bf16, int64_t lddy, const 
   }();
   int per_sm = D <= 256 ? 3 : (D <= 384 ? 2 : 1);
   if (tune > 0) per_sm = std::min(per_sm, tune);
-  dim3 grid(std::min(ceil_div(M, LN_WARPS), sm_count() * per_sm)), block(LN_WARPS * 32);
+  dim3 grid(std::min(ceil_div(M, LN_WARPS), reduce_sm_count() * per_sm)), block(LN_WARPS * 32);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   MMAE_CHECK(dgamma && dbeta, MMAE_ERR_ARG, "mmae_layernorm_backward: dgamma / dbeta are required");
   float* partial = colred_scratch(size_t(grid.x) * 3 * D, st);

@@ -6,6 +6,7 @@
 // Work is organised in strips: one CTA per (sample, patch row) = P image rows, only masked patches are touched.
 #include "common.cuh"
 #include "../../include/multimae_b200.h"
+#include "internal.h"
 
 namespace mmae {
 void count_launch();
@@ -34,6 +35,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) regr_loss_kernel(int kind, int n
                                                                  const float* __restrict__ tgt,
                                                                  const int64_t* __restrict__ mask, int C, int H, int W,
                                                                  int P, float* __restrict__ sample_sum,
+                                                                 float* __restrict__ partial,
                                                                  const float* __restrict__ coef,
                                                                  const float* __restrict__ grad_out,
                                                                  float* __restrict__ dpred) {
@@ -102,7 +104,11 @@ __global__ void __launch_bounds__(LOSS_THREADS) regr_loss_kernel(int kind, int n
   }
   if constexpr (!BWD) {
     const float tot = block_sum(acc, red);
-    if (threadIdx.x == 0 && tot != 0.f) atomicAdd(sample_sum + b, tot);
+    if (partial) {   // deterministic mode: one partial per (patch row, sample), added in patch-row order
+      if (threadIdx.x == 0) partial[int64_t(ph) * gridDim.x / nh + b] = tot;
+    } else if (threadIdx.x == 0 && tot != 0.f) {
+      atomicAdd(sample_sum + b, tot);
+    }
   }
 }
 
@@ -112,6 +118,7 @@ __global__ void __launch_bounds__(LOSS_THREADS) ce_loss_kernel(const float* __re
                                                                const int64_t* __restrict__ target,
                                                                const int64_t* __restrict__ mask, int C, int H, int W,
                                                                int P, float smoothing, float* __restrict__ sample_sum,
+                                                               float* __restrict__ partial,
                                                                const float* __restrict__ coef,
                                                                const float* __restrict__ grad_out,
                                                                float* __restrict__ dlogits) {
@@ -178,7 +185,11 @@ __global__ void __launch_bounds__(LOSS_THREADS) ce_loss_kernel(const float* __re
   }
   if constexpr (!BWD) {
     const float tot = block_sum(acc, red);
-    if (threadIdx.x == 0 && tot != 0.f) atomicAdd(sample_sum + b, tot);
+    if (partial) {
+      if (threadIdx.x == 0) partial[int64_t(ph) * gridDim.x / nh + b] = tot;
+    } else if (threadIdx.x == 0 && tot != 0.f) {
+      atomicAdd(sample_sum + b, tot);
+    }
   }
 }
 
@@ -242,15 +253,24 @@ extern "C" int mmae_masked_loss_forward(int kind, int norm_pix, float label_smoo
   float* coef = ws + B;
   MMAE_CUDA_OK(cudaMemsetAsync(sample_sum, 0, sizeof(float) * B, st));
   const int nh = H / scale, nw = W / scale;
+  float* partial = nullptr;   // deterministic mode: [nh, B] per-block sums instead of atomics
+  if (deterministic()) {
+    partial = colred_scratch(size_t(nh) * B, st);
+    if (!partial) return MMAE_ERR_CUDA;
+  }
   if (kind == 2) {
     launch_k(ce_loss_kernel<false>, B * nh, LOSS_THREADS, 0, st, pred, reinterpret_cast<const int64_t*>(target), mask, C, H, W,
-                                                           scale, label_smoothing, sample_sum, nullptr, nullptr, nullptr);
+                                                           scale, label_smoothing, sample_sum, partial, nullptr, nullptr, nullptr);
   } else {
     launch_k(regr_loss_kernel<false>, B * nh, LOSS_THREADS, 0, st, kind, norm_pix, pred, reinterpret_cast<const float*>(target),
-                                                             mask, C, H, W, scale, sample_sum, nullptr, nullptr, nullptr);
+                                                             mask, C, H, W, scale, sample_sum, partial, nullptr, nullptr, nullptr);
   }
   count_launch();
   MMAE_LAUNCH_OK();
+  if (partial) {
+    const int rc = colred_finalize(partial, nh, B, B, sample_sum, nullptr, nullptr, st);
+    if (rc) return rc;
+  }
   // mask == NULL ("loss on unmasked"): plain mean over every element == per-sample means averaged (equal counts)
   launch_k(loss_finalize_kernel, 1, 256, 0, st, sample_sum, mask, B, nh * nw, float(scale) * scale, kind == 2 ? 1.f : float(C),
                                           coef, loss_out);
@@ -272,10 +292,10 @@ extern "C" int mmae_masked_loss_backward(int kind, int norm_pix, float label_smo
   const int nh = H / scale;
   if (kind == 2) {
     launch_k(ce_loss_kernel<true>, B * nh, LOSS_THREADS, 0, st, pred, reinterpret_cast<const int64_t*>(target), mask, C, H, W,
-                                                          scale, label_smoothing, nullptr, coef, grad_out, dpred);
+                                                          scale, label_smoothing, nullptr, nullptr, coef, grad_out, dpred);
   } else {
     launch_k(regr_loss_kernel<true>, B * nh, LOSS_THREADS, 0, st, kind, norm_pix, pred, reinterpret_cast<const float*>(target),
-                                                            mask, C, H, W, scale, nullptr, coef, grad_out, dpred);
+                                                            mask, C, H, W, scale, nullptr, nullptr, coef, grad_out, dpred);
   }
   count_launch();
   MMAE_LAUNCH_OK();

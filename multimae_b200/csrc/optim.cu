@@ -21,9 +21,11 @@ namespace mmae {
 void count_launch();
 namespace {
 
-// out[0] += sum(g^2) after unscaling, out[1] = 1.0 if any non-finite value was seen (left untouched otherwise)
+// out[0] += sum(g^2) after unscaling, out[1] = 1.0 if any non-finite value was seen (left untouched otherwise).  With
+// `partial` (deterministic mode) block b writes its sum to partial[b] instead, for an ordered second pass.
 __global__ void __launch_bounds__(256) unscale_norm_kernel(float* __restrict__ g, int64_t n, const float* __restrict__ inv_scale_ptr,
-                                                           float inv_scale_imm, float post_scale, float* __restrict__ out) {
+                                                           float inv_scale_imm, float post_scale, float* __restrict__ out,
+                                                           float* __restrict__ partial) {
   pdl_prologue();
   __shared__ float red[8];
   const float inv = (inv_scale_ptr ? inv_scale_ptr[0] : inv_scale_imm) * post_scale;
@@ -64,7 +66,10 @@ __global__ void __launch_bounds__(256) unscale_norm_kernel(float* __restrict__ g
     float t = red[threadIdx.x];
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) t += __shfl_xor_sync(0xffu, t, o);
-    if (threadIdx.x == 0) atomicAdd(out, t);
+    if (threadIdx.x == 0) {
+      if (partial) partial[blockIdx.x] = t;
+      else atomicAdd(out, t);
+    }
   }
   if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) out[1] = 1.0f;
 }
@@ -319,12 +324,21 @@ extern "C" int mmae_grad_unscale_norm(float* grads, int64_t n, const float* inv_
   MMAE_CUDA_OK(cudaMemsetAsync(out2, 0, 2 * sizeof(float), st));
   if (n > 0) {
     int64_t blocks = (n / 4 + 255) / 256;
-    const int64_t cap = int64_t(sm_count()) * 8;
+    const int64_t cap = int64_t(reduce_sm_count()) * 8;   // the grid-stride sums follow the grid
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    launch_k(unscale_norm_kernel, (unsigned)blocks, 256, 0, st, grads, n, inv_scale_dev, inv_scale, post_scale, out2);
+    float* partial = nullptr;
+    if (deterministic()) {
+      partial = colred_scratch(size_t(blocks), st);
+      if (!partial) return MMAE_ERR_CUDA;
+    }
+    launch_k(unscale_norm_kernel, (unsigned)blocks, 256, 0, st, grads, n, inv_scale_dev, inv_scale, post_scale, out2, partial);
     count_launch();
     MMAE_LAUNCH_OK();
+    if (partial) {
+      const int rc = colred_finalize(partial, int(blocks), 1, 1, out2, nullptr, nullptr, st);
+      if (rc) return rc;
+    }
   }
   if (norm_out) {
     launch_k(sqrt_kernel, 1, 1, 0, st, out2, norm_out);

@@ -239,6 +239,15 @@ static int g_pdl = []() {
 }();
 bool pdl_enabled() { return g_pdl != 0; }
 }  // namespace mmae
+namespace mmae {
+static int g_deterministic = 0;
+bool deterministic() { return g_deterministic != 0; }
+int reduce_sm_count() { return g_deterministic ? DET_SM_COUNT : sm_count(); }
+}  // namespace mmae
+extern "C" int mmae_set_deterministic(int enable) {
+  mmae::g_deterministic = enable != 0;
+  return MMAE_OK;
+}
 extern "C" int mmae_set_sm_budget(int sms) {
   mmae::g_sm_budget = sms;
   return MMAE_OK;

@@ -109,6 +109,23 @@ def invalidate_mirrors():
         m.invalidate_mirror()
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# Deterministic mode follows torch.use_deterministic_algorithms (warn_only=True counts as on): the model checks the flag
+# where a step starts and the criteria, the scaler and the flat optimizers where they are called, and the library's
+# switch (mmae_set_deterministic) is set only when the flag has changed.  A captured CUDA graph (train_step.TrainStep)
+# replays the kernels it was captured with, so it keeps the mode of its capture.
+# ---------------------------------------------------------------------------------------------------------------------
+_deterministic = False          # the library's switch as last set here; it loads switched off
+
+
+def sync_deterministic():
+    global _deterministic
+    want = torch.are_deterministic_algorithms_enabled()
+    if want != _deterministic:
+        L.check(L.lib().mmae_set_deterministic(int(want)), "mmae_set_deterministic")
+        _deterministic = want
+
+
 def _grad_ptr(arena, name):
     return arena.views[name].data_ptr()
 

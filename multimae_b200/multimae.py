@@ -329,6 +329,7 @@ class MultiMAE(nn.Module):
                 alphas: Union[float, List[float]] = 1.0, sample_tasks_uniformly: bool = False,
                 fp32_output_adapters: List[str] = []):
         Fn.fresh_mirrors()                                    # bf16 weight twins follow any torch-side parameter change
+        Fn.sync_deterministic()
         x, adapters, placeholders, B, H, W, dev = self._prepare(x)
         input_info = self.generate_input_info(input_task_tokens=placeholders, image_size=(H, W))
         total = input_info["num_task_tokens"]
@@ -472,6 +473,7 @@ class MultiViT(MultiMAE):
 
     def forward(self, x, return_all_layers=False, **kwargs):
         Fn.fresh_mirrors()
+        Fn.sync_deterministic()
         tokens, input_info = self.process_input(x)
         if not return_all_layers:
             encoder_tokens = Fn.block_stack(self.encoder, tokens)

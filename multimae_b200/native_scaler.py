@@ -115,6 +115,7 @@ class NativeScalerWithGradNormCount:
 
     def __call__(self, loss, optimizer, clip_grad=None, skip_grad=None, parameters=None, create_graph=False,
                  update_grad=True):
+        Fn.sync_deterministic()
         self._lazy_init(loss.device)
         if parameters is not None and not isinstance(parameters, (list, tuple)):
             parameters = list(parameters)            # the script passes the generator model.parameters()

@@ -145,6 +145,7 @@ class FlatAdamW(_FlatParams, torch.optim.Optimizer):
         """One kernel over the flat buffers.  The step counter lives on the device and is advanced by the call itself,
         only when the step is taken (found_inf == 0): a skipped step leaves moments, parameters AND the bias correction
         untouched, like GradScaler.step."""
+        Fn.sync_deterministic()
         g = self.param_groups[0]
         if not (self._dyn.is_cuda and torch.cuda.is_current_stream_capturing()):
             self.sync_hyperparams()
@@ -331,6 +332,7 @@ class GroupedFlatAdamW(_FlatParams, torch.optim.Optimizer):
         """One launch over every group (more for a table longer than one launch holds).  The step count lives on the
         device and advances only when the step is taken (found_inf[0] == 0): a skipped step leaves parameters, moments, the
         bf16 twin and the bias correction untouched, like GradScaler.step, and needs no host sync."""
+        Fn.sync_deterministic()
         betas, eps = self._shared()
         for k, g in enumerate(self.param_groups):
             self._lrs[k] = float(g["lr"])

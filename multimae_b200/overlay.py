@@ -91,6 +91,20 @@ def _legacy_checkpoint_load():
     torch.load = load
 
 
+def _deterministic_from_env():
+    """MMAE_DETERMINISTIC=1 (or `warn`): torch.use_deterministic_algorithms(True) (warn_only=True for `warn`) before the
+    script runs, which also puts the CUDA path into its deterministic mode (functional.sync_deterministic).  cuBLAS needs
+    CUBLAS_WORKSPACE_CONFIG for deterministic results in the script's own torch ops; :4096:8 is set unless it is given."""
+    mode = os.environ.get("MMAE_DETERMINISTIC", "0").strip().lower()
+    if mode in ("", "0"):
+        return
+    if mode not in ("1", "warn"):
+        raise ValueError("MMAE_DETERMINISTIC=%r: expected 0, 1 or warn" % mode)
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+    import torch
+    torch.use_deterministic_algorithms(True, warn_only=mode == "warn")
+
+
 def install(reference_root=None, replace_ddp=True, legacy_checkpoint_load=True):
     """Install the overlay into sys.modules.  `reference_root`: checkout of EPFL-VILAB/MultiMAE (for its `utils` package)."""
     if "torch._six" not in sys.modules:            # utils/native_scaler.py:11 imports a module removed in torch >= 2
@@ -99,6 +113,7 @@ def install(reference_root=None, replace_ddp=True, legacy_checkpoint_load=True):
         sys.modules["torch._six"] = six
     if legacy_checkpoint_load:
         _legacy_checkpoint_load()
+    _deterministic_from_env()
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
     pkg = types.ModuleType("multimae")
