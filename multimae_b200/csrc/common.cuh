@@ -555,6 +555,9 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t rows, uint64_
                       uint32_t box_cols, uint32_t box_rows);
 // 3D bf16 tensor [d2, d1, d0] (d0 innermost) with element strides s1, s2; 128B swizzle
 int make_tmap_2d_store(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols, uint64_t ld);
+// same tensor, box = 64 rows x one 128-byte row (64 bf16 / 32 fp32 columns), 128B swizzle
+int make_tmap_2d_store_sw128(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols,
+                             uint64_t ld);
 int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1,
                       uint64_t s2, uint32_t b0, uint32_t b1, uint32_t b2);
 // same layout for TMA stores; b0 = 64 columns (SWIZZLE_128B staging tile) or 32 columns (SWIZZLE_64B)

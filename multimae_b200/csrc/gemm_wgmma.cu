@@ -135,13 +135,13 @@ __device__ __forceinline__ void stage_pair(uint8_t* box, int r, int c, float v0,
 }
 
 // TMA producer (one thread): walks the CTA's items in order and fills the ring; slot and phase follow a k-block count
-// that runs across items, so the next item's stages load while the consumers finish the current one
-template <int BN, int CL, bool A_MN, bool B_MN>
+// that runs across items, so the next item's stages load while the consumers finish the current one.  STAGES: the
+// ring's depth (the stage layout is GemmCfg<BN>'s whatever the depth)
+template <int BN, int CL, bool A_MN, bool B_MN, int STAGES = GemmCfg<BN>::STAGES>
 __device__ __forceinline__ void produce(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, const CUtensorMap* tmA,
                                         const CUtensorMap* tmB, const GemmParams& p, int rank, int first_item,
                                         int item_stride, int num_items) {
   using C = GemmCfg<BN>;
-  constexpr int STAGES = C::STAGES;
   constexpr int BH = BN / CL;   // B rows (output columns) this CTA loads
   static_assert(!B_MN || BH % 64 == 0, "MN-major B is loaded in 64-column chunks");
   uint32_t it = 0;   // k-blocks loaded so far, over all items
@@ -478,21 +478,170 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   }
 }
 
-// PP: the ping-pong kernel (CL = 1), else the cooperative one; ORD: the cooperative one's ordered split-K form
-template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false, bool ORD = false>
+// Asynchronous-epilogue kernel (gemm_async_epi_kernel): the cooperative kernel's items, ring and MMAs, for the
+// outputs that leave through a plain TMA store (p.tma_store 1 = bf16 or 2 = fp32; no split, accumulate, GELU or
+// residual).  Each consumer warpgroup stages its whole 64 x BN slab at once in a region of its own and hands it to the
+// TMA unit as one bulk group, then goes straight on to its next item's MMAs: the stores drain during that mainloop, and
+// the warpgroup waits for them to have read the region only when it stages the next slab.  Stages: BN = 128: 6 x 32 KB
+// + 2 x 16 KB of staging; 192: 4 x 40 KB + 2 x 24 KB; 256: 3 x 48 KB + 2 x 32 KB; fp32 (BN = 128): 5 x 32 KB + 2 x 32 KB.
+template <int BN, bool F32>
+struct AsyncEpiCfg {
+  static_assert(!F32 || BN == 128, "an fp32 slab wider than 128 columns does not fit next to the ring");
+  static constexpr int STAGES = F32 ? 5 : (BN == 256 ? 3 : (BN == 192 ? 4 : 6));
+  static constexpr int STAGE_BYTES = GemmCfg<BN>::STAGE_BYTES;
+  static constexpr int BOX_COLS = F32 ? 32 : 64;           // one 128-byte swizzle row of the output type
+  static constexpr int BOX_BYTES = 64 * 128;               // 64 rows x 128 bytes
+  static constexpr int SLAB_BYTES = (BN / BOX_COLS) * BOX_BYTES;
+  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = EPI_OFFSET + 2 * SLAB_BYTES;
+  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // + barriers + alignment slack
+  static_assert(TOTAL <= 232448, "GEMM exceeds the 227 KB shared-memory limit");
+};
+
+// Whole-slab epilogue of gemm_async_epi_kernel: v = alpha * acc (+ bias), rows [row0, row0 + 64), columns [n0, n0 + BN),
+// the values and their order of operations those of epilogue_slab's TMA path.  The slab is BN / BOX_COLS boxes of
+// 64 rows x 128 bytes, each in the 128B-swizzle layout of the store map (16-byte chunk c of row r at chunk c ^ (r & 7)),
+// so the 8 rows a warp writes per store land in 8 different chunks: no bank conflicts.  fp32: of each thread's column
+// pair, threads whose pair lies in the odd chunk write the second element first, which keeps the two threads of each
+// bank pair apart.  `bar`: the warpgroup's named barrier; thread t of 128.
+template <int BN, bool F32>
+__device__ __forceinline__ void epilogue_slab_async(const float (&acc)[BN / 2], int row0, int n0, const GemmParams& p,
+                                                    const CUtensorMap* tmC, uint8_t* slab, int bar, int t) {
+  using C = AsyncEpiCfg<BN, F32>;
+  const int lane = t & 31;
+  const int rl = (t >> 5) * 16 + (lane >> 2);   // this thread's first row within the 64; its second is rl + 8
+  const int sw = lane >> 2;                     // (rl & 7) == ((rl + 8) & 7)
+  const float* bias = p.ep.bias;
+  if (t == 0) bulk_wait_read_all();   // the slab this region held one item ago has been read by its stores
+  asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+  uint8_t* row_a = slab + rl * 128;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + j * 8 + 2 * (t & 3);
+    float v[4] = {acc[4 * j] * p.ep.alpha, acc[4 * j + 1] * p.ep.alpha, acc[4 * j + 2] * p.ep.alpha,
+                  acc[4 * j + 3] * p.ep.alpha};
+    if (bias && col < p.N) {
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+      v[0] += bb.x; v[1] += bb.y; v[2] += bb.x; v[3] += bb.y;
+    }
+    if constexpr (!F32) {
+      // 8 columns = one 16-byte chunk of a 64-column box
+      uint8_t* a = row_a + (j >> 3) * C::BOX_BYTES + ((((j & 7) ^ sw) << 4) | ((t & 3) << 2));
+      *reinterpret_cast<uint32_t*>(a) = pack_bf16x2(v[0], v[1]);
+      *reinterpret_cast<uint32_t*>(a + 8 * 128) = pack_bf16x2(v[2], v[3]);
+    } else {
+      // 8 columns = two 16-byte chunks of a 32-column box; the pair of thread t is in chunk 2 (j & 3) + ((t & 3) >> 1)
+      const int h = (t >> 1) & 1;
+      uint8_t* a = row_a + (j >> 2) * C::BOX_BYTES + ((((2 * (j & 3) + h) ^ sw) << 4) | ((t & 1) << 3));
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int f = e ^ h;
+        *reinterpret_cast<float*>(a + 4 * f) = f ? v[1] : v[0];
+        *reinterpret_cast<float*>(a + 8 * 128 + 4 * f) = f ? v[3] : v[2];
+      }
+    }
+  }
+  fence_proxy_async_smem();
+  asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+  if (t == 0) {
+#pragma unroll
+    for (int b = 0; b < BN / C::BOX_COLS; ++b)
+      if (n0 + b * C::BOX_COLS < p.N) tma_store_2d(tmC, slab + b * C::BOX_BYTES, n0 + b * C::BOX_COLS, row0);
+    bulk_commit_group();
+  }
+}
+
+// The cooperative kernel (CL = 1, no split) with epilogue_slab_async: both consumer warpgroups work on every item, 64
+// rows each, with the same produce / mma_kblock sequence, so its output bits are those of gemm_bf16_kernel<BN, 1, ...>.
+template <int BN, bool F32, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+    gemm_async_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                          const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+  pdl_launch_dependents();   // as in gemm_bf16_kernel
+  using C = AsyncEpiCfg<BN, F32>;
+  constexpr int STAGES = C::STAGES;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int wg = threadIdx.x >> 7;
+  const int num_items = p.tiles_n * p.tiles_m;
+  const int first_item = blockIdx.x;
+  const int item_stride = gridDim.x;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmC);
+#pragma unroll
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) produce<BN, 1, A_MN, B_MN, STAGES>(smem, full_bar, empty_bar, &tmA, &tmB, p, 0, first_item,
+                                                             item_stride, num_items);
+  } else {
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
+    const int t = threadIdx.x & 127;
+    uint8_t* slab = smem + C::EPI_OFFSET + cw * C::SLAB_BYTES;
+    uint32_t it = 0;       // k-blocks consumed so far, over all items
+    float acc[BN / 2];     // written by each item's first wgmma (scale-d = 0)
+
+    for (int item = first_item; item < num_items; item += item_stride) {
+      const WorkItem w = decode_item<BN, 1>(item, p, 0);
+      for (int kb = 0; kb < w.nkb; ++kb, ++it) {
+        const int s = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+        wgmma_fence();
+        mma_kblock<BN, A_MN, B_MN>(acc, smem + s * C::STAGE_BYTES, cw, kb == 0);
+        wgmma_commit();
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+        if (kb > 0 && t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+      if (t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      epilogue_slab_async<BN, F32>(acc, w.m0 + cw * 64, w.n0, p, &tmC, slab, 2 + cw, t);
+    }
+    if (t == 0) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
+  }
+}
+
+// PP: the ping-pong kernel (CL = 1), else the cooperative one; ORD: the cooperative one's ordered split-K form; AE = 1 /
+// 2: the asynchronous-epilogue kernel for a bf16 / fp32 TMA-stored output (CL = 1, one split)
+template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false, bool ORD = false, int AE = 0>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                 cudaStream_t stream) {
   static_assert(!PP || CL == 1, "the ping-pong kernel runs single CTAs");
   static_assert(!ORD || (CL == 1 && !PP), "ordered split-K runs the single-CTA cooperative kernel");
-  using C = GemmCfg<BN>;
+  static_assert(!AE || (CL == 1 && !PP && !ORD), "the asynchronous-epilogue kernel runs single CTAs");
+  constexpr int TOTAL = AE ? AsyncEpiCfg<BN, AE == 2>::TOTAL : GemmCfg<BN>::TOTAL;
   auto kern = [] {
-    if constexpr (PP) return gemm_bf16_pingpong_kernel<BN, A_MN, B_MN>;
+    if constexpr (AE) return gemm_async_epi_kernel<BN, AE == 2, A_MN, B_MN>;
+    else if constexpr (PP) return gemm_bf16_pingpong_kernel<BN, A_MN, B_MN>;
     else return gemm_bf16_kernel<BN, CL, A_MN, B_MN, ORD>;
   }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = C::TOTAL;
+  cfg.dynamicSmemBytes = TOTAL;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -506,7 +655,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   // CTAs (CL = 1) or clusters (CL = 2) of this kernel the device can hold at once
   static int resident = 0;
   if (resident == 0) {
-    MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::TOTAL));
+    MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
     if constexpr (CL > 1) {
       cfg.gridDim = dim3(CL);
       MMAE_CUDA_OK(cudaOccupancyMaxActiveClusters(&resident, kern, &cfg));
@@ -522,7 +671,8 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   const int slots = std::min(resident, std::max(1, sm_count() / CL));
   cfg.gridDim = dim3(std::min(items, slots) * CL);
   const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K,
-                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (ORD ? 8 : 0) | (p.splits << 8));
+                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (ORD ? 8 : 0) | (AE ? 16 : 0) |
+                                           (p.splits << 8));
   if constexpr (CL == 1) {
     cfg.attrs = attr + 1;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
@@ -575,7 +725,7 @@ using namespace mmae;
 static int g_gemm_variant = []() {
   const char* e = getenv("MMAE_GEMM_VARIANT");
   const int v = e ? atoi(e) : -1;
-  return v >= -1 && v <= 7 ? v : -1;
+  return v >= -1 && v <= 10 ? v : -1;
 }();
 static int g_gemm_tma_store = []() {
   const char* e = getenv("MMAE_GEMM_TMA_STORE");
@@ -583,7 +733,7 @@ static int g_gemm_tma_store = []() {
 }();
 
 extern "C" int mmae_gemm_set_variant(int variant) {
-  MMAE_CHECK(variant >= -1 && variant <= 7, MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1 .. 7)", variant);
+  MMAE_CHECK(variant >= -1 && variant <= 10, MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1 .. 10)", variant);
   g_gemm_variant = variant;
   return MMAE_OK;
 }
@@ -594,9 +744,15 @@ extern "C" int mmae_gemm_set_tma_store(int enable) {
 }
 
 // variant -> tile: 0 / 1 / 3 / 2 = one CTA, BN = 64 / 128 / 192 / 256; 6 / 5 / 4 = two-CTA cluster (256-row tile, B shared
-// by multicast), BN = 128 / 192 / 256; 7 = one CTA of ping-pong consumers, BN = 128
-static int variant_bn(int v) { return v == 0 ? 64 : (v == 1 || v == 6 || v == 7) ? 128 : (v == 3 || v == 5) ? 192 : 256; }
+// by multicast), BN = 128 / 192 / 256; 7 = one CTA of ping-pong consumers, BN = 128; 8 / 9 / 10 = one CTA with the
+// asynchronous whole-slab epilogue, BN = 128 / 192 / 256 (a call it cannot take runs variant 1 / 3 / 2)
+static int variant_bn(int v) {
+  return v == 0 ? 64 : (v == 1 || v == 6 || v == 7 || v == 8) ? 128 : (v == 3 || v == 5 || v == 9) ? 192 : 256;
+}
 static int variant_cl(int v) { return v >= 4 && v <= 6 ? 2 : 1; }
+static bool variant_async(int v) { return v >= 8; }
+// the cooperative single-CTA variant of an asynchronous-epilogue variant's tile
+static int variant_coop(int v) { return v == 8 ? 1 : (v == 9 ? 3 : (v == 10 ? 2 : v)); }
 
 // Fixed cost of one work item in the persistent kernel, in k-block times of its tile: its epilogue and the hand-over to
 // the next item.  scripts/gpu_time_gemm.py --fixed-cost measured 13.4, 14.0, 10.0 and 5.0 us per extra 128 x 256 fp32
@@ -613,6 +769,12 @@ constexpr int KB_PER_ITEM_FIXED = 4;
 // decoders' bf16 forward GEMMs with N >= 768 at K = 256 4-5 % faster than the cooperative tiles, but the N = 256 and
 // dgrad (MN-major B) shapes 10-48 % slower, and the step as a whole slower than with the 128 x 192 tile alone; so the
 // model does not pick it, and variant 7 runs only when set.
+// The asynchronous-epilogue kernel (variants 8-10) leaves little of that: measured as the bf16 items above (N = 768, a
+// bias), 128 x 128 items cost 2.1 (K = 256) and 2.5 (K = 768) k-block times of 0.392 us, 128 x 192 3.6 and 5.1 of
+// 0.516 us, 128 x 256 2.8 and 1.5 of 0.752 us; fp32 128 x 128 items without a bias 2.1 and 5.6 of 0.349 us, against
+// 5.6 and 4.5 for the cooperative kernel's (same card and limit).  The model takes 2.  Its unsplit candidates all
+// share the constant, so for bf16 outputs it picks the tile width the cooperative kernel had.
+constexpr int ASYNC_KB_PER_ITEM_FIXED = 2;
 // Split-K never cuts an item below this many k-blocks, which bounds the fp32 reduce-add traffic it adds
 constexpr int MIN_KB_PER_SPLIT = 16;
 // Deterministic mode: the automatic split makes ceil(k-blocks / DET_KB_PER_SPLIT) splits of equal k-block counts, so
@@ -666,6 +828,11 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   const int tm = ceil_div(M, BM);
   if (split_k <= 0 && !(ep->out_f32 && !ep->out_bf16 && !ep->preact_bf16 && !ep->dgelu_z && ep->act == 0)) split_k = 1;
   if (det && split_k <= 0) split_k = ceil_div(num_kb, DET_KB_PER_SPLIT);
+  // unsplit, the output leaves through a plain TMA store: the asynchronous-epilogue kernel can take the call (bf16 at
+  // every width it has, fp32 at BN = 128)
+  const bool async_ok = g_gemm_tma_store && split_k <= 1 && !ep->accumulate && ep->act == 0 && !ep->residual &&
+                        !ep->preact_bf16 && !ep->dgelu_z && (!ep->out_bf16 != !ep->out_f32);
+  const bool async_f32 = ep->out_f32 != nullptr;
 
   // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time (clusters:
   // sm_count() / 2 items of 256 rows), so a launch lasts ceil(items / slots) rounds of one item, and an item costs
@@ -675,24 +842,37 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   // rounds of 132 SMs, against 297 of 128 x 256 in 2.25.  The automatic split (split_k <= 0) fills the last round of the
   // long-K weight gradients instead of leaving it mostly idle.  An explicit variant fixes the tile, an explicit split_k
   // the split.
+  // The asynchronous-epilogue kernel replaces the cooperative one of its width among the candidates wherever it can
+  // take the call; its items, unsplit, cost ASYNC_KB_PER_ITEM_FIXED.
   int variant = g_gemm_variant;
   {
-    const int cand_var[3] = {1, 2, 3};
-    const int nvar = variant >= 0 ? 1 : 3;
+    int cand_var[4] = {1, 2, 3, -1};
+    if (async_ok) {
+      cand_var[0] = 8;
+      if (!async_f32) {
+        cand_var[1] = 10;
+        cand_var[2] = 9;
+      } else if (split_k <= 0) {
+        cand_var[3] = 1;   // the split forms of the 128-column tile stay open
+      }
+    }
+    const int nvar = variant >= 0 ? 1 : (cand_var[3] >= 0 ? 4 : 3);
     long best_cost = -1;
-    int best_split = 1, best_var = variant >= 0 ? variant : 1;
+    int best_split = 1, best_var = variant >= 0 ? variant : cand_var[0];
     for (int i = 0; i < nvar; ++i) {
       const int v = variant >= 0 ? variant : cand_var[i];
       const int bn = variant_bn(v), cl = variant_cl(v);
       if (variant < 0 && bn > 128 && N < bn) continue;
       const long tiles = long(ceil_div(tm, cl)) * ceil_div(N, bn);
       const int slots = std::max(1, sms / cl);
+      const bool ae = variant_async(v) && async_ok;
+      const int fixed = ae ? ASYNC_KB_PER_ITEM_FIXED : KB_PER_ITEM_FIXED;
       const int s_lo = split_k > 0 ? split_k : 1;
-      const int s_hi = split_k > 0 ? split_k : std::max(1, num_kb / MIN_KB_PER_SPLIT);
+      const int s_hi = split_k > 0 || ae ? s_lo : std::max(1, num_kb / MIN_KB_PER_SPLIT);
       for (int s = s_lo; s <= s_hi; ++s) {
         const int kbps = ceil_div(num_kb, std::min(s, num_kb));
         const long rounds = (tiles * ceil_div(num_kb, kbps) + slots - 1) / slots;
-        const long cost = rounds * (bn + 40) * cl * (kbps + KB_PER_ITEM_FIXED);
+        const long cost = rounds * (bn + 40) * cl * (kbps + fixed);
         if (best_cost < 0 || cost < best_cost) {
           best_cost = cost;
           best_split = s;
@@ -719,6 +899,9 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
 #undef MMAE_LD_OK
 
   const bool ordered = det && split_k > 1;
+  // a call the asynchronous-epilogue kernel cannot take (split, or an fp32 output wider than 128 columns) runs the
+  // cooperative kernel of the same width
+  if (variant_async(variant) && (!async_ok || split_k > 1 || (async_f32 && variant != 8))) variant = variant_coop(variant);
   // ordered split-K runs the cooperative single-CTA kernel of the same tile width
   if (ordered) variant = (variant == 6 || variant == 7) ? 1 : (variant == 4 ? 2 : (variant == 5 ? 3 : variant));
   if (variant == 5 && b_mn_major) variant = 4;   // an MN-major B half must be whole 64-column chunks
@@ -753,7 +936,12 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   // accumulation (split-K, accumulate) through TMA reduce-add tiles
   p.tma_store = 0;
   CUtensorMap tmC = tmA;
-  if (g_gemm_tma_store && !ep->preact_bf16 && !ep->dgelu_z && !ep->residual) {
+  if (variant_async(variant)) {
+    p.tma_store = async_f32 ? 2 : 1;
+    rc = async_f32 ? make_tmap_2d_store_sw128(&tmC, ep->out_f32, 4, (uint64_t)M, (uint64_t)N, (uint64_t)ep->ld_out_f32)
+                   : make_tmap_2d_store_sw128(&tmC, ep->out_bf16, 2, (uint64_t)M, (uint64_t)N, (uint64_t)ep->ld_out_bf16);
+    if (rc) return rc;
+  } else if (g_gemm_tma_store && !ep->preact_bf16 && !ep->dgelu_z && !ep->residual) {
     if (ep->out_bf16 && !ep->out_f32 && split_k == 1 && !ep->accumulate) {
       p.tma_store = 1;
       rc = make_tmap_2d_store(&tmC, ep->out_bf16, 2, (uint64_t)M, (uint64_t)N, (uint64_t)ep->ld_out_bf16);
@@ -792,6 +980,18 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     if (!a_mn_major) return launch_gemm<192, 2, false, false>(tmA, tmB, tmC, p, st);
     return launch_gemm<192, 2, true, false>(tmA, tmB, tmC, p, st);
   }
+#define MMAE_DISPATCH_AE(BN_, AE_)                                                                                \
+  do {                                                                                                            \
+    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, 1, false, false, false, false, AE_>(tmA, tmB, tmC, p, st); \
+    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, 1, false, true, false, false, AE_>(tmA, tmB, tmC, p, st);   \
+    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, 1, true, false, false, false, AE_>(tmA, tmB, tmC, p, st);   \
+    return launch_gemm<BN_, 1, true, true, false, false, AE_>(tmA, tmB, tmC, p, st);                                  \
+  } while (0)
+  if (variant == 8 && p.tma_store == 2) MMAE_DISPATCH_AE(128, 2);
+  if (variant == 8) MMAE_DISPATCH_AE(128, 1);
+  if (variant == 9) MMAE_DISPATCH_AE(192, 1);
+  if (variant == 10) MMAE_DISPATCH_AE(256, 1);
+#undef MMAE_DISPATCH_AE
   if (variant == 0) MMAE_DISPATCH(64, 1, false);
   if (variant == 3) MMAE_DISPATCH(192, 1, false);
   if (variant == 2) MMAE_DISPATCH(256, 1, false);

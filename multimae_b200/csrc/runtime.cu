@@ -135,6 +135,28 @@ int make_tmap_2d_store(CUtensorMap* out, const void* base, int elem_bytes, uint6
   return MMAE_OK;
 }
 
+// Output-tile map of the GEMM's whole-slab epilogue: box = 64 rows x 128 bytes (64 bf16 or 32 fp32 columns), staged
+// with the 128B swizzle so that the accumulator fragments go to shared memory without bank conflicts.
+int make_tmap_2d_store_sw128(CUtensorMap* out, const void* base, int elem_bytes, uint64_t rows, uint64_t cols,
+                             uint64_t ld) {
+  encode_tiled_fn fn = get_encode_fn();
+  if (!fn) return MMAE_ERR_CUDA;
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {ld * (uint64_t)elem_bytes};
+  cuuint32_t box[2] = {128u / (uint32_t)elem_bytes, 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                  const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled(store, sw128) failed: %d (rows=%llu cols=%llu ld=%llu base=%p)", (int)r,
+                   (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld, base);
+    return MMAE_ERR_CUDA;
+  }
+  return MMAE_OK;
+}
+
 int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t s1,
                       uint64_t s2, uint32_t b0, uint32_t b1, uint32_t b2) {
   encode_tiled_fn fn = get_encode_fn();
@@ -281,7 +303,8 @@ extern "C" int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launch
   return MMAE_OK;
 }
 
-// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bit2 ping-pong, bits 8.. split_k); returns
+// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bit2 ping-pong, bit3 ordered split-K, bit4
+// asynchronous epilogue, bits 8.. split_k); returns
 // bytes written
 extern "C" int64_t mmae_profile_gemm_dump(char* buf, int64_t cap) {
   int64_t off = 0;

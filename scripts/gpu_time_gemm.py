@@ -3,6 +3,7 @@
     python scripts/gpu_time_gemm.py               # every distinct GEMM shape / operand-major combination of the step
     python scripts/gpu_time_gemm.py --fixed-cost  # per-tile fixed cost: intercept of time over k-blocks
     python scripts/gpu_time_gemm.py --variant 7   # the step's shapes on one tile variant (mmae_gemm_set_variant)
+    python scripts/gpu_time_gemm.py --variant 3 9 # ... on several, side by side (wgrad shapes included)
 
 Shapes: encoder M = 128 x 99 tokens (D 768, MLP 3072), decoders M = 128 x 196 query tokens and 128 x 99 context tokens
 (D 256, MLP 1024), with the epilogue each call has in the step: forward = bf16 out + bias, dgrad = bf16 out with an
@@ -14,7 +15,8 @@ dense BF16 rate (989 TFLOP/s).
 12 split-K work items per SM.  The MMA work stays the same, so the time added per extra item is the fixed cost of one
 item: its epilogue, its reduce-add traffic and the hand-over between items.  (One tile per SM at K = 64 against K = 768
 does not isolate it: at K = 64 a tile's output write takes longer than its one k-block of MMAs.)  It then times
-bf16-output items with a bias, as the forward GEMMs run them, at K = 256 and 768 for each tile of VARIANT_BN
+bf16-output items with a bias, as the forward GEMMs run them, at K = 256 and 768 for each tile of VARIANT_BN, and
+fp32-output items without one for the 128-column tiles of the cooperative and asynchronous-epilogue kernels
 (fixed_cost_bf16)."""
 import argparse
 import os
@@ -49,7 +51,9 @@ SHAPES = [
     ("dec", "context proj wgrad", 1024, 768, DC, "wgrad"),
 ]
 PEAK_TFLOPS = 989.0
-VARIANT_BN = {1: 128, 2: 256, 7: 128}   # variants timed by --fixed-cost (7: ping-pong): their output tile width
+# variants timed by --fixed-cost (7: ping-pong, 8 / 9 / 10: asynchronous epilogue): their output tile width
+VARIANT_BN = {1: 128, 3: 192, 2: 256, 7: 128, 8: 128, 9: 192, 10: 256}
+F32_VARIANTS = (1, 8)
 
 
 def timed(fn, n=50):
@@ -88,14 +92,23 @@ def gemm_call(dev, M, N, K, kind):
     return lambda: KN.gemm(A, B, a_mn=True, b_mn=True, out_f32=out, accumulate=True, split_k=0)
 
 
-def shapes(variant):
+def shapes(variants):
+    """Microseconds per call of every shape under each variant in turn (TF/s and share of peak for the first)."""
     dev = torch.device("cuda:0")
-    L.lib().mmae_gemm_set_variant(variant)
-    print("%-16s %-26s %6s %5s %6s %-5s %9s %7s %6s" % ("class", "gemm", "M", "N", "K", "kind", "us", "TF/s", "%989"))
-    for cls, name, M, N, K, kind in SHAPES:
-        us = timed(gemm_call(dev, M, N, K, kind))
-        tf = 2.0 * M * N * K / (us * 1e-6) / 1e12
-        print("%-16s %-26s %6d %5d %6d %-5s %9.1f %7.1f %6.1f" % (cls, name, M, N, K, kind, us, tf, 100 * tf / PEAK_TFLOPS))
+    print("%-16s %-26s %6s %5s %6s %-5s" % ("class", "gemm", "M", "N", "K", "kind") +
+          "".join(" %9s" % ("us v%d" % v) for v in variants) + " %7s %6s" % ("TF/s", "%989"))
+    try:
+        for cls, name, M, N, K, kind in SHAPES:
+            call = gemm_call(dev, M, N, K, kind)
+            us = []
+            for v in variants:
+                L.lib().mmae_gemm_set_variant(v)
+                us.append(timed(call))
+            tf = 2.0 * M * N * K / (us[0] * 1e-6) / 1e12
+            print("%-16s %-26s %6d %5d %6d %-5s" % (cls, name, M, N, K, kind) + "".join(" %9.1f" % u for u in us) +
+                  " %7.1f %6.1f" % (tf, 100 * tf / PEAK_TFLOPS))
+    finally:
+        L.lib().mmae_gemm_set_variant(-1)
 
 
 def fixed_cost():
@@ -127,8 +140,9 @@ def fixed_cost_bf16(dev, sms):
     (3 -> 12); k-block time = slope of the per-item time over K (768 -> 3072); fixed cost = per-item time minus the item's
     k-blocks at that rate: the epilogue and the hand-over that the tensor cores do not overlap."""
     N = 768
-    print("%-8s %-7s %5s %10s %12s %12s %12s" % ("variant", "tile", "K", "us/item", "us/k-block", "fixed us", "fixed k-blk"))
-    for variant in sorted(VARIANT_BN):
+    print("%-8s %-7s %-5s %5s %10s %12s %12s %12s" % ("variant", "tile", "out", "K", "us/item", "us/k-block", "fixed us",
+                                                     "fixed k-blk"))
+    for variant, f32 in [(v, False) for v in sorted(VARIANT_BN)] + [(v, True) for v in F32_VARIANTS]:
         bn = VARIANT_BN[variant]
         tiles_n = N // bn
         bias = torch.randn(N, device=dev)
@@ -142,8 +156,12 @@ def fixed_cost_bf16(dev, sms):
                     assert sms * n % tiles_n == 0
                     M = 128 * sms * n // tiles_n
                     A = rnd(dev, M, K)
-                    out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
-                    t[n] = timed(lambda: KN.gemm(A, B, bias=bias, out_bf16=out), n=100)
+                    if f32:
+                        out = torch.empty(M, N, device=dev)
+                        t[n] = timed(lambda: KN.gemm(A, B, out_f32=out), n=100)
+                    else:
+                        out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
+                        t[n] = timed(lambda: KN.gemm(A, B, bias=bias, out_bf16=out), n=100)
                     del A, out
                 per_item[K] = (t[12] - t[3]) / 9
         finally:
@@ -151,13 +169,15 @@ def fixed_cost_bf16(dev, sms):
         kb = (per_item[3072] - per_item[768]) / ((3072 - 768) // 64)
         for K in (256, 768):
             fixed = per_item[K] - K // 64 * kb
-            print("%-8d %-7s %5d %10.3f %12.3f %12.3f %12.2f" % (variant, "128x%d" % bn, K, per_item[K], kb, fixed, fixed / kb))
+            print("%-8d %-7s %-5s %5d %10.3f %12.3f %12.3f %12.2f" % (variant, "128x%d" % bn, "fp32" if f32 else "bf16", K,
+                                                                     per_item[K], kb, fixed, fixed / kb))
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--fixed-cost", action="store_true", help="time the per-tile fixed cost instead of the step's shapes")
-    ap.add_argument("--variant", type=int, default=-1, help="tile variant of every call (-1: the heuristic's choice)")
+    ap.add_argument("--variant", type=int, nargs="+", default=[-1],
+                    help="tile variant(s) of every call (-1: the heuristic's choice), timed side by side")
     a = ap.parse_args()
     torch.manual_seed(0)
     print("# %s (name, power limit, SM clock, max SM clock; before)" % gpu_state())
