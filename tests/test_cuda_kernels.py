@@ -1,7 +1,8 @@
 """GPU: every primitive of the C ABI against a plain PyTorch fp32 computation of the same op on the same inputs.
 
 Tolerances: fp32-accumulating GEMM on bf16 inputs vs fp32 matmul of the same bf16 values: 3e-5 relative L2 (accumulation
-order only); outputs rounded to bf16: 4e-3; attention (bf16 P / dS operands): 1e-2; fp32 element-wise kernels: 1e-5."""
+order only); outputs rounded to bf16: 4e-3; fp32 element-wise kernels: 1e-5.  Attention, both tiers, is held to float64
+element by element in test_cuda_attention_float64.py."""
 import os
 
 import pytest
@@ -198,48 +199,6 @@ def test_layernorm(dev, KN, shape):
     assert rel_l2(dgam, gr.grad + g0.double()) < 1e-4 and rel_l2(dbet, br.grad + b0.double()) < 1e-4
 
 
-ATTN_CASES = [(3, 12, 99, 99, 64, True), (2, 8, 196, 99, 32, False), (2, 8, 196, 196, 32, True), (1, 2, 393, 393, 64, True),
-              (1, 2, 130, 70, 32, False), (2, 1, 17, 5, 64, False), (2, 16, 99, 99, 64, True), (2, 3, 128, 128, 64, True),
-              (1, 2, 100, 33, 64, False), (1, 2, 256, 256, 64, True), (1, 4, 200, 129, 32, False), (5, 8, 196, 196, 32, True)]
-
-
-# switch values (attention.cu): 0 = mma.sync kernels everywhere; 1 = wgmma forward for <= 128 keys only; 3, 7, 15, 19, 195,
-# 99 = wgmma forward wherever it applies (<= 256 keys), mma.sync above 256 keys and for the backward
-@pytest.mark.parametrize("tc", [0, 1, 3, 7, 15, 19, 195, 99])
-@pytest.mark.parametrize("case", ATTN_CASES)
-def test_attention_forward_backward(dev, KN, tc, case):
-    from multimae_b200 import _lib as L
-    L.lib().mmae_attention_set_tc(tc)
-    B, H, Nq, Nk, dh, self_attn = case
-    D, scale = H * dh, dh ** -0.5
-    if self_attn:
-        qkv = _bf16(dev, B * Nq, 3 * D)
-        q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
-    else:
-        q, kv = _bf16(dev, B * Nq, D), _bf16(dev, B * Nk, 2 * D)
-        k, v = kv[:, :D], kv[:, D:]
-    o, lse = KN.attention_fwd(q, k, v, B, H, Nq, Nk, dh, scale)
-    qf = q.float().reshape(B, Nq, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    kf = k.float().reshape(B, Nk, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    vf = v.float().reshape(B, Nk, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    s = (qf @ kf.transpose(-2, -1)) * scale
-    ref = (torch.softmax(s, -1) @ vf).transpose(1, 2).reshape(B * Nq, D)
-    assert rel_l2(o, ref) < 1e-2 and rel_l2(lse, torch.logsumexp(s, -1)) < 1e-4
-    do = _bf16(dev, B * Nq, D)
-    ref.backward(do.float())
-    if self_attn:
-        dqkv = torch.empty(B * Nq, 3 * D, device=dev, dtype=torch.bfloat16)
-        dq, dk, dv = dqkv[:, :D], dqkv[:, D:2 * D], dqkv[:, 2 * D:]
-    else:
-        dq = torch.empty(B * Nq, D, device=dev, dtype=torch.bfloat16)
-        dkv = torch.empty(B * Nk, 2 * D, device=dev, dtype=torch.bfloat16)
-        dk, dv = dkv[:, :D], dkv[:, D:]
-    KN.attention_bwd(q, k, v, o, do, lse, dq, dk, dv, B, H, Nq, Nk, dh, scale)
-    assert rel_l2(dq, qf.grad.transpose(1, 2).reshape(B * Nq, D)) < 1e-2
-    assert rel_l2(dk, kf.grad.transpose(1, 2).reshape(B * Nk, D)) < 1e-2
-    assert rel_l2(dv, vf.grad.transpose(1, 2).reshape(B * Nk, D)) < 1e-2
-
-
 @pytest.mark.parametrize("case", [(3, 3, 14, 14, 16), (2, 1, 14, 14, 16), (2, 133, 14, 14, 4), (2, 5, 3, 7, 8), (1, 2, 2, 3, 4)])
 def test_unpatchify_and_patchify_bf16(dev, case):
     """tokens [B*nh*nw, C*P*P] (c, py, px) <-> image [B, C, nh*P, nw*P] (output_adapters.py:277-280), strided token rows."""
@@ -305,7 +264,7 @@ def test_standardize_depth_against_oracle_and_golden(dev, golden_dir, variant):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# fp32 tier primitives (fp32_output_adapters): 3 x bf16 split Linear, fp32 attention, fp32 GELU
+# fp32 tier primitives (fp32_output_adapters): 3 x bf16 split Linear, fp32 GELU
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("shape", [(48, 2128, 128), (392, 256, 768), (1000, 1024, 256), (48, 128, 128)])
 def test_linear_f32_split_gemm(dev, shape):
@@ -332,40 +291,6 @@ def test_linear_f32_split_gemm(dev, shape):
     assert rel_l2(dx, (dy.double() @ W.double()).float()) < 2e-5
     assert rel_l2(dW - 0.5, (dy.double().t() @ x.double()).float()) < 2e-5
     assert rel_l2(db - 0.25, dy.double().sum(0).float()) < 1e-5
-
-
-@pytest.mark.parametrize("case", [(3, 4, 16, 13), (2, 8, 196, 99), (2, 8, 196, 196), (1, 2, 130, 70)])
-def test_attention_f32(dev, case):
-    from multimae_b200 import _lib as L
-    lib = L.lib()
-    B, H, Nq, Nk = case
-    dh, D = 32, H * 32
-    scale = dh ** -0.5
-    q = torch.randn(B * Nq, D, device=dev)
-    kv = torch.randn(B * Nk, 2 * D, device=dev)
-    k, v = kv[:, :D], kv[:, D:]
-    o = torch.empty(B * Nq, D, device=dev)
-    lse = torch.empty(B, H, Nq, device=dev)
-    L.check(lib.mmae_attention_f32_forward(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
-                                           o.data_ptr(), o.stride(0), lse.data_ptr(), B, H, Nq, Nk, dh, scale, L.current_stream()))
-    qf = q.double().reshape(B, Nq, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    kf = k.double().reshape(B, Nk, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    vf = v.double().reshape(B, Nk, H, dh).transpose(1, 2).detach().requires_grad_(True)
-    s = (qf @ kf.transpose(-2, -1)) * scale
-    ref = (torch.softmax(s, -1) @ vf).transpose(1, 2).reshape(B * Nq, D)
-    assert rel_l2(o, ref.float()) < 1e-5 and rel_l2(lse, torch.logsumexp(s, -1).float()) < 1e-5
-    do = torch.randn(B * Nq, D, device=dev)
-    ref.backward(do.double())
-    dq = torch.empty_like(q)
-    dkv = torch.empty_like(kv)
-    delta = torch.empty(B, H, Nq, device=dev)
-    L.check(lib.mmae_attention_f32_backward(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
-                                            o.data_ptr(), o.stride(0), do.data_ptr(), do.stride(0), lse.data_ptr(),
-                                            delta.data_ptr(), dq.data_ptr(), dq.stride(0), dkv.data_ptr(), dkv.stride(0),
-                                            dkv[:, D:].data_ptr(), dkv.stride(0), B, H, Nq, Nk, dh, scale, L.current_stream()))
-    assert rel_l2(dq, qf.grad.transpose(1, 2).reshape(B * Nq, D).float()) < 1e-5
-    assert rel_l2(dkv[:, :D], kf.grad.transpose(1, 2).reshape(B * Nk, D).float()) < 1e-5
-    assert rel_l2(dkv[:, D:], vf.grad.transpose(1, 2).reshape(B * Nk, D).float()) < 1e-5
 
 
 def test_gelu_f32(dev):
