@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MMAE_ABI_VERSION 23
+#define MMAE_ABI_VERSION 24
 
 int mmae_abi_version(void);
 const char* mmae_last_error(void);
@@ -35,9 +35,8 @@ int64_t mmae_launch_count(void);
  * recorded events and returns the summed algorithmic FLOPs (2*M*N*K), summed kernel milliseconds and launch count. */
 int mmae_profile_gemm(int enable);
 int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launches);
-/* text dump, one line per recorded launch: "M N K flags ms" (flags: bit0 A MN-major, bit1 B MN-major, bit2 ping-pong
- * kernel (variant 7), bit3 ordered split-K (deterministic mode), bit4 asynchronous-epilogue kernel (variants 8-10),
- * bits 8+ split_k) */
+/* text dump, one line per recorded launch: "M N K flags ms" (flags: bit0 A MN-major, bit1 B MN-major, bit2 unused,
+ * bit3 ordered split-K (deterministic mode), bit4 asynchronous-epilogue kernel (variants 8-10), bits 8+ split_k) */
 int64_t mmae_profile_gemm_dump(char* buf_host, int64_t capacity);
 
 /* ------------------------------------------------------------------------------------------------
@@ -76,13 +75,12 @@ typedef struct mmae_gemm_epilogue {
   int64_t ld_residual, ld_dgelu_z, ld_preact, ld_out_f32, ld_out_bf16;
 } mmae_gemm_epilogue;
 
-/* Kernel variant for measurements: -1 = heuristic (default), 0 / 1 / 3 / 2 = one CTA per 128 x 64 / 128 / 192 / 256
- * tile, 6 / 5 / 4 = two-CTA cluster per 256 x 128 / 192 / 256 tile (the B tile loaded once and multicast to both CTAs),
- * 7 = one CTA per SM whose two consumer warpgroups each own whole 128 x 128 tiles and take turns on the tensor cores
- * (ping-pong), 8 / 9 / 10 = one CTA per 128 x 128 / 192 / 256 tile whose consumers stage each output slab whole and
- * start the next tile's MMAs while its TMA stores drain (unsplit bf16 outputs, or fp32 outputs at 128 columns, with
- * alpha and an optional bias only; any other call runs variant 1 / 3 / 2).  The heuristic (-1) runs the 8 / 9 / 10
- * kernels wherever they can take the call.  Env MMAE_GEMM_VARIANT sets the initial value. */
+/* Kernel variant for measurements: -1 = heuristic (default), 1 / 3 / 2 = one CTA per 128 x 128 / 192 / 256 tile whose
+ * consumers run each tile's epilogue together, 8 / 9 / 10 = one CTA per 128 x 128 / 192 / 256 tile whose consumers
+ * stage each output slab whole and start the next tile's MMAs while its TMA stores drain (unsplit bf16 outputs, or fp32
+ * outputs at 128 columns, with alpha and an optional bias only; any other call runs variant 1 / 3 / 2).  Any other
+ * value is rejected (MMAE_ERR_ARG).  The heuristic (-1) runs the 8 / 9 / 10 kernels wherever they can take the call.
+ * Env MMAE_GEMM_VARIANT sets the initial value (-1 if it names no variant). */
 int mmae_gemm_set_variant(int variant);
 /* 1 (default): plain bf16 / fp32 outputs (optionally with bias / GELU) leave through shared memory + TMA tile stores, fp32
  * accumulation (split-K, accumulate) through TMA reduce-add tiles; 0: per-thread global stores / red.global adds.

@@ -297,17 +297,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// same, multicast: the tile lands at the same shared-memory offset in every CTA of `cta_mask`, each of whose mbarriers at
-// the offset of `bar` receives the transaction bytes
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], "
-      "[%2], %5;"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
 // 2D tile store shared -> global (bulk async group completion); out-of-bounds parts of the box are clipped by the TMA unit
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
@@ -399,11 +388,6 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
   d |= uint64_t((sbo_bytes >> 4) & 0x3FFFu) << 32;
   d |= uint64_t(1) << 62;
   return d;
-}
-
-// arrive (count 1) on the mbarrier at cluster address `mbar_cluster` (mapa of a barrier in this or a peer CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t mbar_cluster) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mbar_cluster) : "memory");
 }
 
 // Shared-memory matrix descriptor, no swizzle (K-major "interleave" layout): 8 x 8 bf16 core matrices of 128 contiguous

@@ -1,26 +1,20 @@
 // wgmma / TMA GEMM for sm_90a:  C[M,N] = epilogue(alpha * A * B^T), bf16 operands, fp32 accumulate in registers.
 //
-// Persistent: the grid holds at most one CTA (or two-CTA cluster) per SM, and each walks a fixed sequence of work items.
-// A work item is one 128 x BN output tile (BN = 64 / 128 / 192 / 256) over one K range (split-K).  CTA c of a grid of
-// g takes items c, c + g, c + 2g, ...; items are ordered n-tile fastest, then m-tile, then split, so the CTAs running
-// at the same time share their A rows (the large, token-sized operand) and the whole of B stays in L2.  Three
-// warpgroups:
+// Persistent: the grid holds at most one CTA per SM, and each walks a fixed sequence of work items.  A work item is one
+// 128 x BN output tile (BN = 128 / 192 / 256) over one K range (split-K).  CTA c of a grid of g takes items c, c + g,
+// c + 2g, ...; items are ordered n-tile fastest, then m-tile, then split, so the CTAs running at the same time share
+// their A rows (the large, token-sized operand) and the whole of B stays in L2.  Three warpgroups:
 //   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled shared-memory ring, mbarrier
 //                    complete_tx); gives its registers to the consumers (setmaxnreg).  Ring slot and phase follow a
 //                    k-block count that runs across work items, so the next item's stages load during an epilogue.
-//   warpgroups 1-2 : consumers: wgmma 64 x BN x 16 straight from the ring (K-major or MN-major operands through the
-//                    descriptor's transpose bit), then the fused epilogue from the accumulator registers (bias / GELU /
-//                    dGELU / residual, bf16 and fp32 outputs, red.global adds for split-K), or for plain bf16 / fp32
-//                    outputs through a staging area of their own and TMA tile stores / reduce-adds.  Two schemes:
-//     cooperative (gemm_bf16_kernel): both consumers work on every item, 64 rows each, and run its epilogue together
-//                    while the tensor cores idle.
-//     ping-pong (gemm_bf16_pingpong_kernel, BN = 128, one CTA): consumer i owns the CTA's items i, i + 2, ..., all 128
-//                    rows, and the two take turns on the mainloop, so one's epilogue runs under the other's MMAs.
-//                    ptxas: 168 registers per thread (the consumers raise theirs to 232), no spills; 230,656 bytes of
-//                    dynamic shared memory (6 x 32 KB stages + 2 x 16 KB staging), GemmCfg<128>'s.
-// CL = 2: a cluster of two CTAs along M shares the B tile - each CTA loads half of it and multicasts it to both, so a
-// 256 x BN output tile reads B from L2 once.  Both CTAs walk the same item sequence (one M-half each), so their rings
-// stay in lockstep; a stage is refilled only after the consumers of BOTH CTAs released it.
+//   warpgroups 1-2 : consumers: both work on every item, 64 rows each, with wgmma 64 x BN x 16 straight from the ring
+//                    (K-major or MN-major operands through the descriptor's transpose bit).  Two schemes:
+//     cooperative (gemm_bf16_kernel): the two run the item's fused epilogue together while the tensor cores idle:
+//                    from the accumulator registers (bias / GELU / dGELU / residual, bf16 and fp32 outputs, red.global
+//                    adds for split-K), or for plain bf16 / fp32 outputs through a staging area of their own and TMA
+//                    tile stores / reduce-adds.
+//     asynchronous epilogue (gemm_async_epi_kernel, unsplit plain bf16 / fp32 outputs): each stages its whole slab and
+//                    goes on to the next item's MMAs while the TMA stores drain.
 //
 #include <algorithm>
 #include <cstdlib>
@@ -47,17 +41,17 @@ struct GemmParams {
   int num_kb;        // total k-blocks (ceil(K / BK))
   int kb_per_split;  // k-blocks handled by one split
   int tiles_n;       // ceil(N / BN)
-  int tiles_m;       // M units of one CTA (CL = 1) or one cluster (CL = 2): ceil(ceil(M / BM) / CL)
+  int tiles_m;       // ceil(M / BM)
   int splits;
   int tma_store;     // output through shared memory + TMA: 1 = bf16 store, 2 = fp32 store, 3 = fp32 reduce-add
   mmae_gemm_epilogue ep;
 };
 
-// ~192 KB of stages (BN = 64: 8 x 24 KB, 128: 6 x 32 KB, 192: 4 x 40 KB, 256: 4 x 48 KB) + 32 KB of TMA-store staging
-// (per consumer warpgroup 16 KB: two 64 x 32 fp32 boxes or four bf16 boxes, used in turn).  One CTA per SM.
+// ~192 KB of stages (BN = 128: 6 x 32 KB, 192: 4 x 40 KB, 256: 4 x 48 KB) + 32 KB of TMA-store staging (per consumer
+// warpgroup 16 KB: two 64 x 32 fp32 boxes or four bf16 boxes, used in turn).  One CTA per SM.
 template <int BN>
 struct GemmCfg {
-  static constexpr int STAGES = BN == 256 ? 4 : (BN == 192 ? 4 : (BN == 128 ? 6 : 8));
+  static constexpr int STAGES = BN == 128 ? 6 : 4;
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
@@ -72,13 +66,13 @@ struct WorkItem {
   int m0, n0, split, kb_begin, nkb;
 };
 
-template <int BN, int CL>
-__device__ __forceinline__ WorkItem decode_item(int item, const GemmParams& p, int rank) {
+template <int BN>
+__device__ __forceinline__ WorkItem decode_item(int item, const GemmParams& p) {
   WorkItem w;
   const int rest = item / p.tiles_n;
   w.n0 = (item - rest * p.tiles_n) * BN;
   w.split = rest / p.tiles_m;
-  w.m0 = ((rest - w.split * p.tiles_m) * CL + rank) * BM;
+  w.m0 = (rest - w.split * p.tiles_m) * BM;
   w.kb_begin = w.split * p.kb_per_split;
   w.nkb = min(p.kb_per_split, p.num_kb - w.kb_begin);   // >= 1: the host never makes an empty split
   return w;
@@ -137,16 +131,14 @@ __device__ __forceinline__ void stage_pair(uint8_t* box, int r, int c, float v0,
 // TMA producer (one thread): walks the CTA's items in order and fills the ring; slot and phase follow a k-block count
 // that runs across items, so the next item's stages load while the consumers finish the current one.  STAGES: the
 // ring's depth (the stage layout is GemmCfg<BN>'s whatever the depth)
-template <int BN, int CL, bool A_MN, bool B_MN, int STAGES = GemmCfg<BN>::STAGES>
+template <int BN, bool A_MN, bool B_MN, int STAGES = GemmCfg<BN>::STAGES>
 __device__ __forceinline__ void produce(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, const CUtensorMap* tmA,
-                                        const CUtensorMap* tmB, const GemmParams& p, int rank, int first_item,
-                                        int item_stride, int num_items) {
+                                        const CUtensorMap* tmB, const GemmParams& p, int first_item, int item_stride,
+                                        int num_items) {
   using C = GemmCfg<BN>;
-  constexpr int BH = BN / CL;   // B rows (output columns) this CTA loads
-  static_assert(!B_MN || BH % 64 == 0, "MN-major B is loaded in 64-column chunks");
   uint32_t it = 0;   // k-blocks loaded so far, over all items
   for (int item = first_item; item < num_items; item += item_stride) {
-    const WorkItem w = decode_item<BN, CL>(item, p, rank);
+    const WorkItem w = decode_item<BN>(item, p);
     for (int kb = 0; kb < w.nkb; ++kb, ++it) {
       const int s = it % STAGES;
       const uint32_t ph = (it / STAGES) & 1;
@@ -161,22 +153,11 @@ __device__ __forceinline__ void produce(uint8_t* smem, uint64_t* full_bar, uint6
 #pragma unroll
         for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * (64 * BK * 2), tmA, &full_bar[s], w.m0 + c * 64, k0);
       }
-      if constexpr (CL == 1) {
-        if constexpr (!B_MN) {
-          tma_load_2d(sB, tmB, &full_bar[s], k0, w.n0);
-        } else {
-#pragma unroll
-          for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), tmB, &full_bar[s], w.n0 + c * 64, k0);
-        }
+      if constexpr (!B_MN) {
+        tma_load_2d(sB, tmB, &full_bar[s], k0, w.n0);
       } else {
-        if constexpr (!B_MN) {
-          tma_load_2d_multicast(sB + rank * BH * 128, tmB, &full_bar[s], k0, w.n0 + rank * BH, 0x3);
-        } else {
 #pragma unroll
-          for (int c = 0; c < BH / 64; ++c)
-            tma_load_2d_multicast(sB + (rank * (BH / 64) + c) * (64 * BK * 2), tmB, &full_bar[s],
-                                  w.n0 + rank * BH + c * 64, k0, 0x3);
-        }
+        for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * (64 * BK * 2), tmB, &full_bar[s], w.n0 + c * 64, k0);
       }
     }
   }
@@ -199,8 +180,7 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], const uint8_t* 
                              : gmma_desc_sw128(b_addr + j * (WG_K * 2), 16, 1024);
     if constexpr (BN == 256) wgmma_m64n256k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
     else if constexpr (BN == 192) wgmma_m64n192k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-    else if constexpr (BN == 128) wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
-    else wgmma_m64n64k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
+    else wgmma_m64n128k16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, sd);
   }
 }
 
@@ -288,109 +268,15 @@ __device__ __forceinline__ void epilogue_slab(const float (&acc)[BN / 2], int ro
 }
 
 // Cooperative consumers: both warpgroups work on the same item, 64 rows each, and run its epilogue together.
-// ORD (ordered split-K, deterministic mode; CL = 1, p.tma_store = 2): split s stores its tile into rows
+// ORD (ordered split-K, deterministic mode; p.tma_store = 2): split s stores its tile into rows
 // [s * tiles_m * BM, (s + 1) * tiles_m * BM) of the workspace map tmC, and splitk_reduce_kernel adds the slices in order.
-template <int BN, int CL, bool A_MN, bool B_MN, bool ORD = false>
+template <int BN, bool A_MN, bool B_MN, bool ORD = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   // the grid is never larger than what is co-resident (launch_gemm), so every item runs on a CTA that already holds its
   // SM: a dependent kernel released here can only take SMs this grid does not use
   pdl_launch_dependents();   // the wait follows the barrier setup below
-  using C = GemmCfg<BN>;
-  constexpr int STAGES = C::STAGES;
-
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  const int wg = threadIdx.x >> 7;
-  const int rank = CL > 1 ? int(cluster_ctarank()) : 0;
-  const int num_items = p.tiles_n * p.tiles_m * p.splits;
-  const int first_item = blockIdx.x / CL;
-  const int item_stride = gridDim.x / CL;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    if (p.tma_store) tma_prefetch_desc(&tmC);
-#pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2 * CL);   // one arrival per consumer warpgroup of every CTA the stage is multicast to
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();   // the peer's barriers exist before any multicast / remote arrival
-  pdl_wait();   // the previous kernel's outputs (our operands) are complete and visible from here on
-
-  if (wg == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) produce<BN, CL, A_MN, B_MN>(smem, full_bar, empty_bar, &tmA, &tmB, p, rank, first_item,
-                                                      item_stride, num_items);
-  } else {
-    // ------------------------------------------------------------------ consumers (warpgroups 1, 2)
-    setmaxnreg_inc<232>();
-    const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
-    const int t = threadIdx.x & 127;
-    uint8_t* epi = smem + C::EPI_OFFSET + cw * (2 * C::EPI_BOX_BYTES);
-    uint32_t it = 0;       // k-blocks consumed so far, over all items
-    uint32_t boxes = 0;    // TMA-store boxes issued so far by this warpgroup
-    // frees ring stage `s` in this CTA and, for a cluster, in the peer whose multicast also fills it
-    auto release = [&](int s) {
-      if (t == 0) {
-        if constexpr (CL == 1) mbar_arrive(&empty_bar[s]);
-        else
-          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa_u32(smem_u32(&empty_bar[s]), uint32_t(r)));
-      }
-    };
-    float acc[BN / 2];   // written by each item's first wgmma (scale-d = 0)
-
-    for (int item = first_item; item < num_items; item += item_stride) {
-      const WorkItem w = decode_item<BN, CL>(item, p, rank);
-      for (int kb = 0; kb < w.nkb; ++kb, ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-        wgmma_fence();
-        mma_kblock<BN, A_MN, B_MN>(acc, smem + s * C::STAGE_BYTES, cw, kb == 0);
-        wgmma_commit();
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
-        if (kb > 0) release((it - 1) % STAGES);
-      }
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
-      release((it - 1) % STAGES);   // the producer refills it with the next item's operands during the epilogue
-      const int slice_row = ORD ? w.split * p.tiles_m * BM : 0;
-      epilogue_slab<BN>(acc, slice_row + w.m0 + cw * 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
-    }
-    if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
-  }
-  // no CTA of a cluster may leave while its peer can still arrive on its barriers
-  if constexpr (CL > 1) cluster_sync_all();
-}
-
-// Ping-pong consumers: warpgroup i takes the CTA's items i, i + 2, i + 4, ..., all 128 rows of each (two 64-row slabs of
-// MMAs per k-step, 2 x BN / 2 accumulators per thread).  Named barriers 4 and 5 make the two take turns on the
-// mainloop: warpgroup 1 starts an item's MMAs once warpgroup 0 has issued the last of its item's, and the other way
-// round, so one warpgroup's epilogue runs while the other's MMAs keep the tensor cores busy.  The ring is the
-// cooperative kernel's, filled in the same order, but each stage has one consumer: its empty barrier takes 1 arrival.
-// Each slab sees the same wgmma sequence and epilogue as the cooperative kernel's warpgroup for it, so the two kernels'
-// outputs are bitwise equal.
-template <int BN, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-    gemm_bf16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                              const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-  pdl_launch_dependents();   // as in gemm_bf16_kernel
   using C = GemmCfg<BN>;
   constexpr int STAGES = C::STAGES;
 
@@ -412,67 +298,51 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);   // released by the one warpgroup whose item the stage holds
+      mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
+  pdl_wait();   // the previous kernel's outputs (our operands) are complete and visible from here on
 
   if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) produce<BN, 1, A_MN, B_MN>(smem, full_bar, empty_bar, &tmA, &tmB, p, 0, first_item,
-                                                     item_stride, num_items);
+    if (threadIdx.x == 0) produce<BN, A_MN, B_MN>(smem, full_bar, empty_bar, &tmA, &tmB, p, first_item, item_stride,
+                                                  num_items);
   } else {
+    // ------------------------------------------------------------------ consumers (warpgroups 1, 2)
     setmaxnreg_inc<232>();
-    const int cw = wg - 1;                 // takes the CTA's items cw, cw + 2, ...
+    const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
     const int t = threadIdx.x & 127;
     uint8_t* epi = smem + C::EPI_OFFSET + cw * (2 * C::EPI_BOX_BYTES);
-    uint32_t it = 0;       // k-blocks of the CTA's items before the current one
+    uint32_t it = 0;       // k-blocks consumed so far, over all items
     uint32_t boxes = 0;    // TMA-store boxes issued so far by this warpgroup
-    float acc[2][BN / 2];  // rows [0, 64) and [64, 128) of the tile
+    float acc[BN / 2];   // written by each item's first wgmma (scale-d = 0)
 
-    int j = 0;   // the item's place in the CTA's sequence
-    for (int item = first_item; item < num_items; item += item_stride, ++j) {
-      const WorkItem w = decode_item<BN, 1>(item, p, 0);
-      if ((j & 1) != cw) {   // the other warpgroup's item: its k-blocks pass through the ring before our next one
-        it += w.nkb;
-        continue;
-      }
-      // our turn on the tensor cores: the other warpgroup has issued the MMAs of the item before this one
-      if (j > 0) asm volatile("bar.sync %0, 256;" ::"r"(4 + cw) : "memory");
+    for (int item = first_item; item < num_items; item += item_stride) {
+      const WorkItem w = decode_item<BN>(item, p);
       for (int kb = 0; kb < w.nkb; ++kb, ++it) {
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[s], ph);
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) {
-          reg_fence(acc[0][i]);
-          reg_fence(acc[1][i]);
-        }
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
         wgmma_fence();
-        mma_kblock<BN, A_MN, B_MN>(acc[0], smem + s * C::STAGE_BYTES, 0, kb == 0);
-        mma_kblock<BN, A_MN, B_MN>(acc[1], smem + s * C::STAGE_BYTES, 1, kb == 0);
+        mma_kblock<BN, A_MN, B_MN>(acc, smem + s * C::STAGE_BYTES, cw, kb == 0);
         wgmma_commit();
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) {
-          reg_fence(acc[0][i]);
-          reg_fence(acc[1][i]);
-        }
+        for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
         if (kb > 0 && t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       }
-      // hand the tensor cores to the other warpgroup's next item (the one after this), if the CTA has one
-      if (item + item_stride < num_items) asm volatile("bar.arrive %0, 256;" ::"r"(5 - cw) : "memory");
       wgmma_wait<0>();
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) {
-        reg_fence(acc[0][i]);
-        reg_fence(acc[1][i]);
-      }
+      for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+      // the producer refills the stage with the next item's operands during the epilogue
       if (t == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
-      epilogue_slab<BN>(acc[0], w.m0, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
-      epilogue_slab<BN>(acc[1], w.m0 + 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
+      const int slice_row = ORD ? w.split * p.tiles_m * BM : 0;
+      epilogue_slab<BN>(acc, slice_row + w.m0 + cw * 64, w.n0, w.split == 0, p, &tmC, epi, boxes, 2 + cw, t);
     }
     if (t == 0 && p.tma_store) bulk_wait_all();   // the stores are complete before the CTA's shared memory goes away
   }
@@ -551,8 +421,8 @@ __device__ __forceinline__ void epilogue_slab_async(const float (&acc)[BN / 2], 
   }
 }
 
-// The cooperative kernel (CL = 1, no split) with epilogue_slab_async: both consumer warpgroups work on every item, 64
-// rows each, with the same produce / mma_kblock sequence, so its output bits are those of gemm_bf16_kernel<BN, 1, ...>.
+// The cooperative kernel (no split) with epilogue_slab_async: both consumer warpgroups work on every item, 64 rows
+// each, with the same produce / mma_kblock sequence, so its output bits are those of gemm_bf16_kernel<BN, ...>.
 template <int BN, bool F32, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_async_epi_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -588,8 +458,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) produce<BN, 1, A_MN, B_MN, STAGES>(smem, full_bar, empty_bar, &tmA, &tmB, p, 0, first_item,
-                                                             item_stride, num_items);
+    if (threadIdx.x == 0) produce<BN, A_MN, B_MN, STAGES>(smem, full_bar, empty_bar, &tmA, &tmB, p, first_item,
+                                                          item_stride, num_items);
   } else {
     setmaxnreg_inc<232>();
     const int cw = wg - 1;                 // rows [64 cw, 64 cw + 64) of the tile
@@ -599,7 +469,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     float acc[BN / 2];     // written by each item's first wgmma (scale-d = 0)
 
     for (int item = first_item; item < num_items; item += item_stride) {
-      const WorkItem w = decode_item<BN, 1>(item, p, 0);
+      const WorkItem w = decode_item<BN>(item, p);
       for (int kb = 0; kb < w.nkb; ++kb, ++it) {
         const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
@@ -624,61 +494,42 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   }
 }
 
-// PP: the ping-pong kernel (CL = 1), else the cooperative one; ORD: the cooperative one's ordered split-K form; AE = 1 /
-// 2: the asynchronous-epilogue kernel for a bf16 / fp32 TMA-stored output (CL = 1, one split)
-template <int BN, int CL, bool A_MN, bool B_MN, bool PP = false, bool ORD = false, int AE = 0>
+// ORD: the cooperative kernel's ordered split-K form; AE = 1 / 2: the asynchronous-epilogue kernel for a bf16 / fp32
+// TMA-stored output (one split)
+template <int BN, bool A_MN, bool B_MN, bool ORD = false, int AE = 0>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
                 cudaStream_t stream) {
-  static_assert(!PP || CL == 1, "the ping-pong kernel runs single CTAs");
-  static_assert(!ORD || (CL == 1 && !PP), "ordered split-K runs the single-CTA cooperative kernel");
-  static_assert(!AE || (CL == 1 && !PP && !ORD), "the asynchronous-epilogue kernel runs single CTAs");
+  static_assert(!AE || !ORD, "the asynchronous-epilogue kernel runs unsplit");
   constexpr int TOTAL = AE ? AsyncEpiCfg<BN, AE == 2>::TOTAL : GemmCfg<BN>::TOTAL;
   auto kern = [] {
     if constexpr (AE) return gemm_async_epi_kernel<BN, AE == 2, A_MN, B_MN>;
-    else if constexpr (PP) return gemm_bf16_pingpong_kernel<BN, A_MN, B_MN>;
-    else return gemm_bf16_kernel<BN, CL, A_MN, B_MN, ORD>;
+    else return gemm_bf16_kernel<BN, A_MN, B_MN, ORD>;
   }();
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = TOTAL;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  // CTAs (CL = 1) or clusters (CL = 2) of this kernel the device can hold at once
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  // CTAs of this kernel the device can hold at once: one per SM
   static int resident = 0;
   if (resident == 0) {
     MMAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL));
-    if constexpr (CL > 1) {
-      cfg.gridDim = dim3(CL);
-      MMAE_CUDA_OK(cudaOccupancyMaxActiveClusters(&resident, kern, &cfg));
-    } else {
-      int dev = 0, sms = 0;
-      MMAE_CUDA_OK(cudaGetDevice(&dev));
-      MMAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      resident = sms;
-    }
+    int dev = 0;
+    MMAE_CUDA_OK(cudaGetDevice(&dev));
+    MMAE_CUDA_OK(cudaDeviceGetAttribute(&resident, cudaDevAttrMultiProcessorCount, dev));
     MMAE_CHECK(resident > 0, MMAE_ERR_CUDA, "mmae_gemm_bf16: the GEMM kernel does not fit on an SM");
   }
   const int items = p.tiles_n * p.tiles_m * p.splits;
-  const int slots = std::min(resident, std::max(1, sm_count() / CL));
-  cfg.gridDim = dim3(std::min(items, slots) * CL);
+  const int slots = std::min(resident, std::max(1, sm_count()));
+  cfg.gridDim = dim3(std::min(items, slots));
   const bool prof = gemm_profile_begin(stream, 2.0 * p.M * p.N * p.K, p.M, p.N, p.K,
-                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (PP ? 4 : 0) | (ORD ? 8 : 0) | (AE ? 16 : 0) |
+                                       (A_MN ? 1 : 0) | (B_MN ? 2 : 0) | (ORD ? 8 : 0) | (AE ? 16 : 0) |
                                            (p.splits << 8));
-  if constexpr (CL == 1) {
-    cfg.attrs = attr + 1;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  } else {
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  }
   MMAE_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmC, p));
   if (prof) gemm_profile_end(stream);
   count_launch();
@@ -721,11 +572,14 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
 
 using namespace mmae;
 
+// -1 (the cost model) or a variant below
+static bool variant_valid(int v) { return v == -1 || (v >= 1 && v <= 3) || (v >= 8 && v <= 10); }
+
 // MMAE_GEMM_VARIANT / MMAE_GEMM_TMA_STORE set the initial values of the two switches below
 static int g_gemm_variant = []() {
   const char* e = getenv("MMAE_GEMM_VARIANT");
   const int v = e ? atoi(e) : -1;
-  return v >= -1 && v <= 10 ? v : -1;
+  return variant_valid(v) ? v : -1;
 }();
 static int g_gemm_tma_store = []() {
   const char* e = getenv("MMAE_GEMM_TMA_STORE");
@@ -733,7 +587,7 @@ static int g_gemm_tma_store = []() {
 }();
 
 extern "C" int mmae_gemm_set_variant(int variant) {
-  MMAE_CHECK(variant >= -1 && variant <= 10, MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1 .. 10)", variant);
+  MMAE_CHECK(variant_valid(variant), MMAE_ERR_ARG, "mmae_gemm_set_variant: %d (-1, 1, 2, 3, 8, 9 or 10)", variant);
   g_gemm_variant = variant;
   return MMAE_OK;
 }
@@ -743,13 +597,9 @@ extern "C" int mmae_gemm_set_tma_store(int enable) {
   return MMAE_OK;
 }
 
-// variant -> tile: 0 / 1 / 3 / 2 = one CTA, BN = 64 / 128 / 192 / 256; 6 / 5 / 4 = two-CTA cluster (256-row tile, B shared
-// by multicast), BN = 128 / 192 / 256; 7 = one CTA of ping-pong consumers, BN = 128; 8 / 9 / 10 = one CTA with the
-// asynchronous whole-slab epilogue, BN = 128 / 192 / 256 (a call it cannot take runs variant 1 / 3 / 2)
-static int variant_bn(int v) {
-  return v == 0 ? 64 : (v == 1 || v == 6 || v == 7 || v == 8) ? 128 : (v == 3 || v == 5 || v == 9) ? 192 : 256;
-}
-static int variant_cl(int v) { return v >= 4 && v <= 6 ? 2 : 1; }
+// variant -> tile: 1 / 3 / 2 = the cooperative kernel, BN = 128 / 192 / 256; 8 / 9 / 10 = the asynchronous whole-slab
+// epilogue, BN = 128 / 192 / 256 (a call it cannot take runs variant 1 / 3 / 2)
+static int variant_bn(int v) { return (v == 1 || v == 8) ? 128 : (v == 3 || v == 9) ? 192 : 256; }
 static bool variant_async(int v) { return v >= 8; }
 // the cooperative single-CTA variant of an asynchronous-epilogue variant's tile
 static int variant_coop(int v) { return v == 8 ? 1 : (v == 9 ? 3 : (v == 10 ? 2 : v)); }
@@ -763,12 +613,6 @@ static int variant_coop(int v) { return v == 8 ? 1 : (v == 9 ? 3 : (v == 10 ? 2 
 // (K = 256) and 10.3 (K = 768) k-block times of 0.353 us, 128 x 256 tiles 11.0 and 8.4 of 0.686 us.  (Measured while the
 // TMA epilogue still loaded the bias inside each staged box: see epilogue_slab.)
 constexpr int KB_PER_ITEM_FIXED = 4;
-// The ping-pong kernel (variant 7) hides part of that behind the other warpgroup's MMAs: measured as above, its 128 x 128
-// items cost 8.7 k-block times of 0.337 us past their own k-blocks at K = 256 and at K = 768 (4.29 and 6.99 us per item
-// against the cooperative 128 x 128 kernel's 4.77 and 7.87 us).  In the bench step (same card and limit) it ran the
-// decoders' bf16 forward GEMMs with N >= 768 at K = 256 4-5 % faster than the cooperative tiles, but the N = 256 and
-// dgrad (MN-major B) shapes 10-48 % slower, and the step as a whole slower than with the 128 x 192 tile alone; so the
-// model does not pick it, and variant 7 runs only when set.
 // The asynchronous-epilogue kernel (variants 8-10) leaves little of that: measured as the bf16 items above (N = 768, a
 // bias), 128 x 128 items cost 2.1 (K = 256) and 2.5 (K = 768) k-block times of 0.392 us, 128 x 192 3.6 and 5.1 of
 // 0.516 us, 128 x 256 2.8 and 1.5 of 0.752 us; fp32 128 x 128 items without a bias 2.1 and 5.6 of 0.349 us, against
@@ -801,7 +645,7 @@ int launch_ordered(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p,
   if (rc) return rc;
   const mmae_gemm_epilogue ep = p.ep;
   p.tma_store = 2;
-  const int lrc = launch_gemm<BN, 1, A_MN, B_MN, false, true>(tmA, tmB, tmC, p, st);
+  const int lrc = launch_gemm<BN, A_MN, B_MN, true>(tmA, tmB, tmC, p, st);
   if (lrc) return lrc;
   const int64_t total = int64_t(p.M) * (p.N / 4);
   const unsigned blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>((total + 255) / 256, int64_t(sm_count()) * 16));
@@ -834,10 +678,10 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
                         !ep->preact_bf16 && !ep->dgelu_z && (!ep->out_bf16 != !ep->out_f32);
   const bool async_f32 = ep->out_f32 != nullptr;
 
-  // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time (clusters:
-  // sm_count() / 2 items of 256 rows), so a launch lasts ceil(items / slots) rounds of one item, and an item costs
-  // ~(k-blocks + KB_PER_ITEM_FIXED) k-block times.  A k-block of a 128 x BN tile costs ~(BN + 40): the A tile's loads
-  // and MMA issue do not shrink with BN, which makes wide tiles the better choice whenever their rounds are as full.
+  // Tile width and split count from one model of the persistent grid: it runs sm_count() items at a time, so a launch
+  // lasts ceil(items / slots) rounds of one item, and an item costs ~(k-blocks + KB_PER_ITEM_FIXED) k-block times.  A
+  // k-block of a 128 x BN tile costs ~(BN + 40): the A tile's loads and MMA issue do not shrink with BN, which makes wide
+  // tiles the better choice whenever their rounds are as full.
   // 128 x 192 wins where its rounds are fuller: the encoder's N = 768 GEMMs make 99 x 4 = 396 tiles, exactly three
   // rounds of 132 SMs, against 297 of 128 x 256 in 2.25.  The automatic split (split_k <= 0) fills the last round of the
   // long-K weight gradients instead of leaving it mostly idle.  An explicit variant fixes the tile, an explicit split_k
@@ -861,10 +705,10 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     int best_split = 1, best_var = variant >= 0 ? variant : cand_var[0];
     for (int i = 0; i < nvar; ++i) {
       const int v = variant >= 0 ? variant : cand_var[i];
-      const int bn = variant_bn(v), cl = variant_cl(v);
+      const int bn = variant_bn(v);
       if (variant < 0 && bn > 128 && N < bn) continue;
-      const long tiles = long(ceil_div(tm, cl)) * ceil_div(N, bn);
-      const int slots = std::max(1, sms / cl);
+      const long tiles = long(tm) * ceil_div(N, bn);
+      const int slots = std::max(1, sms);
       const bool ae = variant_async(v) && async_ok;
       const int fixed = ae ? ASYNC_KB_PER_ITEM_FIXED : KB_PER_ITEM_FIXED;
       const int s_lo = split_k > 0 ? split_k : 1;
@@ -872,7 +716,7 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
       for (int s = s_lo; s <= s_hi; ++s) {
         const int kbps = ceil_div(num_kb, std::min(s, num_kb));
         const long rounds = (tiles * ceil_div(num_kb, kbps) + slots - 1) / slots;
-        const long cost = rounds * (bn + 40) * cl * (kbps + fixed);
+        const long cost = rounds * (bn + 40) * (kbps + fixed);
         if (best_cost < 0 || cost < best_cost) {
           best_cost = cost;
           best_split = s;
@@ -902,11 +746,7 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   // a call the asynchronous-epilogue kernel cannot take (split, or an fp32 output wider than 128 columns) runs the
   // cooperative kernel of the same width
   if (variant_async(variant) && (!async_ok || split_k > 1 || (async_f32 && variant != 8))) variant = variant_coop(variant);
-  // ordered split-K runs the cooperative single-CTA kernel of the same tile width
-  if (ordered) variant = (variant == 6 || variant == 7) ? 1 : (variant == 4 ? 2 : (variant == 5 ? 3 : variant));
-  if (variant == 5 && b_mn_major) variant = 4;   // an MN-major B half must be whole 64-column chunks
   const int BNsel = variant_bn(variant);
-  const int CLsel = variant_cl(variant);
 
   CUtensorMap tmA, tmB;
   int rc;
@@ -918,7 +758,7 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   }
   if (rc) return rc;
   if (!b_mn_major) {
-    rc = make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, BK, BNsel / CLsel);
+    rc = make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, BK, BNsel);
   } else {
     rc = make_tmap_2d_bf16(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 64, BK);
   }
@@ -929,7 +769,7 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
   p.num_kb = num_kb;
   p.kb_per_split = kb_per_split;
   p.tiles_n = ceil_div(N, BNsel);
-  p.tiles_m = ceil_div(tm, CLsel);
+  p.tiles_m = tm;
   p.splits = split_k;
   p.ep = *ep;
   // plain bf16 / fp32 outputs (optionally with bias / GELU) leave through shared memory and TMA tile stores; fp32
@@ -961,41 +801,24 @@ extern "C" int mmae_gemm_bf16(const void* A, int64_t lda, int a_mn_major, const 
     if (a_mn_major && !b_mn_major) return launch_ordered<BN_, true, false>(tmA, tmB, p, st);    \
     return launch_ordered<BN_, true, true>(tmA, tmB, p, st);                                    \
   } while (0)
-    if (BNsel == 64) MMAE_DISPATCH_ORD(64);
     if (BNsel == 192) MMAE_DISPATCH_ORD(192);
     if (BNsel == 256) MMAE_DISPATCH_ORD(256);
     MMAE_DISPATCH_ORD(128);
 #undef MMAE_DISPATCH_ORD
   }
-#define MMAE_DISPATCH(BN_, CL_, PP_)                                                                      \
-  do {                                                                                                    \
-    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, false, false, PP_>(tmA, tmB, tmC, p, st); \
-    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, CL_, false, true, PP_>(tmA, tmB, tmC, p, st);   \
-    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, CL_, true, false, PP_>(tmA, tmB, tmC, p, st);   \
-    return launch_gemm<BN_, CL_, true, true, PP_>(tmA, tmB, tmC, p, st);                                  \
+#define MMAE_DISPATCH(BN_, AE_)                                                                       \
+  do {                                                                                                \
+    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, false, false, false, AE_>(tmA, tmB, tmC, p, st); \
+    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, false, true, false, AE_>(tmA, tmB, tmC, p, st);   \
+    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, true, false, false, AE_>(tmA, tmB, tmC, p, st);   \
+    return launch_gemm<BN_, true, true, false, AE_>(tmA, tmB, tmC, p, st);                                  \
   } while (0)
-  if (variant == 4) MMAE_DISPATCH(256, 2, false);
-  if (variant == 6) MMAE_DISPATCH(128, 2, false);
-  if (variant == 5) {
-    if (!a_mn_major) return launch_gemm<192, 2, false, false>(tmA, tmB, tmC, p, st);
-    return launch_gemm<192, 2, true, false>(tmA, tmB, tmC, p, st);
-  }
-#define MMAE_DISPATCH_AE(BN_, AE_)                                                                                \
-  do {                                                                                                            \
-    if (!a_mn_major && !b_mn_major) return launch_gemm<BN_, 1, false, false, false, false, AE_>(tmA, tmB, tmC, p, st); \
-    if (!a_mn_major && b_mn_major) return launch_gemm<BN_, 1, false, true, false, false, AE_>(tmA, tmB, tmC, p, st);   \
-    if (a_mn_major && !b_mn_major) return launch_gemm<BN_, 1, true, false, false, false, AE_>(tmA, tmB, tmC, p, st);   \
-    return launch_gemm<BN_, 1, true, true, false, false, AE_>(tmA, tmB, tmC, p, st);                                  \
-  } while (0)
-  if (variant == 8 && p.tma_store == 2) MMAE_DISPATCH_AE(128, 2);
-  if (variant == 8) MMAE_DISPATCH_AE(128, 1);
-  if (variant == 9) MMAE_DISPATCH_AE(192, 1);
-  if (variant == 10) MMAE_DISPATCH_AE(256, 1);
-#undef MMAE_DISPATCH_AE
-  if (variant == 0) MMAE_DISPATCH(64, 1, false);
-  if (variant == 3) MMAE_DISPATCH(192, 1, false);
-  if (variant == 2) MMAE_DISPATCH(256, 1, false);
-  if (variant == 7) MMAE_DISPATCH(128, 1, true);
-  MMAE_DISPATCH(128, 1, false);
+  if (variant == 8 && p.tma_store == 2) MMAE_DISPATCH(128, 2);
+  if (variant == 8) MMAE_DISPATCH(128, 1);
+  if (variant == 9) MMAE_DISPATCH(192, 1);
+  if (variant == 10) MMAE_DISPATCH(256, 1);
+  if (variant == 3) MMAE_DISPATCH(192, 0);
+  if (variant == 2) MMAE_DISPATCH(256, 0);
+  MMAE_DISPATCH(128, 0);
 #undef MMAE_DISPATCH
 }

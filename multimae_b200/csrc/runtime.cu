@@ -303,7 +303,7 @@ extern "C" int mmae_profile_gemm_read(double* flops, double* ms, int64_t* launch
   return MMAE_OK;
 }
 
-// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bit2 ping-pong, bit3 ordered split-K, bit4
+// one line per recorded launch: "M N K flags ms" (flags: bit0 a_mn, bit1 b_mn, bit2 unused, bit3 ordered split-K, bit4
 // asynchronous epilogue, bits 8.. split_k); returns
 // bytes written
 extern "C" int64_t mmae_profile_gemm_dump(char* buf, int64_t cap) {

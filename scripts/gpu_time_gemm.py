@@ -2,7 +2,7 @@
 
     python scripts/gpu_time_gemm.py               # every distinct GEMM shape / operand-major combination of the step
     python scripts/gpu_time_gemm.py --fixed-cost  # per-tile fixed cost: intercept of time over k-blocks
-    python scripts/gpu_time_gemm.py --variant 7   # the step's shapes on one tile variant (mmae_gemm_set_variant)
+    python scripts/gpu_time_gemm.py --variant 8   # the step's shapes on one tile variant (mmae_gemm_set_variant)
     python scripts/gpu_time_gemm.py --variant 3 9 # ... on several, side by side (wgrad shapes included)
 
 Shapes: encoder M = 128 x 99 tokens (D 768, MLP 3072), decoders M = 128 x 196 query tokens and 128 x 99 context tokens
@@ -51,8 +51,8 @@ SHAPES = [
     ("dec", "context proj wgrad", 1024, 768, DC, "wgrad"),
 ]
 PEAK_TFLOPS = 989.0
-# variants timed by --fixed-cost (7: ping-pong, 8 / 9 / 10: asynchronous epilogue): their output tile width
-VARIANT_BN = {1: 128, 3: 192, 2: 256, 7: 128, 8: 128, 9: 192, 10: 256}
+# variants timed by --fixed-cost (8 / 9 / 10: asynchronous epilogue): their output tile width
+VARIANT_BN = {1: 128, 3: 192, 2: 256, 8: 128, 9: 192, 10: 256}
 F32_VARIANTS = (1, 8)
 
 

@@ -1,11 +1,11 @@
 """GPU: the persistent wgmma GEMM's work-item schedule and the SM-count-sized reduction kernels under reduced SM budgets,
 against float64.
 
-The GEMM grid holds at most one CTA (or two-CTA cluster) per SM of the budget (mmae_set_sm_budget), and each walks a
-strided sequence of work items (n-tile fastest, then m-tile, then split) with a TMA ring whose slot and phase run across
-items.  The budget also sets the tile / split choice, the row blocking of the column-sum kernels and of their last-block
-fold, and the LayerNorm backward grid.  Budget 1 puts every item (every row block) on one CTA; budgets 3, 7 and 17 are odd,
-so that sms / 2 truncates for the cluster variants.
+The GEMM grid holds at most one CTA per SM of the budget (mmae_set_sm_budget), and each walks a strided sequence of work
+items (n-tile fastest, then m-tile, then split) with a TMA ring whose slot and phase run across items.  The budget also
+sets the tile / split choice, the row blocking of the column-sum kernels and of their last-block fold, and the LayerNorm
+backward grid.  Budget 1 puts every item (every row block) on one CTA; budgets 3, 7 and 17 are odd, so that the last round
+of items (of row blocks) leaves part of the grid idle.
 
 Error budgets, against a float64 reference of the same bf16 operands:
   * whole matrix, relative L2: fp32 outputs 3e-5 (fp32 accumulation order only), bf16 outputs 4e-3 (the suite's budgets);
@@ -34,7 +34,7 @@ FULL = 0                 # budget 0: every SM
 MAJORS = [(False, False), (False, True), (True, False), (True, True)]
 
 # variant -> (tile width BN, TMA ring stages), gemm_wgmma.cu variant_bn / GemmCfg
-VARIANT_TILE = {0: (64, 8), 1: (128, 6), 2: (256, 4), 3: (192, 4), 4: (256, 4), 5: (192, 4), 6: (128, 6)}
+VARIANT_TILE = {1: (128, 6), 2: (256, 4), 3: (192, 4)}
 
 
 @pytest.fixture(scope="module")
@@ -214,7 +214,7 @@ def KN():
     return kernels
 
 
-# Small shapes for the variant x epilogue x budget product; at budget 1 one CTA (cluster) runs all of their items
+# Small shapes for the variant x epilogue x budget product; at budget 1 one CTA runs all of their items
 SMALL = [pytest.param((40, 776, 200), id="M<64-partial_box-raggedK"),
          pytest.param((648, 136, 320), id="odd_128row_tiles-N%BN-5kb"),
          pytest.param((1000, 1024, 64), id="1kb_per_item-many_items")]
@@ -222,7 +222,7 @@ SMALL = [pytest.param((40, 776, 200), id="M<64-partial_box-raggedK"),
 
 @pytest.mark.parametrize("shape", SMALL)
 @pytest.mark.parametrize("budget", [FULL, 1])
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 def test_epilogues_every_variant(dev, knobs, KN, variant, budget, shape):
     """Every epilogue kind, through the TMA-store and the register paths, at every explicit tile variant."""
     worst = Worst()
@@ -234,7 +234,7 @@ def test_epilogues_every_variant(dev, knobs, KN, variant, budget, shape):
 
 
 @pytest.mark.parametrize("budget", [FULL, 1])
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 def test_ring_depth_every_variant(dev, knobs, KN, variant, budget):
     """Items of STAGES - 1, STAGES and STAGES + 1 k-blocks of the variant's ring: with fewer k-blocks than stages the
     producer runs whole items ahead of the consumers, and the ring's slot / phase wrap inside or between items."""
@@ -277,7 +277,7 @@ def test_shape_table_heuristic(dev, knobs, KN, shape, budget):
     worst.report("shape %s budget %d" % (shape, budget))
 
 
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 def test_bitwise_same_across_budgets_and_launches(dev, knobs, KN, variant):
     """With a fixed tile and split_k = 1 one CTA sums each tile in a fixed k order: the output bits may not depend on the
     SM budget (grid size, items per CTA) or on the launch."""

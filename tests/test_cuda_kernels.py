@@ -35,12 +35,12 @@ def KN():
     L.lib().mmae_set_sm_budget(int(os.environ.get("MMAE_SM_BUDGET", 0)))
 
 
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 @pytest.mark.parametrize("shape", [(128, 128, 64), (256, 384, 768), (200, 136, 200), (396, 2128, 256), (1000, 768, 512),
                                    (2560, 2304, 768)])
 def test_gemm_all_operand_majors(dev, KN, variant, shape):
     from multimae_b200 import _lib as L
-    L.lib().mmae_gemm_set_variant(variant)
+    L.check(L.lib().mmae_gemm_set_variant(variant))
     M, N, K = shape
     A, B = _bf16(dev, M, K), _bf16(dev, N, K)
     ref = A.float() @ B.float().t()
@@ -53,10 +53,10 @@ def test_gemm_all_operand_majors(dev, KN, variant, shape):
             assert rel_l2(out, ref) < 3e-5, (variant, shape, a_mn, b_mn, rel_l2(out, ref))
 
 
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6, -1])
+@pytest.mark.parametrize("variant", [1, 2, 3, -1])
 def test_gemm_split_k_wgrad_shapes(dev, KN, variant):
     from multimae_b200 import _lib as L
-    L.lib().mmae_gemm_set_variant(variant)
+    L.check(L.lib().mmae_gemm_set_variant(variant))
     for (M, N, K, split) in [(768, 768, 12672, 1), (768, 768, 12672, 4), (768, 3072, 1280, 3), (256, 256, 25088, 16),
                              (256, 256, 25088, 0), (2304, 768, 12672, 0)]:          # 0 = automatic split + tile choice
         A, B = _bf16(dev, M, K), _bf16(dev, N, K)
@@ -65,10 +65,10 @@ def test_gemm_split_k_wgrad_shapes(dev, KN, variant):
         assert rel_l2(out, A.float() @ B.float().t()) < 3e-5
 
 
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 def test_gemm_fused_epilogues(dev, KN, variant):
     from multimae_b200 import _lib as L
-    L.lib().mmae_gemm_set_variant(variant)
+    L.check(L.lib().mmae_gemm_set_variant(variant))
     M, N, K = 384, 512, 256
     A, B = _bf16(dev, M, K), _bf16(dev, N, K)
     bias, resid = torch.randn(N, device=dev), torch.randn(M, N, device=dev)
@@ -92,16 +92,16 @@ def test_gemm_fused_epilogues(dev, KN, variant):
     assert rel_l2(out, 1 + 0.5 * acc) < 3e-5
 
 
-@pytest.mark.parametrize("variant", [1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [1, 2, 3])
 @pytest.mark.parametrize("shape", [(128, 128, 64), (200, 136, 200), (396, 2128, 256), (1000, 776, 512), (2560, 2304, 768),
                                    (25088, 256, 256)])
 def test_gemm_tma_store_epilogue(dev, KN, variant, shape):
     """bf16 outputs through shared memory + TMA tile stores: ragged M / N edges, a strided output view, bias and GELU;
     bit-identical to the per-thread store path and untouched bytes outside the [M, N] view.  Both paths also run with an
-    SM budget of 1 (one CTA or cluster walks every tile, reusing its staging boxes across tiles) and must give the same
+    SM budget of 1 (one CTA walks every tile, reusing its staging boxes across tiles) and must give the same
     bits as with every SM."""
     from multimae_b200 import _lib as L
-    L.lib().mmae_gemm_set_variant(variant)
+    L.check(L.lib().mmae_gemm_set_variant(variant))
     M, N, K = shape
     A, B = _bf16(dev, M, K), _bf16(dev, N, K)
     bias = torch.randn(N, device=dev)
@@ -138,16 +138,16 @@ def test_gemm_tma_store_epilogue(dev, KN, variant, shape):
                 assert torch.equal(outs[0], o), (variant, shape, list(kw))
 
 
-def test_gemm_heuristic_picks_pair_kernels_correctly(dev, KN):
-    """On the big encoder shapes the heuristic's choice, a single-CTA 128 x 192 tile and the two-CTA cluster (pair) kernels
-    give the same results."""
+def test_gemm_heuristic_agrees_with_every_tile(dev, KN):
+    """On the big encoder shapes the heuristic's choice and the 128 x 128, 128 x 256 and 128 x 192 tiles give the same
+    results."""
     from multimae_b200 import _lib as L
     for (M, N, K, b_mn) in [(12672, 3072, 768, False), (12672, 3072, 768, True), (12672, 768, 3072, False)]:
         A, B = _bf16(dev, M, K), _bf16(dev, N, K)
         bias = torch.randn(N, device=dev)
         outs = []
-        for variant in (-1, 3, 4, 6):
-            L.lib().mmae_gemm_set_variant(variant)
+        for variant in (-1, 1, 2, 3):
+            L.check(L.lib().mmae_gemm_set_variant(variant))
             o = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
             KN.gemm(A, B.t().contiguous() if b_mn else B, b_mn=b_mn, bias=bias, out_bf16=o)
             outs.append(o)

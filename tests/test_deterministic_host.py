@@ -184,17 +184,17 @@ def _sass_functions(cubin):
 
 
 def _gemm_key(name):
-    """'gemm_bf16_kernel<128, 1, false, false>' for the kernels that run with deterministic mode off (the ordered
+    """'gemm_bf16_kernel<128, false, false>' for the kernels that run with deterministic mode off (the ordered
     split-K form, ORD = true, is new); None for anything else."""
-    m = re.search(r"(gemm_bf16_kernel|gemm_bf16_pingpong_kernel)<([^>]*)>", name)
+    m = re.search(r"gemm_bf16_kernel<([^>]*)>", name)
     if not m:
         return None
-    args = [a.strip() for a in m.group(2).split(",")]
-    if m.group(1) == "gemm_bf16_kernel" and len(args) == 5:
-        if args[4] != "false":
+    args = [a.strip() for a in m.group(1).split(",")]
+    if len(args) == 4:
+        if args[3] != "false":
             return None
-        args = args[:4]
-    return "%s<%s>" % (m.group(1), ", ".join(args))
+        args = args[:3]
+    return "gemm_bf16_kernel<%s>" % ", ".join(args)
 
 
 def _sass_digests(cubin):
@@ -238,7 +238,7 @@ def test_new_kernels_have_no_spills(cubins):
                 assert (st, ld) == (0, 0), (d, st, ld)
                 checked.append(d)
     assert sum("splitk_reduce_kernel" in d for d in checked) == 1
-    assert sum("gemm_bf16_kernel" in d for d in checked) == 16     # 4 tile widths x 4 operand layouts
+    assert sum("gemm_bf16_kernel" in d for d in checked) == 12     # 3 tile widths x 4 operand layouts
     assert sum("semseg_emb_bwd_det_kernel" in d for d in checked) == 1
 
 
@@ -246,6 +246,6 @@ def test_existing_gemm_kernels_compile_to_the_same_sass(cubins):
     golden = json.load(open(GOLDEN))
     now = _sass_digests(cubins["gemm_wgmma.cu"][0])
     assert set(now) == set(golden)
-    assert len(golden) >= 20
+    assert len(golden) == 12
     changed = sorted(k for k in golden if now[k] != golden[k])
     assert not changed, changed

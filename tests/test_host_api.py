@@ -178,6 +178,9 @@ def test_c_abi_rejects_bad_arguments_and_dropout_with_messages():
         (lambda: lib.mmae_standardize_depth(None, None, 1, 16, 1, 9, 1e-6, None, None), ARG, b"bad args"),
         (lambda: lib.mmae_standardize_depth(16, 16, 1, 16, 9, 9, 1e-6, None, None), ARG, b"lo < hi"),
         (lambda: lib.mmae_standardize_depth_set_variant(3), ARG, b"1 or 2"),
+        (lambda: lib.mmae_gemm_set_variant(0), ARG, b"mmae_gemm_set_variant: 0 (-1, 1, 2, 3, 8, 9 or 10)"),
+        (lambda: lib.mmae_gemm_set_variant(7), ARG, b"mmae_gemm_set_variant: 7 (-1, 1, 2, 3, 8, 9 or 10)"),
+        (lambda: lib.mmae_gemm_set_variant(11), ARG, b"mmae_gemm_set_variant: 11 (-1, 1, 2, 3, 8, 9 or 10)"),
         (lambda: lib.mmae_layernorm_forward(16, 100, 16, 16, 16, 100, None, 0, 16, 16, 4, 100, 1e-6, None), UNSUPPORTED,
          b"multiple of 128"),
         (lambda: lib.mmae_attention_forward(16, 64, 16, 64, 16, 64, 16, 64, None, 1, 1, 8, 8, 48, 0.1, 0.0, None, None),
